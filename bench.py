@@ -8,7 +8,7 @@ lineitem, the metric BASELINE.json names: rows/s + achieved HBM GB/s, next to th
 
 A step = one pass of Q1 over this rank's lineitem shard.  Weak scaling: every rank holds its own
 SF-`sf` shard (600 037 902 rows at SF-100, 22.8 GB of Q1 columns resident in HBM); the only data-path
-collective is one all-reduce of the 6x5 partial-state matrix.  Inputs are 180x larger than L2, so no
+collective is one all-reduce of the 6x5 partial-state matrix.  Inputs are 450x larger than H100's L2, so no
 explicit L2 flush is needed between steps.  One JSON line on stdout (rank 0).
 """
 from __future__ import annotations
@@ -32,30 +32,14 @@ Q1_AGGS = ["l_quantity", "l_extendedprice", "l_extendedprice * (1 - l_discount)"
 METRIC = "tpch_q1_rows_per_s"
 
 
-def profiled_traffic_bytes():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed
-    `ncu --set full` capture (profiles/r01_q1_fused_tma.txt); None when the summary is not there."""
-    import re
-    p = os.path.join(ROOT, "profiles", "r01_q1_fused_tma.txt")
-    try:
-        m = re.search(r"DRAM traffic ([0-9.]+) GB", open(p).read())
-        return float(m.group(1)) * 1e9 if m else None
-    except OSError:
-        return None
-
-
-def measured_peak_gbs():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+def hbm_peak_gbs():
+    return 3350.0, "data sheet (NVIDIA H100 SXM, HBM3 3.35 TB/s; not a measured figure)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
+    """nvidia-smi clocks / throttle reasons / power limit sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index: int = 0):
         self.samples, self.proc, self.index = [], None, index
@@ -78,10 +62,10 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
-        sm, mx, reasons = [], None, set()
+        sm, mx, power_w, reasons = [], None, None, set()
         for s in self.samples:
             f = [x.strip() for x in s.split(",")]
-            if len(f) < 6:
+            if len(f) < 7:
                 continue
             try:
                 sm.append(float(f[0])); mx = float(f[1])
@@ -90,8 +74,12 @@ class ClockSampler:
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[2:6]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
+            try:
+                power_w = float(f[6])
+            except ValueError:
+                pass
         sm.sort()
-        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons),
+        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "power_limit_w": power_w, "reasons": sorted(reasons),
                 "samples": len(sm)}
 
 
@@ -150,7 +138,7 @@ def run_reference(args):
 def bind_to_gpu_numa_node(local: int):
     """Pin this rank's host threads to the CPUs of its GPU's NUMA node BEFORE any pinned buffer is allocated (first touch puts
     the pages there): at 8 ranks the end-to-end leg moves 8 x 55 GB/s out of host memory, and buffers on the wrong socket cross
-    the inter-socket link (round 1: 538 ms per step at 8 GPUs against 413 ms at <= 4).  Best effort; returns what it did."""
+    the inter-socket link.  Best effort; returns what it did."""
     try:
         import pynvml
         pynvml.nvmlInit()
@@ -183,9 +171,7 @@ def run_ours(args):
     local = int(os.environ.get("LOCAL_RANK", "0"))
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
-    if world > 1:
-        # 3 channels x 6 GiB of mailbox per rank (of 180 GB): the 17 GB-per-rank as-of shuffle goes in 6 rounds instead of 18
-        os.environ.setdefault("QK_MAILBOX_MB", "6144")
+    gpu_name = torch.cuda.get_device_name(dev)
     numa = bind_to_gpu_numa_node(local) if world > 1 else {"numa_node": None, "why": "single rank: all host cores stay available"}
     if world > 1:
         import datetime
@@ -271,6 +257,8 @@ def run_ours(args):
             dist.all_reduce(state.acc); dist.all_reduce(state.cnt)
     t_end.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"q1_acc": state.acc, "q1_cnt": state.cnt})
     total_ms = t_start.elapsed_time(t_end)
     kern_ms = sum(a.elapsed_time(b) for a, b in kev) / args.steps
     launches = ops.launch_count() - launches0
@@ -415,7 +403,7 @@ def run_ours(args):
         cpu = info
 
     if rank == 0:
-        peak, peak_src = measured_peak_gbs()
+        peak, peak_src = hbm_peak_gbs()
         ach = n_total * Q1_BYTES_PER_ROW / (kern_ms / 1e3) / 1e9
         line = {
             "metric": METRIC, "value": value, "unit": "rows/s", "n_gpus": world, "steps": args.steps,
@@ -426,9 +414,9 @@ def run_ours(args):
                        "l2": "inputs (22.8 GB) are larger than L2; no flush needed", "parallelism": f"shard x{world}, 1 all-reduce of 6x5 partials"},
             "gb_per_s": value * Q1_BYTES_PER_ROW / 1e9,
             "roofline": {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                         "traffic": profiled_traffic_bytes() if (sf == 100 and "fused_tma:q1" in variant_name) else None,
-                         "traffic_source": "profiles/r01_q1_fused_tma.txt (ncu --set full, same kernel and size)", "kernel": variant_name, "kernel_ms": kern_ms, "peak_source": peak_src,
+                         "kernel": variant_name, "kernel_ms": kern_ms, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": n_total * Q1_BYTES_PER_ROW},
+            "gpu": gpu_name,
             "cpu_baseline": cpu, "e2e": e2e, "q6": q6, "q3": q3, "q5": extras.get("q5"), "asof": extras.get("asof"),
             "e2e_parquet": extras.get("e2e_parquet"),
             "gpu_launches": launches, "clocks": clocks, "host_binding": numa,
@@ -438,6 +426,16 @@ def run_ours(args):
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes what the timed path returned in its last step as `out_dir/<name>.npy` (float64), so that two builds can be
+    compared output for output on identical inputs.  Q1's state is [groups, aggregates] sums and per-group counts: a few
+    hundred bytes."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().cpu().numpy().astype(np.float64))
 
 
 def run_q3(args, torch, dev, world, rank, weak=False):
@@ -518,7 +516,7 @@ def run_q3(args, torch, dev, world, rank, weak=False):
             "scan_gb_per_s": scan_bytes / dt / 1e9, "scan_bytes": scan_bytes,
             "roofline": _roofline(scan_bytes / max(world, 1), dt, "Q3 scan bytes per GPU (28 B/lineitem row + 24 B/orders row + 9 B/customer row, SURVEY 8d) over the WHOLE query's wall time"),
             "shuffle_bytes_over_nvlink": float(sent.item()), "shuffle_gb_per_s_per_gpu": float(sent.item()) / max(world, 1) / dt / 1e9,
-            "shuffle_frac_of_nvlink_900": float(sent.item()) / max(world, 1) / dt / 1e9 / 900.0,
+            "shuffle_frac_of_nvlink_450": float(sent.item()) / max(world, 1) / dt / 1e9 / 450.0,    # H100 NVLink 4, per direction
             "exchanges": g.exchange.calls, "exchanges_via_peer_memory": g.exchange.peer_calls, "lanes": g.lanes_used, "chunk_rows": args.chunk_rows,
             "profile_ms": g.report() if g.profile else None,
             "top1": {k: (res[k][0].as_py() if res.num_rows else None) for k in res.column_names} if res is not None else None}
@@ -533,7 +531,7 @@ def _last_graph_report():
 
 
 def _roofline(bytes_per_gpu, seconds, what):
-    peak, src = measured_peak_gbs()
+    peak, src = hbm_peak_gbs()
     ach = bytes_per_gpu / seconds / 1e9
     return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "algorithmic_bytes_per_gpu": bytes_per_gpu,
             "peak_source": src, "what": what}
@@ -761,6 +759,8 @@ def main():
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's Q1 result (group sums, group counts) as DIR/<name>.npy")
     ap.add_argument("--sf", type=float, default=100)
     ap.add_argument("--variant", type=int, default=0, help="0 auto, 1 generic, 2 fused LDG, 3 fused TMA")
     ap.add_argument("--cpu-rows", type=int, default=120_000_000)
@@ -781,7 +781,8 @@ def main():
                     help="1: also time Q5 and the as-of join when running on one GPU; 2: at any GPU count; 0: never")
     ap.add_argument("--asof-quotes", type=int, default=1_050_000_000,
                     help="quote rows per GPU in the as-of extra (+ a fifth as many trades): 8 GPUs x 1.26 B = 10 B rows, BASELINE config 5")
-    ap.add_argument("--q5-sf", type=float, default=300, help="scale factor of the Q5 extra (BASELINE config 4: SF-300), strong scaling")
+    ap.add_argument("--q5-sf", type=float, default=100,
+                    help="scale factor of the Q5 extra, strong scaling (SF-100: 22.5 GB of scan columns, with room for the joins in 80 GB)")
     ap.add_argument("--no-parquet", action="store_true", help="skip the Parquet end-to-end leg of the default line (1 GPU only)")
     ap.add_argument("--q3-sf", type=float, default=100)
     ap.add_argument("--q3-steps", type=int, default=3)

@@ -1,4 +1,4 @@
-/* qk.h -- C-ABI of libqk.so: the sm_100a kernels behind Quokka's operator protocols.
+/* qk.h -- C-ABI of libqk.so: the sm_90a kernels behind Quokka's operator protocols.
  *
  * The reference (marsupialtail/quokka @ 1caf62e) has NO FFI on this path: its operators are Python
  * classes that delegate to Polars / DuckDB / Arrow.  Each entry point below replaces one of those

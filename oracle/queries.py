@@ -1,6 +1,6 @@
 """The judged queries restated on the numpy oracle (TEST INFRASTRUCTURE -- see oracle/__init__.py).
 
-Query text: /root/reference/apps/tpc-h/tpch.py:106-120 (Q1), :168-175 (Q3), :223-236 (Q5),
+Query text: the reference's apps/tpc-h/tpch.py:106-120 (Q1), :168-175 (Q3), :223-236 (Q5),
 cross-checked with the canonical SQL in apps/tpc-h/tpch_ref.py:15-38, :89-115, :142-169;
 as-of: apps/tpc-h/range.py:10-16.  Inputs are numpy column dicts (oracle/tpch_gen.py); string
 columns are dictionary codes and the literals are resolved to codes here, as the product does.

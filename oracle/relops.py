@@ -1,5 +1,5 @@
 """numpy restatement of the reference's relational operators on the hot path.
-TEST INFRASTRUCTURE -- see oracle/__init__.py.  All reference paths are under /root/reference.
+TEST INFRASTRUCTURE -- see oracle/__init__.py.  Reference paths are relative to a checkout of the reference.
 
 Each function cites the reference code whose observable behaviour it restates.  The reference
 delegates the arithmetic to Polars / DuckDB / Arrow (absent here); what is restated is the

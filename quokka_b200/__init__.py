@@ -1,7 +1,7 @@
-"""quokka_b200 -- B200-native execution backend for Quokka's columnar hot path.
+"""quokka_b200 -- H100-native execution backend for Quokka's columnar hot path.
 
 Python mirrors the reference's operator protocols (Executor / input reader / partitioner,
-QuokkaContext / DataStream); the work is done by hand-written sm_100a kernels in libqk.so
+QuokkaContext / DataStream); the work is done by hand-written sm_90a kernels in libqk.so
 (include/qk.h).  There is no CPU fallback.
 
     from quokka_b200 import QuokkaContext

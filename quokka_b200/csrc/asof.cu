@@ -62,7 +62,7 @@ __global__ void __launch_bounds__(256) k_asof_search(const long long* l_time, co
 //                           newest row of the window comes AFTER this left row, ~1 % of left rows) the warp scans the
 //                           window's keys backwards from `lim`, 128 at a time, for an earlier one
 // The first version of this sweep gave every WARP a chunk and a private table: 6 warps per SM, 12 shuffles of binary search
-// and a serial loop over the left rows per 32-row step -- latency-bound at 250 GB/s (profiles/r02_launches_asof_end.txt).
+// and a serial loop over the left rows per 32-row step -- latency-bound.
 // No sort, no scatter: reads 12 B per right row + 4 B again in step 2, 12 B per left row, writes 4 B per left row.
 // Row numbers in the table are the caller's (local row + r_base); carry_in must hold rows below r_base (older rows).
 constexpr int AS_NT = 256, AS_K = 4, AS_W = AS_NT * AS_K;

@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for libqk.so (sm_100a only).
+// common.cuh -- shared host/device helpers for libqk.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -89,7 +89,7 @@ __device__ __forceinline__ bool cmp_i64(int64_t a, int cmp, int64_t b) {
         default: return a != b;
     }
 }
-// L2 residency hints (B200: 126 MB L2 shared by streams and small hot structures).  A table that is probed at random
+// L2 residency hints (H100: 50 MB L2 shared by streams and small hot structures).  A table that is probed at random
 // while column streams many times its size pass through the same L2 -- a Bloom filter, a hash table -- is loaded with
 // evict_last; the streams are loaded with evict_first (and bypass L1), so they do not push the table out.
 __device__ __forceinline__ unsigned long long l2_policy_evict_first() {

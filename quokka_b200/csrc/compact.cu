@@ -45,7 +45,7 @@ struct CompactArgs {
 // Blocked Bloom filter, one 64-bit word per key: the key picks a 32-byte block (a DRAM sector) of its partition's filter, one of
 // the block's four 64-bit words and three bits inside that word, so a test is ONE 8-byte load + one mask compare.  The hash is
 // two rounds of 32-bit multiply-xorshift (the mask kernel is instruction-bound: a 64-bit mix + three 4-byte probes cost
-// ~170 instructions per row, profiles/r02_q3_compact_mask_before.txt).
+// ~170 instructions per row).
 __device__ __forceinline__ void bloom_slots(long long key, long long words_per_part, int nparts, long long* word64, unsigned long long* mask) {
     const unsigned p = part_mod(key, (unsigned)nparts);
     unsigned h = ((unsigned)key ^ ((unsigned)((unsigned long long)key >> 32) * 0x9E3779B1u)) * 0x85EBCA6Bu;

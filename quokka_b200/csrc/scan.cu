@@ -793,7 +793,7 @@ int launch_fused(const FusedArgs& F, const DenseArgs& A, int64_t nrows, int vari
     // variant 3 = default TMA configuration; 4..6 = alternative (threads, rows/thread, stages) shapes kept
     // selectable for profiling
     switch (variant) {
-        case 3: {   // measured best on B200 (SF-100 Q1: 3.31 ms, 6.9 TB/s): 256 threads x 4 rows, 3 stages
+        case 3: {   // default shape: 256 threads x 4 rows, 3 stages
             int rc = launch_tma<Plan, 256, 4, 3>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
             if (rc == 1) rc = launch_tma<Plan, 256, 2, 3>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
             if (rc == 1) rc = launch_tma<Plan, 256, 1, 3>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
@@ -981,8 +981,7 @@ __device__ __forceinline__ void dy_rows(const DyArgs& D, const DenseArgs& A, con
 // ---- the typed tile walk (FAST plans: int32 range terms, fp64 compare terms and factors, uint8 sets and group keys)
 // A descriptor (term / factor / key) is decoded ONCE per tile into registers and then applied to the thread's V rows, with
 // 32-bit shared-memory addresses: the first version decoded per row through generic pointers and spent ~290 instructions per
-// row, 2/3 of them IMAD / LDC / ISETP / BRA of the walk itself (profiles/r02_dyn_plan_q6_occupancy.txt) -- it was bound by
-// issue slots at 0.34 of the HBM roofline.
+// row, 2/3 of them IMAD / LDC / ISETP / BRA of the walk itself -- it was bound by issue slots.
 __device__ __forceinline__ int lds_i32(unsigned a) { int v; asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(a)); return v; }
 __device__ __forceinline__ unsigned lds_u8(unsigned a) { unsigned v; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a)); return v; }
 __device__ __forceinline__ long long lds_i64(unsigned a) { long long v; asm volatile("ld.shared.s64 %0, [%1];" : "=l"(v) : "r"(a)); return v; }
@@ -1384,7 +1383,7 @@ static int launch_dyn_v(DyArgs& D, const DenseArgs& A, int64_t nrows, double* pa
     for (int j = 0; j < A.nagg && fast; ++j)
         for (int f = 0; f < D.agg[j].nfact && fast; ++f) if (D.agg[j].f[f].col >= 0) fast = D.dtype[D.agg[j].f[f].col] == QK_F64;
     // persistent grid: as many CTAs per SM as the plan's shared memory allows -- with one CTA per SM the kernel is bound by
-    // shared-memory latency (ncu: 12.5 % warps active, 27 % issue slots; profiles/r02_dyn_plan_q6_one_cta.txt)
+    // shared-memory latency (few warps active)
     const int sms = sm_count(), per_sm = dyn_ctas_per_sm(D, A, NT, V);
     const int64_t nfull = nrows / TILE, want = (int64_t)sms * (per_sm > 0 ? per_sm : 1);
     const int nb = (int)(nfull < want ? (nfull > 0 ? nfull : 1) : want);

@@ -44,7 +44,7 @@ class QuokkaContext:
                             "csv_stride": 64 * 1024 * 1024,
                             "bloom_join": True, "bloom_pushdown": True, "broadcast_rows": 100_000,      # semi-join reduction of shuffled probe sides
                             # replicate a build side instead of shuffling both sides when build x ranks <= probe: one exchange and one
-                            # Bloom all-gather fewer per such join (Q3 SF-100 on 2 GPUs: 9.9 ms vs 10.4 ms)
+                            # Bloom all-gather fewer per such join
                             "broadcast_cost_based": True, "broadcast_max_rows": 1 << 26,
                             # as-of joins across ranks: every rank holds a contiguous time range of both sorted streams and joins in
                             # place (False = the reference's hash shuffle of both streams by symbol)

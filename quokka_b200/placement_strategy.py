@@ -1,6 +1,6 @@
 """Where an operator's channels live.  The names and constructor arguments are the reference's
 (pyquokka/placement_strategy.py), because user code passes them to `stateful_transform` and
-`TaskGraph.new_*_node`; the meaning is re-mapped onto GPUs: a "node" is one rank (one B200), and every
+`TaskGraph.new_*_node`; the meaning is re-mapped onto GPUs: a "node" is one rank (one GPU), and every
 strategy answers one question for the SPMD driver -- `owners(world_size)`: which ranks own a channel."""
 from __future__ import annotations
 

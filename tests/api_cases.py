@@ -1,5 +1,5 @@
 """Parity cases for the operator API (QuokkaContext / DataStream / Executors), written once and run
-twice: on the CPU container against tests/cpu_shim.py (host logic only) and on the B200 box against the
+twice: without a GPU against tests/cpu_shim.py (host logic only) and on an H100 against the
 real kernels (tests/test_gpu_api.py).  Expected results come from the oracle and the golden fixtures."""
 from __future__ import annotations
 

@@ -1,5 +1,8 @@
-"""Regenerates tests/golden/*.npz from the reference's own fixtures (run in the build container,
-where /root/reference exists; the GPU box only sees the committed .npz files).
+"""Regenerates tests/golden/*.npz from the reference's own fixtures:
+
+  python tests/golden/make_golden.py <checkout of marsupialtail/quokka @ 1caf62e>
+
+The tests read only the committed .npz files; they never need the reference itself.
 
   join_ab.npz   <- apps/graph_api/tutorials/a.csv, b.csv (the lesson2.1.py:57-68 join self-check;
                    expected pairs from pandas.merge, the engine that script compares against)
@@ -8,10 +11,11 @@ where /root/reference exists; the GPU box only sees the committed .npz files).
                    which agrees with the Polars call the script uses as its own reference)
 """
 import os
+import sys
 import numpy as np
 import pandas as pd
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "."
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

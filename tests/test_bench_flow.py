@@ -88,9 +88,10 @@ def test_parquet_leg(bench_on_shim):
         assert r[f"file_bytes_{codec}"] > 0
 
 
-def test_headline_line(bench_on_shim, monkeypatch, capsys):
+def test_headline_line(bench_on_shim, monkeypatch, capsys, tmp_path):
     """The default (headline) arm: warm-up, timed loop with events, untimed extra steps for the clock sampler, parity
-    check, JSON line with every contract key.  CUDA events / devices are faked; the e2e leg (pinned memory) is off."""
+    check, JSON line with every contract key, the last timed step's result dumped as .npy.  CUDA events / devices are
+    faked; the e2e leg (pinned memory) is off."""
     import json
     import quokka_b200
 
@@ -102,14 +103,19 @@ def test_headline_line(bench_on_shim, monkeypatch, capsys):
     monkeypatch.setattr(quokka_b200, "ops", cpu_shim, raising=False)
     monkeypatch.setattr(torch.cuda, "Event", FakeEvent)
     monkeypatch.setattr(torch.cuda, "set_device", lambda *a, **k: None)
+    monkeypatch.setattr(torch.cuda, "get_device_name", lambda *a, **k: "cpu")
     real_device = torch.device
     monkeypatch.setattr(torch, "device", lambda *a, **k: real_device("cpu"))
     monkeypatch.setenv("WORLD_SIZE", "1")
     args = types.SimpleNamespace(sf=0.01, steps=3, warmup=3, variant=0, no_e2e=True, no_q3=False, no_cpu=False, extras=1, cpu_rows=200_000,
                                  only_q3=False, only_asof=False, only_q5=False, only_parquet=False, q3_sf=0.01, q3_steps=1, replicate_builds=False, no_replicate_builds=False,
-                                 asof_quotes=10_000, e2e_rows=1000, e2e_chunk=1000, parquet_sf=0.01, chunk_rows=0, q5_sf=0.01, no_parquet=False)
+                                 asof_quotes=10_000, e2e_rows=1000, e2e_chunk=1000, parquet_sf=0.01, chunk_rows=0, q5_sf=0.01, no_parquet=False,
+                                 dump_outputs=str(tmp_path / "dump"))
     bench_on_shim.run_ours(args)
     line = json.loads(capsys.readouterr().out.strip().splitlines()[-1])
+    acc, cnt = np.load(tmp_path / "dump" / "q1_acc.npy"), np.load(tmp_path / "dump" / "q1_cnt.npy")
+    assert acc.dtype == cnt.dtype == np.float64 and acc.shape == (6, 5) and cnt.shape == (6,)
+    assert int(cnt.sum()) == line["parity"]["sum_of_group_counts"]
     for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype",
                 "data", "config", "roofline", "cpu_baseline", "e2e", "gpu_launches", "clocks", "parity", "q3", "q5", "asof"):
         assert key in line, key

@@ -1,4 +1,4 @@
-"""The C-ABI boundary without a GPU: libqk.so builds for sm_100a, loads, and exports exactly the entry
+"""The C-ABI boundary without a GPU: libqk.so builds for sm_90a, loads, and exports exactly the entry
 points include/qk.h declares; argument errors are reported through qk_last_error (no compute calls)."""
 import ctypes as C
 import os
@@ -31,11 +31,11 @@ def test_library_builds_loads_and_exports_every_declared_symbol():
     assert lib.qk_version() == 100
 
 
-def test_sass_is_blackwell_native():
-    """sm_100a only, TMA-engine bulk copies + mbarrier transactions present in the hot kernels."""
+def test_sass_is_hopper_native():
+    """sm_90a only, TMA-engine bulk copies + mbarrier transactions present in the hot kernels."""
     from quokka_b200 import _lib
     out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out and "sm_90" not in out
+    assert "sm_90a" in out and "sm_100" not in out and "sm_80" not in out
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
     assert sass.count("UBLKCP") >= 10 and "SYNCS.ARRIVE.TRANS64" in sass
 

@@ -1,4 +1,4 @@
-"""The operator API against the real sm_100a kernels (same cases as tests/test_api_cpu.py)."""
+"""The operator API against the real sm_90a kernels (same cases as tests/test_api_cpu.py)."""
 import pytest
 
 import api_cases as A

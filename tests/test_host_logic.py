@@ -104,7 +104,7 @@ def test_case_like_extract_and_booleans():
         E.compile_expr(E.parse("b like 'x%'"), sch)
     assert E.compile_expr(E.parse("true"), sch) == [(L.OP_CONST, 0, 0, 1.0, 0)] and E.parse("false").value == 0
     # Q14's shape at TPC-H size: 25 of 150 p_type values match 'PROMO%' -- still one node, inside the kernel's limits
-    # (round 1 expanded this to 108 nodes, which the device library refuses: GPUTEST_r01)
+    # (round 1 expanded this to 108 nodes, which the device library refuses)
     types = [f"{a} {b} {c}" for a in ("STANDARD", "SMALL", "MEDIUM", "LARGE", "ECONOMY", "PROMO")
              for b in ("ANODIZED", "BURNISHED", "PLATED", "POLISHED", "BRUSHED") for c in ("TIN", "NICKEL", "BRASS", "STEEL", "COPPER")]
     sch2 = {"p_type": E.ColumnInfo(0, L.QK_U8, types), "x": E.ColumnInfo(1, L.QK_F64), "y": E.ColumnInfo(2, L.QK_F64)}
