@@ -214,9 +214,12 @@ QK_API int qk_hashagg_finalize(const qk_hashagg_desc* desc, const void* state, q
  * Replaces `partition_key_str` (pyquokka/quokka_runtime.py:217-231): integer keys -> channel
  * `key % nparts` (mode QK_PART_MOD, bit-identical placement to the reference for non-negative keys)
  * followed by Polars `partition_by`.  Also used with QK_PART_CODE (key is already a dense code
- * in [0, nparts): segment-by-symbol for the as-of join).  Stable: rows keep their relative order
- * inside a partition.  dest[i] (device int32) = output position of row i; part_offsets (device
- * int64[nparts+1]) = start of each partition in the output.  Then qk_scatter moves each column. */
+ * in [0, nparts), codes outside are clamped: segment-by-symbol for the as-of join and the windows).
+ * Stable: rows keep their relative order inside a partition.  dest[i] (device int32) = output
+ * position of row i; part_offsets (device int64[nparts+1]) = start of each partition in the output.
+ * Then qk_scatter moves each column.  QK_PART_MOD takes nparts in [1, 16384]; QK_PART_CODE any
+ * nparts >= 1 (above 16384 the partition runs one stable pass per 14-bit digit of the code), bounded
+ * by qk_partition_workspace_bytes(nrows, nparts). */
 #define QK_PART_MOD 0
 #define QK_PART_CODE 1
 QK_API size_t qk_partition_workspace_bytes(int64_t nrows, int32_t nparts);

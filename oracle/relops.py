@@ -179,6 +179,22 @@ def asof_backward(l_time: np.ndarray, l_by: np.ndarray, r_time: np.ndarray, r_by
     return out
 
 
+def asof_backward_fast(l_time, l_by, r_time, r_by):
+    """asof_backward without the per-key loop, for many keys: (by, time) packed into one int64 (by < 2^22, 0 <= time < 2^40),
+    the right side sorted by it (input order among equals), one searchsorted for all left rows."""
+    l_time, r_time = np.asarray(l_time, dtype=np.int64), np.asarray(r_time, dtype=np.int64)
+    l_by, r_by = np.asarray(l_by, dtype=np.int64), np.asarray(r_by, dtype=np.int64)
+    for t, b in ((l_time, l_by), (r_time, r_by)):
+        assert not len(t) or (t.min() >= 0 and t.max() < 2 ** 40 and b.min() >= 0 and b.max() < 2 ** 22), "outside the packed range"
+    r_key = (r_by << 40) | r_time
+    r_order = np.argsort(r_key, kind="stable")
+    rk = r_key[r_order]
+    j = np.searchsorted(rk, (l_by << 40) | l_time, side="right") - 1      # the last right row with key <= (by, t)
+    jc = np.maximum(j, 0)
+    ok = (j >= 0) & (rk[jc] >> 40 == l_by) if len(rk) else np.zeros(len(l_time), bool)
+    return np.where(ok, r_order[jc] if len(rk) else -1, -1).astype(np.int64)
+
+
 # ------------------------------------------------------------------ aggregate decomposition strings
 def decompose_aggregations(aggs: list):
     """Restates parse_multiple_aggregations (pyquokka/sql_utils.py:379-413) for the plain
@@ -258,3 +274,147 @@ def session_window(time, by, timeout, aggs):
             for name, (op, v) in aggs.items():
                 rows[name].append(_agg(op, np.asarray(v)[idx][a:b]) if v is not None else b - a)
     return {k: np.array(v) for k, v in rows.items()}
+
+
+# ------------------------------------------------------------------ vectorised windows (same results as the three above)
+# The functions above loop per row in Python.  These give the same answers at test sizes: the rows are put in (key, time)
+# order, every window becomes a row range [lo, hi) of that order (searchsorted, one call per key at most), and the ranges
+# are aggregated with prefix sums (SUM / COUNT / AVG) and a sparse table (MIN / MAX).  SUM is exact for values that are
+# integer multiples of 2^-63 below 2^40 in magnitude (see range_sum_exact), so the references make no rounding error of
+# their own beyond the final conversion to fp64.
+def window_order(time, by):
+    """(order, sorted time, sorted by, key values, segment starts [nkeys + 1]): the rows by key, then time, then input order."""
+    time, by = np.asarray(time, dtype=np.int64), np.asarray(by)
+    order = np.lexsort((time, by))
+    ts, bs = time[order], by[order]
+    keys, starts = np.unique(bs, return_index=True)
+    return order, ts, bs, keys, np.append(starts, len(bs)).astype(np.int64)
+
+
+def _per_key_searchsorted(ts, seg, key_pos, x, side):
+    """For every query x[j] of key number key_pos[j] (queries grouped by key): seg start + searchsorted in that key's times."""
+    out = np.empty(len(x), dtype=np.int64)
+    if not len(x):
+        return out
+    cut = np.flatnonzero(np.diff(key_pos)) + 1
+    for a, b in zip(np.concatenate([[0], cut]), np.concatenate([cut, [len(x)]])):
+        s0, s1 = seg[key_pos[a]], seg[key_pos[a] + 1]
+        out[a:b] = s0 + np.searchsorted(ts[s0:s1], x[a:b], side=side)
+    return out
+
+
+def sliding_window_ranges(time, by, size):
+    """(order, lo, hi): sorted row r aggregates sorted rows [lo[r], hi[r]) -- its key's rows with time in (t - size, t]."""
+    order, ts, bs, keys, seg = window_order(time, by)
+    kp = np.searchsorted(keys, bs)
+    return order, _per_key_searchsorted(ts, seg, kp, ts - np.int64(size), "right"), _per_key_searchsorted(ts, seg, kp, ts, "right")
+
+
+def hopping_window_ranges(time, by, size, hop):
+    """(order, key, start, lo, hi) of every non-empty window [start, start + size), start = k * hop >= the key's first time
+    truncated to hop, ordered by key and start.  Candidates: for every row the windows k * hop <= t whose start is at most
+    ceil(size / hop) hops back, which covers every window that holds a row; membership is then decided by searchsorted."""
+    order, ts, bs, keys, seg = window_order(time, by)
+    hop, size = np.int64(hop), np.int64(size)
+    slots = int(-(-size // hop))
+    kp = np.searchsorted(keys, bs)
+    k = (ts // hop)[:, None] - np.arange(slots, dtype=np.int64)[None, :]
+    kk = np.repeat(kp, slots)
+    k = k.reshape(-1)
+    first = (ts[seg[:-1]] // hop) if len(keys) else np.zeros(0, np.int64)
+    keep = k >= first[kk]
+    kk, k = kk[keep], k[keep]
+    o = np.lexsort((k, kk))
+    kk, k = kk[o], k[o]
+    new = np.ones(len(k), bool)
+    new[1:] = (kk[1:] != kk[:-1]) | (k[1:] != k[:-1])
+    kk, start = kk[new], k[new] * hop
+    lo = _per_key_searchsorted(ts, seg, kk, start, "left")
+    hi = _per_key_searchsorted(ts, seg, kk, start + size, "left")
+    ne = hi > lo
+    return order, keys[kk[ne]], start[ne], lo[ne], hi[ne]
+
+
+def session_window_ranges(time, by, timeout):
+    """(order, key, start time, lo, hi) of every session, ordered by key and start: a key's rows split at gaps > timeout."""
+    order, ts, bs, keys, seg = window_order(time, by)
+    n = len(ts)
+    new = np.ones(n, bool)
+    new[1:] = (bs[1:] != bs[:-1]) | ((ts[1:] - ts[:-1]) > timeout)
+    lo = np.flatnonzero(new).astype(np.int64)
+    hi = np.append(lo[1:], n).astype(np.int64)
+    return order, bs[lo], ts[lo], lo, hi
+
+
+def range_sum_exact(v, lo, hi):
+    """Sums of v[lo:hi] as np.longdouble, exact up to the final rounding to long double.  Every value is split into its
+    integer part and its fraction scaled by 2^63 (two int64 limbs); int64 prefix sums of the three parts are exact.
+    Requires |v| < 2^40 and v an integer multiple of 2^-63 (true of every fp64 with |v| >= 2^-11)."""
+    v = np.asarray(v, dtype=np.float64)
+    a = np.trunc(v)
+    f = (v - a) * 2.0 ** 63                       # v - trunc(v) is exact; scaling by a power of two too
+    assert np.all(np.abs(v) < 2.0 ** 40) and np.all(f == np.trunc(f)), "values outside the exact range of range_sum_exact"
+    fi = f.astype(np.int64)
+    fh = fi >> 31
+    fl = fi - (fh << 31)
+    sums = []
+    for part in (a.astype(np.int64), fh, fl):
+        p = np.concatenate([[0], np.cumsum(part)])
+        sums.append((p[hi] - p[lo]).astype(np.longdouble))
+    return sums[0] + sums[1] * np.longdouble(2.0 ** -32) + sums[2] * np.longdouble(2.0 ** -63)
+
+
+def range_minmax(v, lo, hi, fn):
+    """fn (np.minimum / np.maximum) over v[lo:hi] for non-empty ranges: sparse table, one level at a time (O(n) memory)."""
+    v = np.asarray(v, dtype=np.float64)
+    out = np.empty(len(lo), dtype=np.float64)
+    if not len(lo):
+        return out
+    w = hi - lo
+    assert np.all(w > 0)
+    level = np.frexp(w.astype(np.float64))[1] - 1          # floor(log2(w))
+    cur = v
+    for j in range(int(level.max()) + 1):
+        q = np.flatnonzero(level == j)
+        out[q] = fn(cur[lo[q]], cur[hi[q] - (1 << j)])      # two overlapping blocks of 2^j rows
+        cur = fn(cur[:len(cur) - (1 << j)], cur[(1 << j):])  # cur[i] = fn over v[i : i + 2^(j+1)]
+    return out
+
+
+def range_aggregate(op, v, lo, hi):
+    """op over v[lo:hi] for every range (v in the order lo / hi index; None for COUNT): fp64, one rounding for SUM / AVG."""
+    if op == "count":
+        return (hi - lo).astype(np.float64)
+    if op in ("min", "max"):
+        return range_minmax(v, lo, hi, np.minimum if op == "min" else np.maximum)
+    s = range_sum_exact(v, lo, hi).astype(np.float64)
+    return s if op == "sum" else s / (hi - lo)
+
+
+def sliding_window_fast(time, by, size, aggs):
+    """sliding_window, vectorised: {name: fp64 array aligned with the input rows}."""
+    order, lo, hi = sliding_window_ranges(time, by, size)
+    out = {}
+    for name, (op, v) in aggs.items():
+        r = np.empty(len(order), dtype=np.float64)
+        r[order] = range_aggregate(op, None if v is None else np.asarray(v)[order], lo, hi)
+        out[name] = r
+    return out
+
+
+def _grouped(ranges, aggs):
+    order, key, start, lo, hi = ranges
+    out = {"by": key, "start": start}
+    for name, (op, v) in aggs.items():
+        out[name] = range_aggregate(op, None if v is None else np.asarray(v)[order], lo, hi)
+    return out
+
+
+def hopping_window_fast(time, by, size, hop, aggs):
+    """hopping_window, vectorised: {"by", "start", name...}, one row per non-empty window, ordered by key and start."""
+    return _grouped(hopping_window_ranges(time, by, size, hop), aggs)
+
+
+def session_window_fast(time, by, timeout, aggs):
+    """session_window, vectorised: {"by", "start", name...}, one row per session, ordered by key and start."""
+    return _grouped(session_window_ranges(time, by, timeout), aggs)

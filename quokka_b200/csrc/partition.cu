@@ -151,6 +151,46 @@ __global__ void __launch_bounds__(P_NT) k_part_dest(const void* key, int dt, int
     }
 }
 
+// ---------------------------------------------------------------- CODE mode over more than P_SMEM_PARTS partitions
+// LSD radix: the clamped code is split into 14-bit digits and every digit gets one stable pass of the kernels above (a
+// P_SMEM_PARTS-way CODE partition of the digit column).  Stable passes from the low digit up leave the rows sorted by the
+// whole code, in input order within a code.
+constexpr int P_DIGIT_BITS = 14;
+static_assert((1 << P_DIGIT_BITS) == P_SMEM_PARTS, "one digit = one shared-memory partition pass");
+
+__device__ __forceinline__ int32_t clamped_code(const void* key, int dt, int64_t row, int nparts) {
+    const int64_t k = load_i64(key, dt, row);
+    return (int32_t)(k < 0 ? 0 : (k >= nparts ? nparts - 1 : k));
+}
+
+// digit[r] = (clamped code of row r >> shift) & (P_SMEM_PARTS - 1)
+__global__ void __launch_bounds__(256) k_radix_digit(const void* key, int dt, int64_t n, int nparts, int shift, int32_t* digit) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        digit[i] = (clamped_code(key, dt, i, nparts) >> shift) & (P_SMEM_PARTS - 1);
+}
+
+// after a pass with destination `pass_dest`: the codes move to their new positions, and the final destination of every
+// original row follows one more step (dest[i] = pass_dest[dest[i]]; skipped after the first pass, which wrote dest itself)
+__global__ void __launch_bounds__(256) k_radix_move(const void* key, int dt, int64_t n, int nparts, const int32_t* pass_dest,
+                                                    int32_t* moved, int32_t* dest, int compose) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        moved[pass_dest[i]] = clamped_code(key, dt, i, nparts);
+        if (compose) dest[i] = pass_dest[dest[i]];
+    }
+}
+
+// part_offsets[p] = first position whose code is >= p, over the fully sorted codes (p = nparts gives n)
+__global__ void __launch_bounds__(256) k_radix_offsets(const int32_t* sorted, int64_t n, int nparts, int64_t* part_offsets) {
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p <= nparts; p += (int64_t)gridDim.x * blockDim.x) {
+        int64_t lo = 0, hi = n;
+        while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (sorted[mid] < p) lo = mid + 1; else hi = mid;
+        }
+        part_offsets[p] = lo;
+    }
+}
+
 // ---------------------------------------------------------------- scatter / gather
 struct MoveArgs {
     const void* src[QK_MAX_COLS];
@@ -235,30 +275,47 @@ int fill_move(MoveArgs& M, const qk_column* cols, int ncols, qk_column* out, int
 
 using namespace qk;
 
-extern "C" size_t qk_partition_workspace_bytes(int64_t nrows, int32_t nparts) {
-    if (nrows < 0 || nparts <= 0) return 0;
+// workspace of one shared-memory partition (nparts <= P_SMEM_PARTS)
+static size_t smem_plan_bytes(int64_t nrows, int32_t nparts) {
     const int64_t cr = chunk_rows_for(nrows, nparts);
     const int64_t nchunks = (nrows + cr - 1) / cr + 1;
     return align_up((size_t)nchunks * nparts * 4, 256) + align_up((size_t)nchunks * nparts * 8, 256) + align_up((size_t)nparts * 8, 256);
 }
 
-extern "C" int qk_partition_plan(const qk_column* key, int32_t nparts, int32_t mode, int32_t* dest,
-                                 int64_t* part_offsets, void* workspace, size_t ws_bytes, void* stream) {
-    const char* who = "qk_partition_plan";
-    if (int rc = check_col(key, who)) return rc;
-    if (!dtype_is_int(key->dtype)) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: only integer keys are supported (the reference pins `key %% n` for ints only)", who);
-    if (nparts <= 0 || nparts > P_SMEM_PARTS) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: nparts must be in [1, %d]", who, P_SMEM_PARTS);
-    if (mode != QK_PART_MOD && mode != QK_PART_CODE) QK_FAIL(QK_ERR_INVALID, "%s: bad mode", who);
-    if (!part_offsets || (key->length > 0 && !dest)) QK_FAIL(QK_ERR_INVALID, "%s: null output", who);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int64_t n = key->length;
-    if (n == 0) {
-        QK_CUDA(cudaMemsetAsync(part_offsets, 0, sizeof(int64_t) * (nparts + 1), st));
-        return QK_OK;
+// partitions of the radix pass that handles the digit at `shift` (the top digit needs fewer than P_SMEM_PARTS)
+static int radix_pass_parts(int32_t nparts, int shift) {
+    const int32_t top = (nparts - 1) >> shift;
+    return top >= P_SMEM_PARTS - 1 ? P_SMEM_PARTS : top + 1;
+}
+
+static int radix_passes(int32_t nparts) {
+    int bits = 0;
+    while (bits < 31 && ((int64_t)(nparts - 1) >> bits) != 0) ++bits;
+    return (bits + P_DIGIT_BITS - 1) / P_DIGIT_BITS;
+}
+
+// radix path: digit, pass destination, two code buffers (n x int32 each), the pass's part_offsets, then one
+// shared-memory partition's workspace
+static size_t radix_plan_bytes(int64_t nrows, int32_t nparts) {
+    size_t inner = 0;
+    for (int d = 0; d < radix_passes(nparts); ++d) {
+        const size_t b = smem_plan_bytes(nrows, radix_pass_parts(nparts, d * P_DIGIT_BITS));
+        inner = b > inner ? b : inner;
     }
+    return 4 * align_up((size_t)nrows * 4, 256) + align_up((size_t)(P_SMEM_PARTS + 1) * 8, 256) + inner;
+}
+
+extern "C" size_t qk_partition_workspace_bytes(int64_t nrows, int32_t nparts) {
+    if (nrows < 0 || nparts <= 0) return 0;
+    return nparts <= P_SMEM_PARTS ? smem_plan_bytes(nrows, nparts) : radix_plan_bytes(nrows, nparts);
+}
+
+// one stable partition with its per-chunk histograms in shared memory (nparts <= P_SMEM_PARTS)
+static int smem_plan(const qk_column* key, int32_t nparts, int32_t mode, int32_t* dest, int64_t* part_offsets, void* workspace,
+                     cudaStream_t st) {
+    const int64_t n = key->length;
     const int64_t chunk_rows = chunk_rows_for(n, nparts);
     const int64_t nchunks = (n + chunk_rows - 1) / chunk_rows;
-    if (!workspace || ws_bytes < qk_partition_workspace_bytes(n, nparts)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
     unsigned* hist = (unsigned*)workspace;
     int64_t* offsets = (int64_t*)((char*)workspace + align_up((size_t)(nchunks + 1) * nparts * 4, 256));
     int64_t* totals = (int64_t*)((char*)offsets + align_up((size_t)(nchunks + 1) * nparts * 8, 256));
@@ -277,6 +334,62 @@ extern "C" int qk_partition_plan(const qk_column* key, int32_t nparts, int32_t m
     k_part_dest<<<(unsigned)nb, P_NT, smem_dest, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, offsets, part_offsets, dest);
     QK_LAUNCH_CHECK("k_part_dest");
     return QK_OK;
+}
+
+static unsigned grid_of(int64_t n) {            // grid-stride kernels: 256 threads per block, at most 16 blocks per SM
+    const int64_t nb = (n + 255) / 256, cap = (int64_t)sm_count() * 16;
+    return (unsigned)(nb < 1 ? 1 : (nb > cap ? cap : nb));
+}
+
+// CODE partition with more than P_SMEM_PARTS parts: one stable shared-memory pass per 14-bit digit of the clamped code,
+// low digit first, then part_offsets by binary search in the sorted codes
+static int radix_plan(const qk_column* key, int32_t nparts, int32_t* dest, int64_t* part_offsets, void* workspace, cudaStream_t st) {
+    const int64_t n = key->length;
+    char* w = (char*)workspace;
+    const size_t col_bytes = align_up((size_t)n * 4, 256);
+    int32_t* digit = (int32_t*)w; w += col_bytes;
+    int32_t* pass_dest = (int32_t*)w; w += col_bytes;
+    int32_t* codes[2] = {(int32_t*)w, (int32_t*)(w + col_bytes)}; w += 2 * col_bytes;
+    int64_t* pass_offsets = (int64_t*)w; w += align_up((size_t)(P_SMEM_PARTS + 1) * 8, 256);
+    const unsigned grid = grid_of(n);
+    const void* src = key->data;
+    int src_dt = key->dtype;
+    const int passes = radix_passes(nparts);
+    for (int d = 0; d < passes; ++d) {
+        const int shift = d * P_DIGIT_BITS;
+        k_radix_digit<<<grid, 256, 0, st>>>(src, src_dt, n, nparts, shift, digit);
+        QK_LAUNCH_CHECK("k_radix_digit");
+        qk_column dcol = *key;
+        dcol.data = digit; dcol.dtype = QK_I32;
+        int32_t* out = d == 0 ? dest : pass_dest;
+        if (int rc = smem_plan(&dcol, radix_pass_parts(nparts, shift), QK_PART_CODE, out, pass_offsets, w, st)) return rc;
+        k_radix_move<<<grid, 256, 0, st>>>(src, src_dt, n, nparts, out, codes[d & 1], dest, d > 0);
+        QK_LAUNCH_CHECK("k_radix_move");
+        src = codes[d & 1]; src_dt = QK_I32;
+    }
+    k_radix_offsets<<<grid_of((int64_t)nparts + 1), 256, 0, st>>>((const int32_t*)src, n, nparts, part_offsets);
+    QK_LAUNCH_CHECK("k_radix_offsets");
+    return QK_OK;
+}
+
+extern "C" int qk_partition_plan(const qk_column* key, int32_t nparts, int32_t mode, int32_t* dest,
+                                 int64_t* part_offsets, void* workspace, size_t ws_bytes, void* stream) {
+    const char* who = "qk_partition_plan";
+    if (int rc = check_col(key, who)) return rc;
+    if (!dtype_is_int(key->dtype)) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: only integer keys are supported (the reference pins `key %% n` for ints only)", who);
+    if (mode != QK_PART_MOD && mode != QK_PART_CODE) QK_FAIL(QK_ERR_INVALID, "%s: bad mode", who);
+    if (nparts <= 0 || (mode == QK_PART_MOD && nparts > P_SMEM_PARTS))
+        QK_FAIL(QK_ERR_UNSUPPORTED, "%s: nparts must be in [1, %d]%s", who, P_SMEM_PARTS, mode == QK_PART_MOD ? " in MOD mode" : "");
+    if (!part_offsets || (key->length > 0 && !dest)) QK_FAIL(QK_ERR_INVALID, "%s: null output", who);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t n = key->length;
+    if (n == 0) {
+        QK_CUDA(cudaMemsetAsync(part_offsets, 0, sizeof(int64_t) * ((size_t)nparts + 1), st));
+        return QK_OK;
+    }
+    if (!workspace || ws_bytes < qk_partition_workspace_bytes(n, nparts)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
+    if (nparts > P_SMEM_PARTS) return radix_plan(key, nparts, dest, part_offsets, workspace, st);
+    return smem_plan(key, nparts, mode, dest, part_offsets, workspace, st);
 }
 
 extern "C" int qk_scatter(const qk_column* cols, int32_t ncols, const int32_t* dest, qk_column* out, void* stream) {

@@ -201,7 +201,13 @@ class HashAggState:
         return ok, ov, _t(out["n"])
 
 
+PART_MOD_MAX_PARTS = 16_384              # csrc/partition.cu: MOD partitions keep their per-chunk histogram in shared memory
+MERGE_MAX_KEYS = 40_960                  # csrc/asof.cu: the merge kernel's per-key table is at most 160 KB of int32
+
+
 def partition_plan(key, nparts, mode=L.PART_MOD):
+    if nparts < 1 or (mode == L.PART_MOD and nparts > PART_MOD_MAX_PARTS):
+        raise L.QkError(f"qk_partition_plan: nparts must be in [1, {PART_MOD_MAX_PARTS}] in MOD mode")
     k = key.numpy().astype(np.int64)
     p = k % nparts if mode == L.PART_MOD else np.clip(k, 0, nparts - 1)
     order = np.argsort(p, kind="stable")
@@ -258,7 +264,7 @@ def asof_backward(l_time, l_by, r_time, r_by, n_by):
 
 
 def asof_merge(l_time, l_by, r_time, r_by, n_by, carry_in=None, r_base=0, want_carry=False):
-    if n_by > 40_000:                        # csrc/asof.cu: the per-key table must fit shared memory
+    if n_by > MERGE_MAX_KEYS:
         return None, None
     lb, rb = l_by.numpy().astype(np.int64), r_by.numpy().astype(np.int64)
     idx = R.asof_backward(l_time.numpy(), lb, r_time.numpy(), rb).astype(np.int64)
