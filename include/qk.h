@@ -361,6 +361,26 @@ QK_API size_t qk_topk_workspace_bytes(int64_t nrows);
 QK_API int qk_topk_candidates(const qk_column* key, int32_t k, int32_t descending, int32_t* out_idx,
                        int64_t* out_n, void* workspace, size_t ws_bytes, void* stream);
 
+/* ---- K9: Gram matrix on the FP64 tensor cores ------------------------------------------------
+ * Replaces the per-batch np.dot(x.T, x) of DataStream.gramian and the sums of DataStream.covariance
+ * (pyquokka/datastream.py:1033-1147).  X = nrows x k, cols[i] one column (QK_F64 / QK_F32 / QK_I32 / QK_I64, all of length
+ * nrows), widened to fp64 as it is staged; shift (device fp64[k] or NULL = 0) is subtracted in fp64 before the product, so a
+ * shifted value rounds as `x.to_numpy() - demean` does.  Accumulates
+ *     gram[i * k + j] += sum_rows (x_i - c_i)(x_j - c_j)   (device fp64[k * k], row-major, symmetric)
+ *     sums[i]         += sum_rows (x_i - c_i)              (device fp64[k], or NULL = not computed)
+ * so successive calls over the batches of a stream sum up.  Products run on mma.sync f64 (DMMA); only the tiles on and above
+ * the diagonal are computed and mirrored.  Deterministic: per-CTA partial tiles are folded in a fixed order, so the same
+ * inputs give bit-identical results on the same device.  Every row is read once when k + 1 <= 128 (one column block).
+ * variant: 0 = auto (m16n8k16 where the tile shape allows it, k + 1 > 8; m8n8k4 below), 1 = m8n8k4, 2 = m16n8k16.
+ * Workspace: qk_gram_workspace_bytes(nrows, k) bytes; the column table travels in it, so any k fits.  nrows == 0 is a no-op.
+ * Errors: k < 1, null data with length > 0, a length != nrows or an unsupported dtype: QK_ERR_INVALID; a validity mask:
+ * QK_ERR_UNSUPPORTED; workspace too small: QK_ERR_CAPACITY. */
+QK_API size_t qk_gram_workspace_bytes(int64_t nrows, int32_t k);
+QK_API int qk_gram(const qk_column* cols, int32_t k, int64_t nrows, const double* shift, double* gram, double* sums,
+                   int32_t variant, void* workspace, size_t ws_bytes, void* stream);
+/* tile shape, MMA shape and row-range split of the last qk_gram call on this thread, e.g. "T128 m8n8k4 s1" */
+QK_API const char* qk_gram_last_plan(void);
+
 /* ---- synthetic TPC-H-shaped / SIP-shaped columns, generated in HBM --------------------------
  * Bit-identical to oracle/tpch_gen.py (counter-based hash of (table, column, row)); lets bench.py hold
  * SF-100 (600 037 902 lineitem rows) resident without a 23 GB host copy.  `column` ids: see

@@ -10,6 +10,7 @@ Only what the judged configs and their tests touch is implemented; the rest rais
 """
 from __future__ import annotations
 
+import numpy as np
 import pyarrow as pa
 
 from . import _lib as L
@@ -738,6 +739,35 @@ class DataStream:
         s = self._new(MapNode(self.node, new))
         s = s.select([tmp.get(c, c) for c in self.schema])
         return s.rename({v: k for k, v in tmp.items()})
+
+    def _gram_stream(self, columns, executor_args, mode):
+        from .executors import GramFinalExecutor, GramPartialExecutor
+        assert type(columns) == list and len(columns) > 0, "columns must be a non-empty list"
+        assert len(set(columns)) == len(columns), "columns must be distinct"
+        for c in columns:
+            assert c in self.schema, f"column {c} not in schema"
+        part = StatefulNode({0: self.node}, GramPartialExecutor(columns, **executor_args), ["__gram"], {0: set(columns)},
+                            {0: PassThroughPartitioner()}, CustomChannelsStrategy(1))
+        node = StatefulNode({0: part}, GramFinalExecutor(columns, mode), list(columns), {0: {"__gram"}},
+                            {0: BroadcastPartitioner()}, SingleChannelStrategy())
+        return DataStream(self.quokka_context, node)
+
+    def gramian(self, columns, demean=None):
+        """DataStream[columns]^T DataStream[columns] (pyquokka/datastream.py:1033-1097): a DataStream with schema `columns` and
+        len(columns) fp64 rows, row i = row i of the matrix.  `demean` (numpy array, one value per column) is subtracted from
+        every row first.  Integer and float columns; string and date columns raise; NULLs count as NaN.  Computed per batch by
+        qk_gram on the FP64 tensor cores, summed per rank, then over the ranks."""
+        if demean is not None:
+            assert type(demean) == np.ndarray, "demean must be a numpy array"
+            assert len(demean) == len(columns), "demean must be the same length as columns"
+        return self._gram_stream(list(columns), {"demean": demean}, "gramian")
+
+    def covariance(self, columns):
+        """Covariance matrix of `columns`, divided by the row count as the reference does (np.cov(bias=True),
+        pyquokka/datastream.py:1100-1147).  Blocking; returns a pyarrow.Table.  One pass over the stream (the reference runs it
+        twice: the means, then the gramian): every rank shifts by the first row it sees and the ranks are re-centred on the
+        global mean at the end.  An empty stream gives NaN."""
+        return self._gram_stream(list(columns), {"shift_first_row": True}, "covariance").collect()
 
     def __repr__(self):
         return "DataStream[" + ",".join(self.schema) + "]"

@@ -14,6 +14,7 @@ import os
 import re
 
 import numpy as np
+import pyarrow as pa
 import torch
 
 from . import _lib as L
@@ -577,6 +578,107 @@ class DistinctExecutor(Executor):
             return
         ok, _, _ = self._ha.finalize()
         self.state = DeviceTable({k: DeviceColumn(o, m[0], m[1]) for k, o, m in zip(self.keys, ok, self._meta)})
+        return self.state
+
+
+# ---------------------------------------------------------------------------------------------- Gram matrix
+def _gram_input(col: DeviceColumn, name: str) -> torch.Tensor:
+    """A column as qk_gram reads it.  Numbers only: string (dictionary) and date / time columns have no product, as np.dot
+    of the reference fails on them.  A NULL (right side of a left / as-of join) becomes NaN, as Polars' to_numpy() makes it."""
+    if col.dictionary is not None:
+        raise L.QkError(f"gramian / covariance: column {name!r} is a string column")
+    if col.arrow_type is not None and not pa.types.is_boolean(col.arrow_type):
+        raise L.QkError(f"gramian / covariance: column {name!r} has type {col.arrow_type}, not a number")
+    t = col.data
+    if t.dtype not in (torch.float64, torch.float32, torch.int32, torch.int64):
+        t = t.to(torch.int32)                              # bool / uint8 flags count as 0 / 1
+    if col.valid is not None:
+        t = torch.where(col.valid.bool(), t.to(torch.float64), torch.full_like(t, float("nan"), dtype=torch.float64))
+    return t.contiguous()
+
+
+class GramPartialExecutor(Executor):
+    """Per-rank phase of DataStream.gramian / covariance (pyquokka/datastream.py:1033-1147, whose per-batch np.dot partials are
+    summed by an AggExecutor per channel): every batch is folded into a GramState by qk_gram.  The shift is `demean` (gramian) or,
+    with shift_first_row, the first row this rank sees (covariance: the final phase re-centres the ranks on the global mean,
+    and a shift near the data keeps the fp64 sums from cancelling).  done() emits the state as ONE flat fp64 column
+    [executor_id, n, c (k), s (k), G (k * k)]: the exchange carries at most 16 columns, a k-column table would not fit."""
+
+    silent_streams = "all"       # execute() only accumulates; the state leaves in done()
+
+    def __init__(self, columns, demean=None, shift_first_row=False) -> None:
+        self.columns = list(columns)
+        self.demean = None if demean is None else np.asarray(demean, dtype=np.float64)
+        self.shift_first_row = shift_first_row
+        self.state = None
+        self.shift = None
+
+    def execute(self, batches, stream_id, executor_id):
+        for b in _clean(batches):
+            xs = [_gram_input(b[c], c) for c in self.columns]
+            if self.state is None:
+                self.state = ops.GramState(len(self.columns), b.device)
+                if self.shift_first_row:
+                    self.shift = torch.cat([x[:1].to(torch.float64) for x in xs])
+                elif self.demean is not None:
+                    self.shift = torch.from_numpy(self.demean.copy()).to(b.device)
+            self.state.update(xs, self.shift)
+
+    def done(self, executor_id):
+        if self.state is None:
+            return None
+        s = self.state
+        shift = self.shift if self.shift is not None else torch.zeros(s.k, dtype=torch.float64, device=s.gram.device)
+        head = torch.tensor([float(executor_id), float(s.n)], dtype=torch.float64, device=s.gram.device)
+        flat = torch.cat([head, shift, s.sums, s.gram.reshape(-1)])
+        return DeviceTable({"__gram": DeviceColumn(flat)})
+
+
+class GramFinalExecutor(Executor):
+    """Final phase of DataStream.gramian / covariance on one channel: sums the per-rank partials in rank order and emits the
+    k x k result as a table with the schema `columns` (row i = row i of the matrix).  mode "gramian": sum of the G_r (every
+    rank used the same shift).  mode "covariance": re-centres rank r's (n_r, c_r, G_r, s_r) on the global mean
+    mu = sum_r (n_r c_r + s_r) / n with d_r = c_r - mu, sum_r [G_r + s_r d_r^T + d_r s_r^T + n_r d_r d_r^T], and divides by n
+    (np.cov(bias=True), as the reference divides by the row count).  O(ranks k^2) fp64 work on the final state."""
+
+    silent_streams = "all"       # the matrix leaves in done()
+
+    def __init__(self, columns, mode="gramian") -> None:
+        assert mode in ("gramian", "covariance")
+        self.columns = list(columns)
+        self.mode = mode
+        self.parts = []
+        self.state = None
+
+    def execute(self, batches, stream_id, executor_id):
+        for b in _clean(batches):
+            flat = b["__gram"].data
+            width = 2 + 2 * len(self.columns) + len(self.columns) ** 2
+            for lo in range(0, flat.numel(), width):        # partials of several ranks may arrive in one batch
+                self.parts.append(flat[lo:lo + width])
+
+    def done(self, executor_id):
+        k = len(self.columns)
+        dev = self.parts[0].device if self.parts else default_device()
+        parts = sorted(self.parts, key=lambda p: float(p[0]))
+        n = sum(float(p[1]) for p in parts)
+        G = torch.zeros(k, k, dtype=torch.float64, device=dev)
+        if self.mode == "gramian":
+            for p in parts:
+                G += p[2 + 2 * k:].reshape(k, k)
+        elif n == 0:
+            G.fill_(float("nan"))
+        else:
+            mu = torch.zeros(k, dtype=torch.float64, device=dev)
+            for p in parts:
+                mu += float(p[1]) * p[2:2 + k] + p[2 + k:2 + 2 * k]
+            mu /= n
+            for p in parts:
+                nr, c, s, g = float(p[1]), p[2:2 + k], p[2 + k:2 + 2 * k], p[2 + 2 * k:].reshape(k, k)
+                d = c - mu
+                G += g + torch.outer(s, d) + torch.outer(d, s) + nr * torch.outer(d, d)
+            G /= n
+        self.state = DeviceTable({c: DeviceColumn(G[:, j].contiguous()) for j, c in enumerate(self.columns)})
         return self.state
 
 

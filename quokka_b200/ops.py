@@ -492,6 +492,41 @@ def topk_candidates(key: torch.Tensor, k: int, descending: bool):
     return idx[:int(cnt.item())]
 
 
+# ------------------------------------------------------------------ K9 Gram matrix
+class GramState:
+    """Running Gram matrix of a stream of k-column batches (qk_gram): gram = sum (X - c)^T (X - c) (fp64 [k, k]),
+    sums = sum (X - c) (fp64 [k]) and n = rows seen.  The shift c is the caller's: pass the same one to every update."""
+
+    def __init__(self, k: int, device):
+        self.k = int(k)
+        if self.k < 1:
+            raise L.QkError("GramState: k must be >= 1")
+        self.gram = torch.zeros(self.k, self.k, dtype=torch.float64, device=device)
+        self.sums = torch.zeros(self.k, dtype=torch.float64, device=device)
+        self.n = 0
+        self.ws = None
+
+    def update(self, columns: Sequence[torch.Tensor], shift: torch.Tensor | None = None, variant: int = 0):
+        if len(columns) != self.k:
+            raise L.QkError(f"GramState.update: {len(columns)} columns for a {self.k}-column state")
+        n = columns[0].numel()
+        if shift is not None:
+            _require_cuda(shift, "gram shift")
+            if shift.dtype != torch.float64 or shift.numel() != self.k:
+                raise L.QkError("GramState.update: the shift must be fp64 with one value per column")
+        need = int(L.lib().qk_gram_workspace_bytes(n, self.k))
+        if self.ws is None or self.ws.numel() < need:
+            self.ws = _ws(need, self.gram.device)
+        L.check(L.lib().qk_gram(cols(columns, "gram column"), self.k, n, shift.data_ptr() if shift is not None else None,
+                                self.gram.data_ptr(), self.sums.data_ptr(), int(variant), self.ws.data_ptr(), self.ws.numel(),
+                                _stream()), "qk_gram")
+        self.n += n
+
+
+def gram_last_plan() -> str:
+    return L.lib().qk_gram_last_plan().decode()
+
+
 # ------------------------------------------------------------------ Parquet column chunks -> Arrow-layout columns
 PQ_PAD = 16      # readable bytes the decoder may touch past the last encoded byte (aligned 8-byte windows)
 
