@@ -381,6 +381,49 @@ QK_API int qk_gram(const qk_column* cols, int32_t k, int64_t nrows, const double
 /* tile shape, MMA shape and row-range split of the last qk_gram call on this thread, e.g. "T128 m8n8k4 s1" */
 QK_API const char* qk_gram_last_plan(void);
 
+/* ---- K10: quantile sketch -------------------------------------------------------------------------
+ * Replaces the host t-digest plugin (ldbpy.NTDigest) of DataStream.approximate_quantile / approximate_median
+ * (pyquokka/datastream.py:905-1031).  Every value is widened to fp64 and mapped to its order-preserving image
+ * (sign bit set for positives, all bits flipped for negatives; NaN first made 0x7FF8000000000000, so it sorts last).  The
+ * sketch is an open-addressed device table of `capacity` qk_qslot (a power of two): per key = column << 22 | bucket,
+ * bucket = image >> QK_QSKETCH_SHIFT (sign, exponent and the top 10 mantissa bits), the row count and the smallest and
+ * largest image.  An empty slot is {QK_QSKETCH_EMPTY, 0, ~0, 0}: the caller fills a new table with that pattern.  The state
+ * depends only on the multiset of values, so sketches of any split of the rows merge into the same table.
+ * ctrl: device uint64[4] owned by the caller, zero when the table is new.  ctrl[0] = occupied slots (reservations included
+ * while a call runs; exact when it has finished), ctrl[1] = tiles deferred by the last update, ctrl[2] = 1 when a probe ran
+ * through the whole table (a caller that broke the load limit; the entries concerned were dropped).
+ *
+ * qk_qsketch_update: folds k columns of nrows rows (QK_F64 / QK_F32 / QK_I64 / QK_I32 / QK_U8) into the table.  valid: NULL
+ * or a HOST array of k device uint8 row masks (an entry may be NULL); a row counts where its mask is non-zero
+ * (qk_column.validity stays NULL, per the convention above).  The work unit is a tile of QK_QSKETCH_TILE rows of one column,
+ * tile t = column * ceil(nrows / QK_QSKETCH_TILE) + row tile.  tiles: NULL = all k * ceil(nrows / TILE) tiles (ntiles must
+ * equal that), or a device int32 list of ntiles tile ids.  A tile whose new buckets would push the load past capacity / 2
+ * is not counted at all: its id is appended to `deferred` (device int32, room for ntiles) and ctrl[1] counts it.  The
+ * caller reads ctrl, grows the table (qk_qsketch_merge of the old entries into a larger one) and runs the deferred list
+ * again; every row is counted exactly once.  ctrl[1] is cleared by the call.  Workspace: qk_qsketch_workspace_bytes(k).
+ * qk_qsketch_merge: inserts n compacted entries (device uint64 key / count / min image / max image arrays; key
+ * QK_QSKETCH_EMPTY is skipped), adding counts and taking min / max, and counts newly claimed slots in ctrl[0].  The caller
+ * keeps ctrl[0] + n <= capacity / 2.
+ * Errors: k < 1, a length != nrows, a bad dtype, a capacity that is not a power of two in [QK_QSKETCH_MIN_CAPACITY, 2^31],
+ * null table / ctrl, an ntiles that does not match: QK_ERR_INVALID; a validity bitmap, more than 2^31 - 1 tiles:
+ * QK_ERR_UNSUPPORTED; a small workspace, n > capacity / 2 in a merge: QK_ERR_CAPACITY. */
+#define QK_QSKETCH_SHIFT 42
+#define QK_QSKETCH_EMPTY 0xFFFFFFFFFFFFFFFFULL
+#define QK_QSKETCH_MIN_CAPACITY 4096
+#define QK_QSKETCH_TILE 2048
+typedef struct qk_qslot {
+    uint64_t key;
+    uint64_t count;
+    uint64_t min_image;
+    uint64_t max_image;
+} qk_qslot;
+QK_API size_t qk_qsketch_workspace_bytes(int32_t k);
+QK_API int qk_qsketch_update(const qk_column* cols, const uint8_t* const* valid, int32_t k, int64_t nrows, qk_qslot* table,
+                             int64_t capacity, uint64_t* ctrl, const int32_t* tiles, int64_t ntiles, int32_t* deferred,
+                             void* workspace, size_t ws_bytes, void* stream);
+QK_API int qk_qsketch_merge(const uint64_t* keys, const uint64_t* counts, const uint64_t* mins, const uint64_t* maxs, int64_t n,
+                            qk_qslot* table, int64_t capacity, uint64_t* ctrl, void* stream);
+
 /* ---- synthetic TPC-H-shaped / SIP-shaped columns, generated in HBM --------------------------
  * Bit-identical to oracle/tpch_gen.py (counter-based hash of (table, column, row)); lets bench.py hold
  * SF-100 (600 037 902 lineitem rows) resident without a 23 GB host copy.  `column` ids: see

@@ -137,6 +137,11 @@ _SIGNATURES = {
     "qk_gram": (C.c_int, [_P(qk_column), C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                           C.c_size_t, C.c_void_p]),
     "qk_gram_last_plan": (C.c_char_p, []),
+    "qk_qsketch_workspace_bytes": (C.c_size_t, [C.c_int32]),
+    "qk_qsketch_update": (C.c_int, [_P(qk_column), C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                    C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "qk_qsketch_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                   C.c_void_p]),
     "qk_synth_column": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_int64), C.c_int64, C.c_int64, C.c_void_p,
                                   C.c_int32, C.c_void_p]),
     "qk_parquet_walk_chunk": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

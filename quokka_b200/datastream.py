@@ -769,6 +769,48 @@ class DataStream:
         global mean at the end.  An empty stream gives NaN."""
         return self._gram_stream(list(columns), {"shift_first_row": True}, "covariance").collect()
 
+    def approximate_quantile(self, columns, quantiles, sample_factor=1):
+        """Approximate quantiles of `columns` (pyquokka/datastream.py:921-1031): a DataStream with schema `columns`, all fp64,
+        and len(quantiles) rows, row i = quantile i in the order given.  `quantiles` is a float or a list of floats in [0, 1].
+
+        Target: Polars' quantile(q) with interpolation "nearest" (the reference's materialised branch): drop NULLs, sort the n
+        values ascending with NaN last, take element round-half-away((n - 1) q).  Every value is widened to fp64 and kept in a
+        sketch built on the device by qk_qsketch_update in one pass: per bucket of values sharing sign, exponent and the top
+        10 mantissa bits, the count, the smallest and the largest value.  The bucket holding the target rank answers (its
+        smallest value at its first rank, its largest at its last, otherwise its midpoint clamped to what it holds).
+        Guarantee:
+          - the result lies in the target's bucket, so |result - target| <= 2^-11 |target| for a normal target;
+          - it equals the target when that bucket holds one distinct value: +-0, +-inf, NaN, integers of magnitude < 2048;
+          - q = 0 and q = 1 give the exact minimum and maximum;
+          - it depends only on the multiset of values: batch splits, channels and ranks give bit-identical answers.
+        Two deviations from the reference: the per-rank sketches are merged exactly, where the reference averages the
+        per-channel t-digest answers (so its result depends on how the rows were split); and `sample_factor` (0 < f <= 1) is
+        checked but every row is counted, since sampling saves nothing in a single memory-bound pass and would make the
+        answer random.  Integer, float and boolean columns; string and date / time columns raise.  A column without non-NULL
+        rows (or an empty stream) gives NULL."""
+        from .executors import QUANTILE_ENTRY_COLUMNS, QuantileFinalExecutor, QuantilePartialExecutor
+        assert type(quantiles) == float or type(quantiles) == list, "quantiles must be a float or a list"
+        if type(quantiles) == float:
+            quantiles = [quantiles]
+        assert len(quantiles) > 0, "quantiles must not be empty"
+        for q in quantiles:
+            assert type(q) in (float, int) and 0 <= q <= 1, "quantile must be between 0 and 1"
+        assert 0 < sample_factor <= 1, "sample_factor must be in (0, 1]"
+        columns = list(columns)
+        assert len(columns) > 0, "columns must be a non-empty list"
+        assert len(set(columns)) == len(columns), "columns must be distinct"
+        for c in columns:
+            assert c in self.schema, f"column {c} not in schema"
+        part = StatefulNode({0: self.node}, QuantilePartialExecutor(columns), list(QUANTILE_ENTRY_COLUMNS), {0: set(columns)},
+                            {0: PassThroughPartitioner()}, CustomChannelsStrategy(1))
+        node = StatefulNode({0: part}, QuantileFinalExecutor(columns, quantiles), columns, {0: set(QUANTILE_ENTRY_COLUMNS)},
+                            {0: BroadcastPartitioner()}, SingleChannelStrategy())
+        return DataStream(self.quokka_context, node)
+
+    def approximate_median(self, columns, sample_factor=1):
+        """approximate_quantile(columns, 0.5, sample_factor) (pyquokka/datastream.py:905-919): one row."""
+        return self.approximate_quantile(columns, 0.5, sample_factor)
+
     def __repr__(self):
         return "DataStream[" + ",".join(self.schema) + "]"
 

@@ -682,6 +682,84 @@ class GramFinalExecutor(Executor):
         return self.state
 
 
+# ---------------------------------------------------------------------------------------------- quantile sketch
+QUANTILE_ENTRY_COLUMNS = ["__qkey", "__qcount", "__qmin", "__qmax"]
+
+
+def _quantile_input(col: DeviceColumn, name: str) -> tuple[torch.Tensor, torch.Tensor | None]:
+    """(values, row mask or None) of a column as qk_qsketch_update reads it.  Numbers only, as for the Gram matrix: string
+    (dictionary) and date / time columns raise.  Booleans and uint8 flags count as 0 / 1.  A NULL (right side of a left / as-of
+    join) is not counted: its validity mask becomes the kernel's row mask."""
+    if col.dictionary is not None:
+        raise L.QkError(f"approximate_quantile: column {name!r} is a string column")
+    if col.arrow_type is not None and not pa.types.is_boolean(col.arrow_type):
+        raise L.QkError(f"approximate_quantile: column {name!r} has type {col.arrow_type}, not a number")
+    t = col.data
+    if t.dtype == torch.bool:
+        t = t.view(torch.uint8)
+    elif t.dtype not in (torch.float64, torch.float32, torch.int64, torch.int32, torch.uint8):
+        t = t.to(torch.int32)
+    valid = None if col.valid is None else col.valid.to(torch.uint8).contiguous()
+    return t.contiguous(), valid
+
+
+class QuantilePartialExecutor(Executor):
+    """Per-rank phase of DataStream.approximate_quantile (pyquokka/datastream.py:905-1031, where each channel feeds a host
+    t-digest): every batch is folded into one QuantileSketch by qk_qsketch_update.  done() emits the sketch's entries as four
+    int64 columns (key, count, min image, max image)."""
+
+    silent_streams = "all"       # execute() only accumulates; the entries leave in done()
+
+    def __init__(self, columns) -> None:
+        self.columns = list(columns)
+        self.state = None
+
+    def execute(self, batches, stream_id, executor_id):
+        for b in _clean(batches):
+            ins = [_quantile_input(b[c], c) for c in self.columns]
+            if self.state is None:
+                self.state = ops.QuantileSketch(len(self.columns), b.device)
+            masks = [v for _, v in ins]
+            self.state.update([t for t, _ in ins], None if all(m is None for m in masks) else masks)
+
+    def done(self, executor_id):
+        if self.state is None:
+            return None
+        return DeviceTable({n: DeviceColumn(t) for n, t in zip(QUANTILE_ENTRY_COLUMNS, self.state.entries())})
+
+
+class QuantileFinalExecutor(Executor):
+    """Final phase of DataStream.approximate_quantile on one channel: merges the entries of every rank into one sketch by
+    qk_qsketch_merge (the merged state is the sketch of all the rows, whatever the split) and emits one fp64 row per
+    quantile, in the order given, with the schema `columns`.  A column without counted rows is NULL."""
+
+    silent_streams = "all"       # the quantiles leave in done()
+
+    def __init__(self, columns, quantiles) -> None:
+        self.columns = list(columns)
+        self.quantiles = [float(q) for q in quantiles]
+        self.parts = []
+        self.state = None
+
+    def execute(self, batches, stream_id, executor_id):
+        for b in _clean(batches):
+            self.parts.append([b[c].data for c in QUANTILE_ENTRY_COLUMNS])
+
+    def done(self, executor_id):
+        k = len(self.columns)
+        dev = self.parts[0][0].device if self.parts else default_device()
+        sk = ops.QuantileSketch(k, dev, capacity=4 * sum(p[0].numel() for p in self.parts))
+        for p in self.parts:
+            sk.merge(*p)
+        vals, valid = sk.quantiles(self.quantiles)
+        cols = {}
+        for j, c in enumerate(self.columns):
+            ok = valid[:, j]
+            cols[c] = DeviceColumn(vals[:, j].contiguous(), valid=None if bool(ok.all()) else ok.to(torch.uint8).contiguous())
+        self.state = DeviceTable(cols)
+        return self.state
+
+
 # ---------------------------------------------------------------------------------------------- as-of
 class SortedAsofExecutor(Executor):
     """ts_executors.py:324-383: streaming backward as-of join of two time-sorted streams per symbol.

@@ -527,6 +527,138 @@ def gram_last_plan() -> str:
     return L.lib().qk_gram_last_plan().decode()
 
 
+# ------------------------------------------------------------------ K10 quantile sketch
+QSKETCH_SHIFT, QSKETCH_TILE, QSKETCH_MIN_CAPACITY = 42, 2048, 4096          # include/qk.h QK_QSKETCH_*
+_SIGN = -(1 << 63)                                                           # int64 with only the sign bit set
+
+
+def _pow2_at_least(n: int) -> int:
+    return 1 << max(0, int(n) - 1).bit_length()
+
+
+def qsketch_quantiles(keys, counts, mins, maxs, k: int, qs) -> tuple[torch.Tensor, torch.Tensor]:
+    """Quantiles `qs` of the k columns of a compacted sketch (any order of entries; min / max are raw images stored in int64):
+    (fp64 [len(qs), k] values, bool [len(qs), k] valid).  Target rank of q among the n counted rows of a column:
+    round-half-away((n - 1) q), the `nearest` rule of Polars' quantile.  The bucket that holds that rank answers: its min when
+    the rank is the bucket's first, its max when it is the last, otherwise the bucket's middle image clamped to [min, max].
+    A column with no counted row is not valid (NULL)."""
+    dev = keys.device
+    nq = len(qs)
+    if keys.numel() == 0:
+        return torch.full((nq, k), float("nan"), dtype=torch.float64, device=dev), torch.zeros(nq, k, dtype=torch.bool, device=dev)
+    order = torch.argsort(keys)
+    keys, counts = keys[order], counts[order]
+    smin, smax = mins[order] ^ _SIGN, maxs[order] ^ _SIGN                  # order-preserving as signed int64
+    col = keys >> 22
+    cum = torch.cumsum(counts, 0)
+    n = torch.zeros(k, dtype=torch.int64, device=dev).index_add_(0, col, counts)
+    base = torch.cumsum(n, 0) - n
+    q = torch.tensor([float(x) for x in qs], dtype=torch.float64, device=dev)
+    x = (n.to(torch.float64) - 1)[None, :] * q[:, None]                       # (n - 1) q in fp64, as Polars computes it
+    f = torch.floor(x)
+    r = (f + (x - f >= 0.5).to(torch.float64)).to(torch.int64)               # x - floor(x) is exact: round half away from zero
+    valid = (n > 0)[None, :].expand(nq, k)
+    target = torch.where(valid, base[None, :] + r, torch.zeros_like(r))
+    idx = torch.searchsorted(cum, target, right=True).clamp_max(keys.numel() - 1)
+    hi = cum[idx] - 1
+    lo = hi - counts[idx] + 1
+    mn, mx = smin[idx], smax[idx]
+    mid = ((keys[idx] & ((1 << 22) - 1)) - (1 << 21)) * (1 << QSKETCH_SHIFT) + (1 << (QSKETCH_SHIFT - 1))
+    s = torch.where(target == lo, mn, torch.where(target == hi, mx, torch.minimum(torch.maximum(mid, mn), mx)))
+    bits = torch.where(s >= 0, s, (~s) ^ _SIGN)
+    return torch.where(valid, bits.view(torch.float64), float("nan")), valid.clone()
+
+
+class QuantileSketch:
+    """Device quantile sketch of k columns (qk_qsketch_update / qk_qsketch_merge): an open-addressed table of
+    [capacity, 4] int64 slots (key, count, min image, max image) and its control words.  update() folds a batch in, growing
+    the table and re-running the tiles the kernel deferred until every tile is counted; entries() compacts the occupied
+    slots; quantiles(qs) answers from them.  rounds / grows count the deferral rounds and table growths."""
+
+    def __init__(self, k: int, device, capacity: int = 1 << 16):
+        self.k = int(k)
+        if self.k < 1:
+            raise L.QkError("QuantileSketch: k must be >= 1")
+        self.device = torch.device(device)
+        self.ctrl = torch.zeros(4, dtype=torch.int64, device=self.device)
+        self._alloc(max(QSKETCH_MIN_CAPACITY, _pow2_at_least(capacity)))
+        self.ws = _ws(L.lib().qk_qsketch_workspace_bytes(self.k), self.device)
+        self.rounds = self.grows = 0
+        self.ctas = 2 * torch.cuda.get_device_properties(self.device).multi_processor_count   # CTAs resident at once
+
+    def _alloc(self, capacity: int):
+        self.capacity = capacity
+        self.table = torch.empty(capacity, 4, dtype=torch.int64, device=self.device)
+        self.table[:, 0] = -1                                                  # QK_QSKETCH_EMPTY
+        self.table[:, 1] = 0
+        self.table[:, 2] = -1                                                  # min image ~0
+        self.table[:, 3] = 0
+        self.ctrl[0] = 0
+
+    def _run(self, columns, valid, n, tiles, ntiles):
+        deferred = torch.empty(max(1, ntiles), dtype=torch.int32, device=self.device)
+        vp = None
+        if valid is not None:
+            vp = C.cast((C.c_void_p * self.k)(*[None if v is None else v.data_ptr() for v in valid]), C.c_void_p)
+        L.check(L.lib().qk_qsketch_update(cols(columns, "quantile column"), vp, self.k, n, self.table.data_ptr(), self.capacity,
+                                          self.ctrl.data_ptr(), None if tiles is None else tiles.data_ptr(), ntiles,
+                                          deferred.data_ptr(), self.ws.data_ptr(), self.ws.numel(), _stream()), "qk_qsketch_update")
+        occupied, ndef, overflow, _ = self.ctrl.tolist()                      # the one read of the batch
+        if overflow:
+            raise L.QkError("qk_qsketch_update: a probe ran through the whole table")
+        return occupied, ndef, deferred
+
+    def update(self, columns: Sequence[torch.Tensor], valid: Sequence[torch.Tensor | None] | None = None):
+        if len(columns) != self.k:
+            raise L.QkError(f"QuantileSketch.update: {len(columns)} columns for a {self.k}-column sketch")
+        if valid is not None:
+            if len(valid) != self.k:
+                raise L.QkError("QuantileSketch.update: one row mask (or None) per column")
+            for v in valid:
+                if v is not None:
+                    _require_cuda(v, "quantile row mask")
+                    if v.dtype != torch.uint8 or v.numel() != columns[0].numel():
+                        raise L.QkError("QuantileSketch.update: a row mask is uint8 with one byte per row")
+        n = columns[0].numel()
+        if n == 0:
+            return
+        ntiles = self.k * ((n + QSKETCH_TILE - 1) // QSKETCH_TILE)
+        occupied, ndef, deferred = self._run(columns, valid, n, None, ntiles)
+        while ndef:
+            self.rounds += 1
+            pending = deferred[:ndef].clone()
+            need = occupied + min(ndef, self.ctas) * QSKETCH_TILE               # room for one wave of new tiles
+            if 2 * need > self.capacity:
+                self.grow(_pow2_at_least(4 * need))
+            occupied, ndef, deferred = self._run(columns, valid, n, pending, ndef)
+
+    def grow(self, capacity: int):
+        """Re-insert every entry into a table of `capacity` slots."""
+        keys, counts, mins, maxs = self.entries()
+        self._alloc(capacity)
+        self.merge(keys, counts, mins, maxs)
+        self.grows += 1
+
+    def merge(self, keys, counts, mins, maxs):
+        """Fold compacted entries (int64 tensors, raw images) in: the final merge of the ranks."""
+        n = keys.numel()
+        if 2 * (int(self.ctrl[0]) + n) > self.capacity:
+            self.grow(_pow2_at_least(4 * (int(self.ctrl[0]) + n)))
+        if n == 0:
+            return
+        ks, cs, lo, hi = (t.contiguous() for t in (keys, counts, mins, maxs))
+        L.check(L.lib().qk_qsketch_merge(ks.data_ptr(), cs.data_ptr(), lo.data_ptr(), hi.data_ptr(), n, self.table.data_ptr(),
+                                         self.capacity, self.ctrl.data_ptr(), _stream()), "qk_qsketch_merge")
+
+    def entries(self):
+        """(key, count, min image, max image) of the occupied slots, int64 tensors in table order."""
+        t = self.table[self.table[:, 0] != -1]
+        return t[:, 0].contiguous(), t[:, 1].contiguous(), t[:, 2].contiguous(), t[:, 3].contiguous()
+
+    def quantiles(self, qs):
+        return qsketch_quantiles(*self.entries(), self.k, qs)
+
+
 # ------------------------------------------------------------------ Parquet column chunks -> Arrow-layout columns
 PQ_PAD = 16      # readable bytes the decoder may touch past the last encoded byte (aligned 8-byte windows)
 
