@@ -14,6 +14,8 @@ import torch
 from . import _lib as L
 from . import expr as E
 from . import ops
+# host arithmetic, the same whichever kernel backend `ops` names: imported by name, not looked up through `ops`
+from .ops import dense_agg_fits
 from .columns import DeviceColumn, DeviceTable
 from .target_info import (BroadcastPartitioner, FunctionPartitioner, HashPartitioner, PassThroughPartitioner,
                           RangePartitioner)
@@ -282,7 +284,7 @@ class PartialAgg:
             for e in key_exprs:
                 n_groups *= max(1, len(t[e.value].dictionary))
         value_aggs = [(op, e, name) for op, e, name in vals if op != "count"]
-        if dense and n_groups <= 1024 and len(value_aggs) <= L.MAX_AGGS:
+        if dense and dense_agg_fits(n_groups, len(value_aggs)):
             return self._dense(t, edge, key_exprs, vals, value_aggs, n_groups)
         if key_exprs and _single_process():
             return self._rows(t, edge, key_exprs, vals, value_aggs)
@@ -366,7 +368,7 @@ class PartialAgg:
         st.update([sub[c].data for c in used], pred, [sch[e.value].slot for e in key_exprs],
                   [E.compile_expr(e, sch) for _, e, _ in value_aggs])
         self.last_path = ops.last_variant()
-        acc, cnt = st.acc.cpu().numpy(), st.cnt.cpu().numpy()        # <= 1024 groups: tiny
+        acc, cnt = st.acc.cpu().numpy(), st.cnt.cpu().numpy()        # <= 200 groups (dense_agg_fits): tiny
         live = np.nonzero(cnt > 0)[0]
         if len(live) == 0:
             return None

@@ -159,6 +159,21 @@ def scan_filter_project(columns: Sequence[torch.Tensor], pred: Program | None, p
 
 
 # ------------------------------------------------------------------ K1+K2 dense aggregate
+DENSE_MAX_GROUPS = 4096            # csrc/scan.cu qk_scan_filter_agg_dense: more groups is QK_ERR_UNSUPPORTED
+DENSE_GENERIC_SMEM = 200 * 1024    # csrc/scan.cu: the interpreter's lane-private states, ng * (nagg * 8 + 4) * 256 B
+
+
+def dense_agg_fits(n_groups: int, nagg: int) -> bool:
+    """Whether qk_scan_filter_agg_dense takes `n_groups` groups x `nagg` value aggregates whatever the expressions are:
+    the bound of its postfix interpreter (variant 1), the one path that runs every program.  Under the default variant a
+    fused plan that does not fit falls back to the interpreter, so a grouping inside this bound never fails for lack of
+    shared memory.  Deliberately conservative: some groupings only the runtime-described plan could hold (about 67-140
+    groups for one SUM) fail here too; they belong to the hash aggregate, like every grouping outside the bound."""
+    n_groups, nagg = int(n_groups), int(nagg)
+    return (1 <= n_groups <= DENSE_MAX_GROUPS and 0 <= nagg <= L.MAX_AGGS
+            and n_groups * (nagg * 8 + 4) * 256 <= DENSE_GENERIC_SMEM)
+
+
 class DenseAggState:
     """Running state of a dense (dictionary-key) aggregate: acc[n_groups, nagg] fp64 + cnt[n_groups]."""
 

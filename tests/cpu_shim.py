@@ -149,9 +149,9 @@ class DenseAggState:
 
     def update(self, columns, pred, group_cols, agg_exprs, variant=0):
         E.check_call(len(columns), pred, agg_exprs, "scan_filter_agg_dense")
-        if len(group_cols) > 4 or len(self.agg_ops) > L.MAX_AGGS or self.n_groups > 4096:
+        if len(group_cols) > 4 or len(self.agg_ops) > L.MAX_AGGS or self.n_groups > real_ops.DENSE_MAX_GROUPS:
             raise L.QkError("scan_filter_agg_dense: ngroup_cols / nagg / groups out of range")
-        if self.n_groups * (len(self.agg_ops) * 8 + 4) * 256 > 200 * 1024:
+        if not real_ops.dense_agg_fits(self.n_groups, len(self.agg_ops)):
             raise L.QkError("scan_filter_agg_dense: groups x aggregates exceed the shared-memory dense path")
         cols = [c.numpy() for c in columns]
         n = len(cols[0]) if cols else 0
@@ -159,7 +159,7 @@ class DenseAggState:
         g = np.zeros(n, dtype=np.int64)
         for k, gc in enumerate(group_cols):
             g = g * self.group_card[k] + cols[gc].astype(np.int64)
-        g = g[mask]
+        g = np.clip(g[mask], 0, self.n_groups - 1)            # the kernels clamp a group id outside the dense range
         seen = self.cnt.numpy() > 0
         self.cnt += _t(np.bincount(g, minlength=self.n_groups).astype(np.int64))
         acc = self.acc.numpy()
@@ -168,9 +168,11 @@ class DenseAggState:
             if op == L.AGG_SUM:
                 acc[:, j] += np.bincount(g, weights=v, minlength=self.n_groups)
             else:
+                # the kernels combine with fmin / fmax (csrc/scan.cu agg_combine): a NaN value is skipped, not propagated
+                f = np.fmin if op == L.AGG_MIN else np.fmax
                 cur = np.full(self.n_groups, np.inf if op == L.AGG_MIN else -np.inf)
-                (np.minimum if op == L.AGG_MIN else np.maximum).at(cur, g, v)
-                acc[:, j] = np.where(seen, (np.minimum if op == L.AGG_MIN else np.maximum)(acc[:, j], cur), cur)
+                f.at(cur, g, v)
+                acc[:, j] = np.where(seen, f(acc[:, j], cur), cur)
         _last["variant"] = "shim-dense"
 
 
