@@ -475,9 +475,28 @@ class SQLAggExecutor(Executor):
         return result
 
 
+_SIGN = np.uint64(1 << 63)
+
+
+def order_image(v: np.ndarray, descending: bool) -> np.ndarray:
+    """uint64 image of a sort column whose ascending order is the ORDER BY order (DESIGN.md section 2), the image
+    csrc/topk.cu image_of() selects on: integers exact over their full range, -0.0 = +0.0, every NaN after +inf.
+    DESC is the bitwise complement, which is monotone and cannot overflow (negating INT64_MIN does)."""
+    if v.dtype.kind == "f":
+        with np.errstate(invalid="ignore"):                       # a signalling NaN stays a NaN
+            b = (v.astype(np.float64) + 0.0).view(np.uint64)     # + 0.0 folds -0.0 onto +0.0
+        img = np.where(b >> np.uint64(63) != 0, ~b, b | _SIGN)
+        img[np.isnan(v)] = ~np.uint64(0)
+    elif v.dtype.kind == "i":
+        img = v.astype(np.int64).view(np.uint64) ^ _SIGN
+    else:
+        img = v.astype(np.uint64)
+    return ~img if descending else img
+
+
 def sort_table(t: DeviceTable, by: list, descending: list, limit: int | None = None) -> DeviceTable:
     """ORDER BY of a (small) result on the host index space: the order is computed from the few sort
-    columns, the rows are moved by the gather kernel."""
+    columns, the rows are moved by the gather kernel.  NULL (valid == 0) sorts last in both directions."""
     if len(t) == 0:
         return t
     keys = []
@@ -487,7 +506,12 @@ def sort_table(t: DeviceTable, by: list, descending: list, limit: int | None = N
         if col.dictionary is not None:                     # order by the string value, not by the code
             rank = np.argsort(np.argsort(np.array(col.dictionary, dtype=object)))
             v = rank[v]
-        keys.append(-v.astype(np.float64) if (d and v.dtype.kind == "f") else (-v.astype(np.int64) if d else v))
+        img = order_image(v, d)
+        if col.valid is not None:
+            null = col.valid.cpu().numpy() == 0
+            keys.append(null)                              # NULLS LAST; NULLs tie with each other
+            img[null] = 0
+        keys.append(img)
     order = np.lexsort(keys[::-1])
     if limit is not None:
         order = order[:limit]
@@ -499,14 +523,23 @@ _TOPK_RE = re.compile(r"^\s*select\s+\*\s+from\s+batch_arrow\s+order\s+by\s+(.+?
 
 def top_k_table(t: DeviceTable, by: list, descending: list, k: int) -> DeviceTable:
     """Radix-select candidates on the primary sort column (qk_topk_candidates), then order the few
-    survivors on all sort columns."""
+    survivors on all sort columns.  Rows whose primary value is NULL come after every valid row: they are
+    left out of the select, and only when fewer than k valid rows exist are the best of them appended."""
     if len(t) == 0:
         return t
     primary = t[by[0]]
     if primary.dictionary is not None or len(t) <= 4096:         # a few rows: ordering them on the host beats ~20 select launches
         return sort_table(t, by, descending, k)
-    idx = ops.topk_candidates(primary.data, k, descending[0])
-    return sort_table(t.gather(idx), by, descending, k)
+    if primary.valid is None:
+        return sort_table(t.gather(ops.topk_candidates(primary.data, k, descending[0])), by, descending, k)
+    valid = primary.valid.bool()
+    vidx = torch.nonzero(valid).flatten().to(torch.int32)
+    if len(vidx) >= k:
+        cand = vidx[ops.topk_candidates(ops.gather([primary.data], vidx)[0], k, descending[0]).long()]
+        return sort_table(t.gather(cand), by, descending, k)
+    nulls = t.gather(torch.nonzero(~valid).flatten().to(torch.int32))
+    rest = top_k_table(nulls, by[1:], descending[1:], k - len(vidx)) if len(by) > 1 else nulls.slice(0, k - len(vidx))
+    return sort_table(concat_tables([t.gather(vidx), rest]), by, descending, k)
 
 
 class ConcatThenSQLExecutor(Executor):

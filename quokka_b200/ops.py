@@ -246,6 +246,9 @@ class HashAggState:
         return int(self.desc.capacity)
 
     def update(self, keys: Sequence[torch.Tensor], vals: Sequence[torch.Tensor]):
+        if len(keys) != self.desc.nkeys or len(vals) != self.desc.nagg:       # the C side reads nkeys / nagg columns
+            raise L.QkError(f"hash aggregate: {len(keys)} key / {len(vals)} value columns for a state of "
+                            f"{self.desc.nkeys} / {self.desc.nagg}")
         n = keys[0].numel()
         self.rows_seen += n
         L.check(L.lib().qk_hashagg_update(C.byref(self.desc), self.state.data_ptr(), cols(keys, "key"),

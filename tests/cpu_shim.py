@@ -12,6 +12,7 @@ from oracle import relops as R
 from quokka_b200 import _lib as L
 from quokka_b200 import expr as E
 from quokka_b200 import ops as real_ops
+from quokka_b200.executors import order_image
 
 qk_dtype = real_ops.qk_dtype
 is_passthrough = real_ops.is_passthrough
@@ -191,16 +192,23 @@ class HashAggState:
 
     def finalize(self, max_groups=None):
         nk = len(self.key_dtypes)
-        keys = {f"k{i}": np.concatenate([b[i] for b in self.keys]) if self.keys else np.zeros(0) for i in range(nk)}
-        aggs = {}
+        keys = [np.concatenate([b[i] for b in self.keys]) if self.keys else np.zeros(0) for i in range(nk)]
+        gid, uniq = R.group_ids(keys)
+        ng = len(uniq[0])
+        if max_groups is not None and ng > max_groups:
+            raise L.QkError(f"hash aggregate produced {ng} groups but the output was sized for {max_groups}")
+        ov = []
         for j, op in enumerate(self.agg_ops):
             v = np.concatenate([b[j] for b in self.vals]) if self.vals else np.zeros(0)
-            aggs[f"v{j}"] = ({L.AGG_SUM: "sum", L.AGG_MIN: "min", L.AGG_MAX: "max"}[op], v)
-        aggs["n"] = ("count", None)
-        out = R.group_aggregate(keys, aggs)
-        ok = [_t(out[f"k{i}"].astype(keys[f"k{i}"].dtype)) for i in range(nk)]
-        ov = [_t(out[f"v{j}"]) for j in range(len(self.agg_ops))]
-        return ok, ov, _t(out["n"])
+            if op == L.AGG_SUM:
+                ov.append(_t(np.bincount(gid, weights=v, minlength=ng)))
+                continue
+            # csrc/hashagg.cu atomic_minmax: a NaN value never replaces the accumulator, which starts at +inf / -inf
+            acc = np.full(ng, np.inf if op == L.AGG_MIN else -np.inf)
+            (np.fmin if op == L.AGG_MIN else np.fmax).at(acc, gid, v)
+            ov.append(_t(acc))
+        ok = [_t(u.astype(k.dtype)) for u, k in zip(uniq, keys)]
+        return ok, ov, _t(np.bincount(gid, minlength=ng).astype(np.int64))
 
 
 PART_MOD_MAX_PARTS = 16_384              # csrc/partition.cu: MOD partitions keep their per-chunk histogram in shared memory
@@ -313,12 +321,14 @@ def window_session_ids(time, by, timeout):
 
 
 def topk_candidates(key, k, descending):
+    if k <= 0:
+        raise L.QkError("qk_topk_candidates: k must be positive")
     v = key.numpy()
     if len(v) <= k:
         return _t(np.arange(len(v), dtype=np.int32))
-    s = np.sort(v)
-    kth = s[-k] if descending else s[k - 1]
-    return _t(np.nonzero(v >= kth if descending else v <= kth)[0].astype(np.int32))
+    img = order_image(v, not descending)                   # csrc/topk.cu image_of: the best rows have the largest image
+    kth = np.sort(img)[-k]
+    return _t(np.nonzero(img >= kth)[0].astype(np.int32))
 
 
 PQ_PAD = real_ops.PQ_PAD
