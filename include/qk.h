@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define QK_VERSION 100
+#define QK_VERSION 100    /* qk_column.lanes took the place of the always-zero `reserved` word, and 0 keeps its meaning */
 #define QK_API __attribute__((visibility("default")))
 
 /* ---- error codes ---- */
@@ -39,13 +39,17 @@ extern "C" {
 #define QK_I64 3    /* int64 */
 #define QK_F32 4
 #define QK_F64 5
+#define QK_F16 6    /* IEEE half: vector columns only (lanes > 1) */
 
 typedef struct qk_column {
     const void* data;        /* device */
     const uint8_t* validity; /* must be NULL */
     int64_t length;
-    int32_t dtype;           /* QK_U8 .. QK_F64 */
-    int32_t reserved;
+    int32_t dtype;           /* QK_U8 .. QK_F16 */
+    int32_t lanes;           /* 0 or 1: scalar column.  > 1: a fixed-width vector column of `length` rows, each `lanes`
+                              * contiguous elements of `dtype` (row-major, row i at data + i * lanes * size(dtype)).
+                              * Only qk_gather, qk_xchg_push, qk_xchg_recv and qk_knn_topk take lanes > 1; every other
+                              * entry point returns QK_ERR_UNSUPPORTED for such a column, and for QK_F16. */
 } qk_column;
 
 /* ---- expression programs (postfix), the subset of pyquokka/sql_utils.py:86-223 `evaluate`
@@ -256,7 +260,9 @@ QK_API int qk_scatter_peer(const qk_column* cols, int32_t ncols, const int32_t* 
  *   dest[i] (qk_partition_plan's output), at element (dest[i] - part_offsets[rank]) from dst_byte_off; a tile of rows
  *   is ordered by destination in shared memory and leaves as one coalesced run per destination.
  * qk_xchg_recv: waits until every peer's rows of this epoch have landed, then copies column c (out[c].length
- *   elements from byte offset src_byte_off[c] of the own mailbox, 16-byte aligned) into out[c]. */
+ *   rows from byte offset src_byte_off[c] of the own mailbox, 16-byte aligned) into out[c].
+ * A row of column c is size(dtype) * max(1, lanes) bytes: qk_xchg_push and qk_xchg_recv move vector columns (lanes > 1);
+ * qk_xchg_push_scatter returns QK_ERR_UNSUPPORTED for them. */
 #define QK_XCHG_META_WORDS 48
 #define QK_XCHG_CTRL_BYTES 16384
 typedef struct qk_xchg {
@@ -274,7 +280,8 @@ QK_API int qk_xchg_push(const qk_xchg* x, uint64_t epoch, const qk_column* cols,
 QK_API int qk_xchg_push_scatter(const qk_xchg* x, uint64_t epoch, const qk_column* cols, int32_t ncols, const int32_t* dest,
                                 const int64_t* part_offsets, const int64_t* dst_byte_off, void* stream);
 QK_API int qk_xchg_recv(const qk_xchg* x, uint64_t epoch, const int64_t* src_byte_off, qk_column* out, int32_t ncols, void* stream);
-/* out[c][i] = cols[c][idx[i]] for i < n_idx; idx == -1 writes 0 (left join / as-of "no match") */
+/* out[c][i] = cols[c][idx[i]] for i < n_idx; idx == -1 writes 0 (left join / as-of "no match").  A vector column (lanes > 1)
+ * moves whole rows; out[c] must have the same dtype and lanes. */
 QK_API int qk_gather(const qk_column* cols, int32_t ncols, const int32_t* idx, int64_t n_idx, qk_column* out,
               void* stream);
 
@@ -423,6 +430,40 @@ QK_API int qk_qsketch_update(const qk_column* cols, const uint8_t* const* valid,
                              void* workspace, size_t ws_bytes, void* stream);
 QK_API int qk_qsketch_merge(const uint64_t* keys, const uint64_t* counts, const uint64_t* mins, const uint64_t* maxs, int64_t n,
                             qk_qslot* table, int64_t capacity, uint64_t* ctrl, void* stream);
+
+/* ---- K11: nearest neighbours by cosine similarity -------------------------------------------------
+ * Replaces the per-batch np.dot + argsort of DFProbeDataStreamNNExecutor1 (pyquokka/executors/vector_executors.py:8-52) behind
+ * DataStream.vector_nn_join.  x = one vector column (QK_F32 or QK_F16, lanes = d in [1, QK_KNN_MAX_DIM], length n rows);
+ * probes = device fp32 [q][d], already normalised (the host normalises in fp64 and rounds to fp32).  For every probe p the
+ * score of row i is s = (x_i . p) / ||x_i||; rows whose squared norm (fp64) is 0 or not finite -- zero rows, rows holding a NaN
+ * or an inf -- and non-finite scores never match.  Writes the k best rows of the call per probe,
+ * out_score[p * k + j] (f32) / out_row[p * k + j] (int64 row of x), in descending score, ties by smaller row; fewer than k
+ * valid rows leave row -1 and score -inf in the remaining slots.  1 <= k <= QK_KNN_MAX_K, q >= 1.
+ * One fused pass: rows are staged into shared memory by cp.async (16-byte copies when the column is 16-byte aligned and a row
+ * is a whole number of 16-byte units), dot products run on the tensor cores (mma.sync TF32, 3xTF32: x_lo p_hi + x_hi p_lo +
+ * x_hi p_hi with f32 accumulation; an f16 row is exact in TF32, so f16 rows take the two probe terms), the row's squared norm
+ * accumulates in fp64 from the same staged chunk, and each CTA keeps a per-probe top-k in shared memory (only scores above its
+ * current k-th enter); the per-CTA lists are folded in CTA order.  The n x q score matrix is never written.
+ * Error: |s - s64| <= (d + 8) * 2^-21, s64 the exact cosine of the stored values and the fp32 probe, for rows whose non-zero
+ * elements have magnitudes in [2^-80, 2^80] (the fp32 products and sums of the dot product stay normal and finite there);
+ * outside that range a score may be less accurate, and a row whose dot product overflows never matches.
+ * Determinism: a score is computed by the same sequence of operations (8-element MMA steps in element order with the three
+ * terms in a fixed order; the squared norm in fixed blocks of 16) whatever the row's position, the batch size, q, k or the grid,
+ * so it is bit-identical across batchings and ranks, and the output, a total order on (score, row), is bit-identical across
+ * calls.
+ * Workspace: qk_knn_workspace_bytes(n, d, q, k); the caller chunks large q to bound it.
+ * qk_knn_merge: per probe, the best k of two candidate lists a (q x ka) and b (q x kb), each sorted by the same rule with
+ * 64-bit keys (arrival order) in place of rows and key -1 after its last entry: descending score, ties by smaller key, ties
+ * of both by a.  out_src[p * k + j] = p * ka + i for a's entry i, q * ka + p * kb + i for b's, -1 for padding (key -1,
+ * score -inf).  Used across the batches of a rank and across ranks. */
+#define QK_KNN_MAX_DIM 4096
+#define QK_KNN_MAX_K 256
+QK_API size_t qk_knn_workspace_bytes(int64_t n, int32_t d, int32_t q, int32_t k);
+QK_API int qk_knn_topk(const qk_column* x, const float* probes, int32_t q, int32_t k, float* out_score, int64_t* out_row,
+                       void* workspace, size_t ws_bytes, void* stream);
+QK_API int qk_knn_merge(int32_t q, const float* a_score, const int64_t* a_key, int32_t ka, const float* b_score,
+                        const int64_t* b_key, int32_t kb, int32_t k, float* out_score, int64_t* out_key, int32_t* out_src,
+                        void* stream);
 
 /* ---- synthetic TPC-H-shaped / SIP-shaped columns, generated in HBM --------------------------
  * Bit-identical to oracle/tpch_gen.py (counter-based hash of (table, column, row)); lets bench.py hold

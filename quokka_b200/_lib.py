@@ -8,7 +8,8 @@ import os
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libqk.so")
 
-QK_U8, QK_I32, QK_I64, QK_F32, QK_F64 = 1, 2, 3, 4, 5
+QK_U8, QK_I32, QK_I64, QK_F32, QK_F64, QK_F16 = 1, 2, 3, 4, 5, 6
+KNN_MAX_DIM, KNN_MAX_K = 4096, 256
 (OP_COL, OP_CONST, OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_NEG, OP_LT, OP_LE, OP_GT, OP_GE, OP_EQ, OP_NE,
  OP_AND, OP_OR, OP_NOT, OP_CMP_COL_IMM, OP_CMP_COL_COL, OP_RINT, OP_IN_SET, OP_SELECT, OP_EXTRACT, OP_RANGE_COL_IMM) = range(1, 24)
 CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_EQ, CMP_NE = range(6)
@@ -32,7 +33,7 @@ class QkError(RuntimeError):
 
 class qk_column(C.Structure):
     _fields_ = [("data", C.c_void_p), ("validity", C.c_void_p), ("length", C.c_int64),
-                ("dtype", C.c_int32), ("reserved", C.c_int32)]
+                ("dtype", C.c_int32), ("lanes", C.c_int32)]
 
 
 class qk_expr_node(C.Structure):
@@ -142,6 +143,11 @@ _SIGNATURES = {
                                     C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "qk_qsketch_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                    C.c_void_p]),
+    "qk_knn_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
+    "qk_knn_topk": (C.c_int, [_P(qk_column), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                              C.c_void_p]),
+    "qk_knn_merge": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "qk_synth_column": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_int64), C.c_int64, C.c_int64, C.c_void_p,
                                   C.c_int32, C.c_void_p]),
     "qk_parquet_walk_chunk": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

@@ -4,7 +4,10 @@ A `DeviceTable` is what the reference passes around as `pyarrow.Table` / `polars
 (pyquokka/core.py:32-35,152-195) -- here each column is a contiguous torch CUDA tensor in Arrow's
 fixed-width layout (int64 / int32 / date32-as-int32 / float64 / float32 / uint8), and string columns are
 dictionary codes with the value list kept on the host (SURVEY.md section 7 "Strings").  Conversion to
-and from Arrow happens only at the edges (readers, collect())."""
+and from Arrow happens only at the edges (readers, collect()).
+
+A vector column (fixed_size_list / list of floats, the embeddings of DataStream.vector_nn_join) is a contiguous 2-D tensor
+(n, d) of float32 or float16, 1 <= d <= 4096."""
 from __future__ import annotations
 
 from dataclasses import dataclass
@@ -37,7 +40,11 @@ class DeviceColumn:
     valid: torch.Tensor | None = None       # uint8 mask, only ever produced by left / as-of joins ("no match")
 
     def __len__(self):
-        return self.data.numel()
+        return self.data.shape[0] if self.data.dim() == 2 else self.data.numel()
+
+    @property
+    def is_vector(self) -> bool:
+        return self.data.dim() == 2
 
     @property
     def qk_dtype(self) -> int:
@@ -158,7 +165,9 @@ class DeviceTable:
         arrays, names = [], []
         for n, c in self.columns.items():
             h = c.data.cpu().numpy()
-            if c.dictionary is not None:
+            if c.is_vector:
+                arr = pa.FixedSizeListArray.from_arrays(pa.array(h.reshape(-1)), h.shape[1])
+            elif c.dictionary is not None:
                 arr = pa.DictionaryArray.from_arrays(pa.array(h.astype(np.int32)), pa.array(c.dictionary, type=pa.string())).cast(pa.string())
             elif c.arrow_type is not None and pa.types.is_boolean(c.arrow_type):
                 arr = pa.array(h.astype(bool))
@@ -182,6 +191,8 @@ class DeviceTable:
         device = device or default_device()
         for n, v in cols.items():
             t = torch.from_numpy(np.ascontiguousarray(v)).to(device)
+            if t.dim() == 2 and not (t.dtype in (torch.float32, torch.float16) and 1 <= t.shape[1] <= MAX_VECTOR_DIM):
+                raise L.QkError(f"column {n!r}: a 2-D column must be float32 / float16 with 1 <= d <= {MAX_VECTOR_DIM}")
             out[n] = DeviceColumn(t, (dictionaries or {}).get(n), pa.date32() if n in dates else None)
         return DeviceTable(out)
 
@@ -205,7 +216,10 @@ def concat_tables(tables: list) -> DeviceTable:
         if any(p.valid is not None for p in parts):
             valid = torch.cat([p.valid if p.valid is not None else torch.ones(len(p), dtype=torch.uint8, device=p.data.device)
                                for p in parts])
-        out[n] = DeviceColumn(torch.cat([p.data for p in parts]), dic, parts[0].arrow_type, valid)
+        datas = [p.data for p in parts]
+        if any(x.dim() == 2 for x in datas):          # vector rows: an empty part may not know the row length
+            datas = [x for x in datas if x.shape[0] > 0] or datas[:1]
+        out[n] = DeviceColumn(torch.cat(datas), dic, parts[0].arrow_type, valid)
     return DeviceTable(out)
 
 
@@ -270,7 +284,54 @@ def _from_numpy(h):
         return torch.from_numpy(np.ascontiguousarray(h))
 
 
+MAX_VECTOR_DIM = 4096
+
+
+def is_vector_type(t: pa.DataType) -> bool:
+    return pa.types.is_fixed_size_list(t) or pa.types.is_list(t) or pa.types.is_large_list(t)
+
+
+def vector_columns(schema: pa.Schema) -> list:
+    """Names of the list-typed fields of an Arrow schema: the columns that load as vector columns."""
+    return [f.name for f in schema if is_vector_type(f.type)]
+
+
+def _vector_to_device(name, col, device) -> DeviceColumn:
+    """fixed_size_list<float32 | float16, d> is stored as it is; list / large_list<float*> whose rows all have one length are
+    accepted too, and float64 elements are rounded to float32 once, here (as DECIMAL becomes fp64 at the reader).  Ragged
+    lists, null rows or elements, non-float elements and d > 4096 raise."""
+    arr = col.combine_chunks() if isinstance(col, pa.ChunkedArray) else col
+    t = arr.type
+    vt = t.value_type
+    if not pa.types.is_floating(vt):
+        raise L.QkError(f"column {name!r}: vector elements must be floats, not {vt}")
+    if arr.null_count:
+        raise L.QkError(f"column {name!r}: a vector column cannot hold null rows")
+    n = len(arr)
+    if pa.types.is_fixed_size_list(t):
+        d = t.list_size
+        values = arr.values.slice(arr.offset * d, n * d)
+    else:
+        offs = arr.offsets.to_numpy(zero_copy_only=False).astype(np.int64)
+        lens = np.diff(offs)
+        d = int(lens[0]) if n else 0
+        if n and (lens != d).any():
+            raise L.QkError(f"column {name!r}: ragged list column (row lengths {int(lens.min())} .. {int(lens.max())}); vector columns need one length")
+        values = arr.values.slice(int(offs[0]) if n else 0, n * d)
+    if n and not 1 <= d <= MAX_VECTOR_DIM:
+        raise L.QkError(f"column {name!r}: vector dimension {d} outside [1, {MAX_VECTOR_DIM}]")
+    if values.null_count:
+        raise L.QkError(f"column {name!r}: a vector column cannot hold null elements")
+    h = values.to_numpy(zero_copy_only=False)
+    if h.dtype == np.float64:
+        h = h.astype(np.float32)
+    # an empty chunk of a variable-size list has no row length: (0, 1); concat_tables drops empty vector parts
+    return DeviceColumn(_from_numpy(h.reshape(n, d if (n or pa.types.is_fixed_size_list(t)) else 1)).to(device), None, None)
+
+
 def _arrow_to_device(name, col, device, dictionaries) -> DeviceColumn:
+    if is_vector_type(col.type):
+        return _vector_to_device(name, col, device)
     if isinstance(col, pa.ChunkedArray):
         if col.null_count:
             raise L.QkError(f"column {name!r} has nulls: validity bitmaps are not supported on the hot path")

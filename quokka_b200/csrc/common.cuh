@@ -39,17 +39,30 @@ static inline int dtype_size(int dt) {
         case QK_U8: return 1;
         case QK_I32: case QK_F32: return 4;
         case QK_I64: case QK_F64: return 8;
+        case QK_F16: return 2;
         default: return 0;
     }
 }
 static inline bool dtype_is_int(int dt) { return dt == QK_U8 || dt == QK_I32 || dt == QK_I64; }
 
-static inline int check_col(const qk_column* c, const char* what) {
+// a column of any row width: scalar (lanes 0 / 1) or vector (lanes > 1) -- for the kernels that only move rows
+static inline int check_rows_col(const qk_column* c, const char* what) {
     if (!c) QK_FAIL(QK_ERR_INVALID, "%s: null column", what);
     if (dtype_size(c->dtype) == 0) QK_FAIL(QK_ERR_INVALID, "%s: bad dtype %d", what, c->dtype);
+    if (c->lanes < 0 || c->lanes > QK_KNN_MAX_DIM) QK_FAIL(QK_ERR_INVALID, "%s: lanes %d out of range", what, (int)c->lanes);
     if (c->validity) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: validity bitmaps are not supported on the hot path", what);
     if (c->length < 0 || c->length > 0x7fffffffLL) QK_FAIL(QK_ERR_INVALID, "%s: length %lld out of range", what, (long long)c->length);
     if (c->length > 0 && !c->data) QK_FAIL(QK_ERR_INVALID, "%s: null data", what);
+    return 0;
+}
+static inline int row_lanes(const qk_column* c) { return c->lanes > 1 ? c->lanes : 1; }
+static inline long long row_bytes(const qk_column* c) { return (long long)dtype_size(c->dtype) * row_lanes(c); }
+
+// a scalar column: what every kernel that reads values takes
+static inline int check_col(const qk_column* c, const char* what) {
+    if (int rc = check_rows_col(c, what)) return rc;
+    if (c->lanes > 1) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: vector columns (lanes %d) are not supported here", what, (int)c->lanes);
+    if (c->dtype == QK_F16) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: f16 elements are only supported in vector columns", what);
     return 0;
 }
 

@@ -104,14 +104,25 @@ __global__ void __launch_bounds__(64) k_xchg_meta(const __grid_constant__ Chan C
 }
 
 // ---------------------------------------------------------------- push
+constexpr int X_NT = 256;
+constexpr int X_TILE = 2048;             // rows per tile
+
 struct PushArgs {
     const void* src[QK_MAX_COLS];
     unsigned long long dst[QK_MAX_PEERS][QK_MAX_COLS];   // peer-mapped address of the FIRST element this rank writes for (dest, column)
     long long send_lo[QK_MAX_PEERS], send_hi[QK_MAX_PEERS];   // contiguous mode: source row range per destination
     long long tile_base[QK_MAX_PEERS + 1];                    // contiguous mode: prefix sums of tiles per destination
-    int8_t width[QK_MAX_COLS];
+    int8_t width[QK_MAX_COLS];                                // element bytes
+    int32_t lanes[QK_MAX_COLS];                               // elements per row (1: scalar column)
     int32_t ncols;
 };
+
+template <class T>
+__device__ __forceinline__ void copy_rows(const void* src, void* dst, long long first_row, long long r0, long long n, int lanes) {
+    const T* s = (const T*)src + (first_row + r0) * lanes; T* o = (T*)dst + r0 * lanes;
+    const long long m = n * lanes;
+    for (long long i = threadIdx.x; i < m; i += X_NT) o[i] = s[i];
+}
 
 __device__ __forceinline__ void signal_data_landed(const Chan& C, XchgCtrl* mine) {
     // every thread's remote stores are ordered before the CTA's arrival; the last CTA to arrive releases the flags
@@ -127,9 +138,6 @@ __device__ __forceinline__ void signal_data_landed(const Chan& C, XchgCtrl* mine
     }
 }
 
-constexpr int X_NT = 256;
-constexpr int X_TILE = 2048;             // rows per tile
-
 // contiguous segments (broadcast / single owner / pre-grouped rows): tile -> (destination, row range)
 __global__ void __launch_bounds__(X_NT) k_xchg_push_contig(const __grid_constant__ Chan C, const __grid_constant__ PushArgs A) {
     XchgCtrl* mine = (XchgCtrl*)C.ctrl[C.me];
@@ -140,6 +148,15 @@ __global__ void __launch_bounds__(X_NT) k_xchg_push_contig(const __grid_constant
         const long long r0 = (tile - A.tile_base[d]) * X_TILE;             // row offset inside the segment
         const long long n = min((long long)X_TILE, A.send_hi[d] - A.send_lo[d] - r0);
         for (int c = 0; c < A.ncols; ++c) {
+            if (A.lanes[c] > 1 || A.width[c] == 2) {                      // vector column: whole rows, element by element
+                switch (A.width[c]) {
+                    case 1: copy_rows<uint8_t>(A.src[c], (void*)A.dst[d][c], A.send_lo[d], r0, n, A.lanes[c]); break;
+                    case 2: copy_rows<uint16_t>(A.src[c], (void*)A.dst[d][c], A.send_lo[d], r0, n, A.lanes[c]); break;
+                    case 4: copy_rows<uint32_t>(A.src[c], (void*)A.dst[d][c], A.send_lo[d], r0, n, A.lanes[c]); break;
+                    default: copy_rows<uint64_t>(A.src[c], (void*)A.dst[d][c], A.send_lo[d], r0, n, A.lanes[c]); break;
+                }
+                continue;
+            }
             switch (A.width[c]) {
                 case 1: {
                     const uint8_t* s = (const uint8_t*)A.src[c] + A.send_lo[d] + r0; uint8_t* o = (uint8_t*)A.dst[d][c] + r0;
@@ -290,14 +307,14 @@ extern "C" int qk_xchg_meta(const qk_xchg* x, uint64_t epoch, const int64_t* par
 }
 
 static int fill_push(PushArgs& A, const qk_xchg* x, const qk_column* cols, int32_t ncols, const int64_t* dst_byte_off,
-                     int64_t* nrows_out, const char* who) {
+                     int64_t* nrows_out, bool vectors_ok, const char* who) {
     if (ncols < 0 || ncols > QK_MAX_COLS) QK_FAIL(QK_ERR_INVALID, "%s: ncols out of range", who);
     if (ncols > 0 && (!cols || !dst_byte_off)) QK_FAIL(QK_ERR_INVALID, "%s: null columns / offsets", who);
     int64_t n = ncols > 0 ? cols[0].length : 0;
     for (int c = 0; c < ncols; ++c) {
-        if (int rc = check_col(&cols[c], who)) return rc;
+        if (int rc = vectors_ok ? check_rows_col(&cols[c], who) : check_col(&cols[c], who)) return rc;
         if (cols[c].length != n) QK_FAIL(QK_ERR_INVALID, "%s: column %d length mismatch", who, c);
-        A.src[c] = cols[c].data; A.width[c] = (int8_t)dtype_size(cols[c].dtype);
+        A.src[c] = cols[c].data; A.width[c] = (int8_t)dtype_size(cols[c].dtype); A.lanes[c] = row_lanes(&cols[c]);
     }
     for (int p = 0; p < x->world; ++p) {
         if (!x->mailbox[p]) QK_FAIL(QK_ERR_INVALID, "%s: mailbox of rank %d missing", who, p);
@@ -320,13 +337,13 @@ extern "C" int qk_xchg_push(const qk_xchg* x, uint64_t epoch, const qk_column* c
     if (int rc = fill_chan(C, x, epoch, who)) return rc;
     static thread_local PushArgs A;
     int64_t n = 0;
-    if (int rc = fill_push(A, x, cols, ncols, dst_byte_off, &n, who)) return rc;
+    if (int rc = fill_push(A, x, cols, ncols, dst_byte_off, &n, true, who)) return rc;
     long long tiles = 0;
     for (int p = 0; p < x->world; ++p) {
         const int64_t lo = (ncols > 0 && send_lo) ? send_lo[p] : 0, hi = (ncols > 0 && send_hi) ? send_hi[p] : 0;
         if (lo < 0 || hi < lo || hi > n) QK_FAIL(QK_ERR_INVALID, "%s: bad row range for rank %d", who, p);
         for (int c = 0; c < ncols; ++c)
-            if (dst_byte_off[(size_t)p * ncols + c] + (hi - lo) * A.width[c] > x->mailbox_bytes)
+            if (dst_byte_off[(size_t)p * ncols + c] + (hi - lo) * A.width[c] * A.lanes[c] > x->mailbox_bytes)
                 QK_FAIL(QK_ERR_CAPACITY, "%s: rows for rank %d do not fit its mailbox", who, p);
         A.send_lo[p] = lo; A.send_hi[p] = hi; A.tile_base[p] = tiles;
         tiles += (hi - lo + X_TILE - 1) / X_TILE;
@@ -347,7 +364,7 @@ extern "C" int qk_xchg_push_scatter(const qk_xchg* x, uint64_t epoch, const qk_c
     if (int rc = fill_chan(C, x, epoch, who)) return rc;
     static thread_local PushArgs A;
     int64_t n = 0;
-    if (int rc = fill_push(A, x, cols, ncols, dst_byte_off, &n, who)) return rc;
+    if (int rc = fill_push(A, x, cols, ncols, dst_byte_off, &n, false, who)) return rc;
     if (n > 0 && (!dest || !part_offsets)) QK_FAIL(QK_ERR_INVALID, "%s: null partition plan", who);
     long long nb = (n + X_TILE - 1) / X_TILE;
     if (nb < 1) nb = 1;
@@ -377,8 +394,8 @@ extern "C" int qk_xchg_recv(const qk_xchg* x, uint64_t epoch, const int64_t* src
     CopyArgs A;
     long long total = 0;
     for (int c = 0; c < ncols; ++c) {
-        if (int rc = check_col(&out[c], who)) return rc;
-        const long long bytes = out[c].length * dtype_size(out[c].dtype);
+        if (int rc = check_rows_col(&out[c], who)) return rc;
+        const long long bytes = out[c].length * row_bytes(&out[c]);
         if (src_byte_off[c] < 0 || (src_byte_off[c] & 15) || src_byte_off[c] + bytes > x->mailbox_bytes)
             QK_FAIL(QK_ERR_INVALID, "%s: column %d lies outside the mailbox or is misaligned", who, c);
         if (bytes > 0 && ((uintptr_t)out[c].data & 15)) QK_FAIL(QK_ERR_INVALID, "%s: output %d is not 16-byte aligned", who, c);

@@ -407,14 +407,52 @@ extern "C" int qk_scatter(const qk_column* cols, int32_t ncols, const int32_t* d
     return QK_OK;
 }
 
+// whole rows of a vector column: element j of output row i = element j of input row idx[i] (0 for idx -1)
+template <class T>
+__global__ void __launch_bounds__(256) k_gather_rows(const T* __restrict__ src, T* __restrict__ dst, const int32_t* idx, int64_t n, int lanes) {
+    const int64_t total = n * lanes;
+    for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t i = e / lanes, j = e - i * lanes;
+        const int64_t s = idx[i];
+        dst[e] = s < 0 ? T(0) : src[s * lanes + j];
+    }
+}
+
 extern "C" int qk_gather(const qk_column* cols, int32_t ncols, const int32_t* idx, int64_t n_idx, qk_column* out, void* stream) {
+    const char* who = "qk_gather";
     MoveArgs M;
     if (ncols == 0 || n_idx == 0) return QK_OK;
     if (!cols || !out || !idx || n_idx < 0) QK_FAIL(QK_ERR_INVALID, "qk_gather: bad arguments");
-    if (int rc = fill_move(M, cols, ncols, out, -1, n_idx, "qk_gather")) return rc;
+    if (ncols < 0 || ncols > QK_MAX_COLS) QK_FAIL(QK_ERR_INVALID, "%s: ncols out of range", who);
+    qk_column scal_in[QK_MAX_COLS], scal_out[QK_MAX_COLS];
+    int nscal = 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    for (int c = 0; c < ncols; ++c) {
+        if (int rc = check_rows_col(&cols[c], who)) return rc;
+        if (int rc = check_rows_col(&out[c], who)) return rc;
+        if (cols[c].dtype != out[c].dtype || row_lanes(&cols[c]) != row_lanes(&out[c]))
+            QK_FAIL(QK_ERR_INVALID, "%s: dtype / lanes mismatch on column %d", who, c);
+        if (out[c].length < n_idx) QK_FAIL(QK_ERR_CAPACITY, "%s: output %d too small", who, c);
+        if (row_lanes(&cols[c]) == 1 && cols[c].dtype != QK_F16) {
+            scal_in[nscal] = cols[c]; scal_out[nscal] = out[c]; ++nscal;
+            continue;
+        }
+        const int L = row_lanes(&cols[c]);
+        int64_t nb = (n_idx * L + 255) / 256;
+        if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
+        switch (dtype_size(cols[c].dtype)) {
+            case 1: k_gather_rows<uint8_t><<<(unsigned)nb, 256, 0, st>>>((const uint8_t*)cols[c].data, (uint8_t*)out[c].data, idx, n_idx, L); break;
+            case 2: k_gather_rows<uint16_t><<<(unsigned)nb, 256, 0, st>>>((const uint16_t*)cols[c].data, (uint16_t*)out[c].data, idx, n_idx, L); break;
+            case 4: k_gather_rows<uint32_t><<<(unsigned)nb, 256, 0, st>>>((const uint32_t*)cols[c].data, (uint32_t*)out[c].data, idx, n_idx, L); break;
+            default: k_gather_rows<uint64_t><<<(unsigned)nb, 256, 0, st>>>((const uint64_t*)cols[c].data, (uint64_t*)out[c].data, idx, n_idx, L); break;
+        }
+        QK_LAUNCH_CHECK("k_gather_rows");
+    }
+    if (nscal == 0) return QK_OK;
+    if (int rc = fill_move(M, scal_in, nscal, scal_out, -1, n_idx, who)) return rc;
     int64_t nb = (n_idx + 255) / 256;
     if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_gather<<<(unsigned)nb, 256, 0, (cudaStream_t)stream>>>(M, idx, n_idx);
+    k_gather<<<(unsigned)nb, 256, 0, st>>>(M, idx, n_idx);
     QK_LAUNCH_CHECK("k_gather");
     return QK_OK;
 }

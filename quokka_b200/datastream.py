@@ -62,12 +62,23 @@ class Expression:
 
 
 # ------------------------------------------------------------------ logical nodes
+def _reject_vectors(vectors, cols, what: str):
+    """Vector columns only move (select / rename / filter on other columns / union / broadcast / vector_nn_join); every use
+    that reads one as a value or a key is refused while the plan is built."""
+    bad = sorted(set(cols) & set(vectors))
+    if bad:
+        raise NotImplementedError(f"{what}: column {bad[0]!r} is a vector column; it can only be selected, renamed, carried "
+                                  "through filters and unions, collected or probed with vector_nn_join")
+
+
 class Node:
     kind = "node"
 
-    def __init__(self, schema, parents=()):
+    def __init__(self, schema, parents=(), vectors=None):
         self.schema = list(schema)
         self.parents = list(parents)
+        # names of the vector (fixed-width list) columns of this node's output
+        self.vectors = set(vectors) if vectors is not None else {c for p in self.parents for c in p.vectors if c in self.schema}
 
     def est_rows(self):
         return max((p.est_rows() for p in self.parents), default=0)
@@ -76,8 +87,8 @@ class Node:
 class SourceNode(Node):
     kind = "source"
 
-    def __init__(self, reader, schema, est_rows, ordered=False):
-        super().__init__(schema)
+    def __init__(self, reader, schema, est_rows, ordered=False, vectors=()):
+        super().__init__(schema, vectors=vectors)
         self.reader, self._est, self.ordered = reader, est_rows, ordered
 
     def est_rows(self):
@@ -88,6 +99,7 @@ class FilterNode(Node):
     kind = "filter"
 
     def __init__(self, parent, pred):
+        _reject_vectors(parent.vectors, pred.columns(), "filter")
         super().__init__(parent.schema, [parent])
         self.pred = pred
 
@@ -96,6 +108,8 @@ class MapNode(Node):
     kind = "map"
 
     def __init__(self, parent, new):
+        for e in new.values():
+            _reject_vectors(parent.vectors, e.columns(), "expression")
         super().__init__(parent.schema + [n for n in new if n not in parent.schema], [parent])
         self.new = dict(new)
 
@@ -111,7 +125,7 @@ class RenameNode(Node):
     kind = "rename"
 
     def __init__(self, parent, mapping):
-        super().__init__([mapping.get(c, c) for c in parent.schema], [parent])
+        super().__init__([mapping.get(c, c) for c in parent.schema], [parent], {mapping.get(c, c) for c in parent.vectors})
         self.mapping = dict(mapping)
 
 
@@ -119,6 +133,9 @@ class JoinNode(Node):
     kind = "join"
 
     def __init__(self, left, right, left_on, right_on, how, suffix):
+        _reject_vectors(left.vectors, [left_on], "join key")
+        _reject_vectors(right.vectors, [right_on], "join key")
+        _reject_vectors(left.vectors | right.vectors, left.vectors | right.vectors, "join (hash-partitioned edge)")
         self.left_on, self.right_on, self.how, self.suffix = left_on, right_on, how, suffix
         if how in ("semi", "anti"):
             schema, self.right_names = list(left.schema), {}
@@ -141,6 +158,9 @@ class AggNode(Node):
 
     def __init__(self, parent, keys, aggs_exprs, orderby):
         """aggs_exprs: [(expression Node containing aggregate calls, alias)] as parsed from agg_sql."""
+        _reject_vectors(parent.vectors, keys, "aggregate key")
+        for e, _ in aggs_exprs:
+            _reject_vectors(parent.vectors, e.columns(), "aggregate")
         super().__init__(list(keys) + [alias for _, alias in aggs_exprs], [parent])
         self.keys, self.aggs_exprs, self.orderby = list(keys), list(aggs_exprs), orderby
 
@@ -152,6 +172,7 @@ class TopKNode(Node):
     kind = "topk"
 
     def __init__(self, parent, by, k, desc):
+        _reject_vectors(parent.vectors, by, "top-k key")
         super().__init__(parent.schema, [parent])
         self.by, self.k, self.desc = by, k, desc
 
@@ -163,6 +184,7 @@ class DistinctNode(Node):
     kind = "distinct"
 
     def __init__(self, parent, keys):
+        _reject_vectors(parent.vectors, keys, "distinct key")
         super().__init__(keys, [parent])
         self.keys = keys
 
@@ -171,6 +193,7 @@ class AsofNode(Node):
     kind = "asof"
 
     def __init__(self, left, right, left_on, right_on, left_by, right_by, suffix):
+        _reject_vectors(left.vectors | right.vectors, left.vectors | right.vectors, "as-of join")
         schema = list(left.schema)
         self.right_names = {}
         for c in right.schema:
@@ -186,8 +209,12 @@ class AsofNode(Node):
 class StatefulNode(Node):
     kind = "stateful"
 
-    def __init__(self, parents: dict, executor, new_schema, required_columns, partitioners, placement):
-        super().__init__(new_schema, list(parents.values()))
+    def __init__(self, parents: dict, executor, new_schema, required_columns, partitioners, placement, vectors=None):
+        for sid, p in parents.items():
+            part = partitioners.get(sid) if isinstance(partitioners, dict) else partitioners
+            if isinstance(part, HashPartitioner):
+                _reject_vectors(p.vectors, p.vectors, "hash-partitioned edge")
+        super().__init__(new_schema, list(parents.values()), vectors)
         self.streams, self.executor = parents, executor
         self.required_columns, self.partitioners, self.placement = required_columns, partitioners, placement
 
@@ -746,6 +773,7 @@ class DataStream:
         assert len(set(columns)) == len(columns), "columns must be distinct"
         for c in columns:
             assert c in self.schema, f"column {c} not in schema"
+        _reject_vectors(self.node.vectors, columns, mode)
         part = StatefulNode({0: self.node}, GramPartialExecutor(columns, **executor_args), ["__gram"], {0: set(columns)},
                             {0: PassThroughPartitioner()}, CustomChannelsStrategy(1))
         node = StatefulNode({0: part}, GramFinalExecutor(columns, mode), list(columns), {0: {"__gram"}},
@@ -801,10 +829,80 @@ class DataStream:
         assert len(set(columns)) == len(columns), "columns must be distinct"
         for c in columns:
             assert c in self.schema, f"column {c} not in schema"
+        _reject_vectors(self.node.vectors, columns, "approximate_quantile")
         part = StatefulNode({0: self.node}, QuantilePartialExecutor(columns), list(QUANTILE_ENTRY_COLUMNS), {0: set(columns)},
                             {0: PassThroughPartitioner()}, CustomChannelsStrategy(1))
         node = StatefulNode({0: part}, QuantileFinalExecutor(columns, quantiles), columns, {0: set(QUANTILE_ENTRY_COLUMNS)},
                             {0: BroadcastPartitioner()}, SingleChannelStrategy())
+        return DataStream(self.quokka_context, node)
+
+    def vector_nn_join(self, probe_df, vec_column=None, vec_column_left=None, vec_column_right=None, k=1, suffix="_probe",
+                       probe_side="right", tmp_directory=None, score_column=None):
+        """The k rows of this stream nearest to every row of `probe_df` by cosine similarity (pyquokka/datastream.py:396-477).
+        `probe_df` is a pyarrow.Table or pandas DataFrame holding a vector column; probe columns whose names clash with the
+        stream's get `suffix`.  Output: the stream's columns, then the probe's, then `score_column` (f32 cosine) if given.
+
+        Every probe is normalised on the host in fp64 and rounded to fp32; a probe with zero norm or a non-finite element raises
+        ValueError.  Rows of the stream score s = (x . p) / ||x|| (qk_knn_topk: one fused pass per batch on the device, 3xTF32
+        tensor-core dot products, |s - exact| <= (d + 8) 2^-21 for elements of magnitude in [2^-80, 2^80], bit-identical however
+        the rows are batched or split across ranks); zero rows and rows holding a NaN or an inf never match.  Per rank the candidates of all batches are merged, then the ranks on one channel.
+        Deviations from the reference: probes come out in probe_df order, each with its rows BEST FIRST (the reference's
+        argsort(...)[-k:] gives ascending similarity), ties broken by arrival (rank, batch, row); a probe gets min(k, valid rows)
+        rows where the reference has no rule for fewer than k.  probe_side="left" (the reference's Lance IVF_PQ index) is not
+        implemented."""
+        from .executors import KNN_HIDDEN, KnnFinalExecutor, KnnPartialExecutor
+        from .columns import vector_columns
+        if vec_column is not None:
+            assert vec_column_left is None and vec_column_right is None, "cannot specify both vec_column and vec_column_left/vec_column_right"
+            vec_column_left = vec_column_right = vec_column
+        else:
+            assert vec_column_right is not None and vec_column_left is not None, "must specify either vec_column or vec_column_left/vec_column_right"
+        assert type(k) == int and k >= 1, "k must be at least 1"
+        if k > L.KNN_MAX_K:
+            raise ValueError(f"k must be at most {L.KNN_MAX_K}")
+        if not isinstance(probe_df, pa.Table):
+            import pandas as pd
+            assert isinstance(probe_df, pd.DataFrame), "probe_df must be a pyarrow Table or a pandas DataFrame"
+            probe_df = pa.Table.from_pandas(probe_df, preserve_index=False)
+        assert vec_column_left in self.schema, "Vector column not in schema"
+        assert vec_column_right in probe_df.column_names, "Probe column not in schema"
+        assert probe_side in ["left", "right"], "probe_side must be either 'left' or 'right'"
+        if probe_side == "left":
+            raise NotImplementedError("vector_nn_join(probe_side='left') probes a Lance IVF_PQ index in the reference; not implemented")
+        if vec_column_left not in self.node.vectors:
+            raise L.QkError(f"vector_nn_join: column {vec_column_left!r} is not a vector column")
+        names = []
+        for c in probe_df.column_names:
+            if c in self.schema:
+                assert c + suffix not in probe_df.column_names, "suffix not sufficient to avoid column name collision"
+                names.append(c + suffix)
+            else:
+                names.append(c)
+        probe_df = probe_df.rename_columns(names)
+        probe_vec = vec_column_right + suffix if vec_column_right in self.schema else vec_column_right
+        vec_col = probe_df[probe_vec]
+        if vec_col.null_count or not pa.types.is_list(vec_col.type) and not pa.types.is_fixed_size_list(vec_col.type) \
+                and not pa.types.is_large_list(vec_col.type):
+            raise ValueError(f"probe column {vec_column_right!r} must be a list column without nulls")
+        rows = vec_col.to_pylist()
+        if len({len(r) for r in rows}) > 1:
+            raise ValueError(f"probe column {vec_column_right!r} is ragged")
+        P = np.asarray(rows, dtype=np.float64).reshape(len(rows), -1)
+        if not np.isfinite(P).all():
+            raise ValueError("vector_nn_join: a probe vector has a non-finite element")
+        norms = np.linalg.norm(P, axis=1)
+        if (norms == 0).any():
+            raise ValueError("vector_nn_join: a probe vector has zero norm")
+        phat = (P / norms[:, None]).astype(np.float32)
+        schema = self.schema + list(probe_df.column_names)
+        if score_column is not None:
+            assert score_column not in schema, "score_column clashes with a column of the result"
+            schema.append(score_column)
+        part = StatefulNode({0: self.node}, KnnPartialExecutor(vec_column_left, phat, k), self.schema + KNN_HIDDEN, {0: set(self.schema)},
+                            {0: PassThroughPartitioner()}, CustomChannelsStrategy(1))
+        final = KnnFinalExecutor(self.schema, probe_df, len(rows), k, score_column)
+        node = StatefulNode({0: part}, final, schema, {0: set(part.schema)}, {0: BroadcastPartitioner()}, SingleChannelStrategy(),
+                            vectors=self.node.vectors | set(vector_columns(probe_df.schema)))
         return DataStream(self.quokka_context, node)
 
     def approximate_median(self, columns, sample_factor=1):

@@ -75,7 +75,7 @@ class QuokkaContext:
         reader = InputParquetDataset(table_location, row_groups_per_batch=self.exec_config["row_groups_per_batch"],
                                      device_decode=self.exec_config["device_parquet"])
         schema = reader.schema().names
-        return DataStream(self, SourceNode(reader, schema, reader.num_rows()))
+        return DataStream(self, SourceNode(reader, schema, reader.num_rows(), vectors=_columns.vector_columns(reader.schema())))
 
     def read_csv(self, table_location: str, schema=None, has_header=False, sep=","):
         """Local CSV file, directory or `/path/*` (df.py:264-410).  `schema`: list of column names; with has_header the
@@ -92,11 +92,12 @@ class QuokkaContext:
                                            device_decode=self.exec_config["device_parquet"])
         schema = reader.schema().names
         assert sorted_by in schema
-        return OrderedStream(self, SourceNode(reader, schema, reader.num_rows(), ordered=True), sorted_by)
+        return OrderedStream(self, SourceNode(reader, schema, reader.num_rows(), ordered=True,
+                                              vectors=_columns.vector_columns(reader.schema())), sorted_by)
 
     def from_arrow(self, df: pa.Table):
         reader = InputArrowDataset(df, self.exec_config["chunk_rows"])
-        return DataStream(self, SourceNode(reader, df.column_names, df.num_rows))
+        return DataStream(self, SourceNode(reader, df.column_names, df.num_rows, vectors=_columns.vector_columns(df.schema)))
 
     def read_dataset(self, dataset):
         """pyquokka/df.py:665-693: the result of `DataStream.compute()` back as a DataStream (Q11, Q15, Q20, Q21 of
@@ -116,19 +117,22 @@ class QuokkaContext:
     def from_arrow_sorted(self, df: pa.Table, sorted_by: str):
         reader = InputArrowDataset(df, self.exec_config["chunk_rows"])
         reader.sorted_by = sorted_by
-        return OrderedStream(self, SourceNode(reader, df.column_names, df.num_rows, ordered=True), sorted_by)
+        return OrderedStream(self, SourceNode(reader, df.column_names, df.num_rows, ordered=True,
+                                              vectors=_columns.vector_columns(df.schema)), sorted_by)
 
     def from_pinned(self, columns: dict, dictionaries: dict | None = None, dates=(), chunk_rows: int | None = None):
         """Arrow-layout columns held in pinned host memory by this rank ({name: pinned torch tensor}); string
         columns are passed as integer codes + `dictionaries[name]`.  Chunks are streamed over PCIe and
         overlapped with the operators (dataset.InputPinnedDataset)."""
         reader = InputPinnedDataset(columns, chunk_rows or self.exec_config["pinned_chunk_rows"], dictionaries, dates)
-        return DataStream(self, SourceNode(reader, list(columns), reader.num_rows() * world_size()))
+        return DataStream(self, SourceNode(reader, list(columns), reader.num_rows() * world_size(),
+                                           vectors=[n for n, t in columns.items() if t.dim() == 2]))
 
     def from_device(self, table: DeviceTable, sorted_by: str | None = None, batch_rows: int | None = None):
         """Columns already resident in this rank's HBM (each rank passes its own shard)."""
         reader = InputDeviceDataset(table, batch_rows)
-        node = SourceNode(reader, table.column_names, len(table) * world_size(), ordered=sorted_by is not None)
+        node = SourceNode(reader, table.column_names, len(table) * world_size(), ordered=sorted_by is not None,
+                          vectors=[n for n, c in table.columns.items() if c.is_vector])
         if sorted_by is not None:
             reader.sorted_by = sorted_by
             return OrderedStream(self, node, sorted_by)

@@ -91,6 +91,8 @@ class EdgeOps:
             bloom = None
         if self.pred is None and trivial and bloom is None:
             return DeviceTable({n: t[e.value] for n, e in defs.items()})
+        if any(c.is_vector for c in t.columns.values()):
+            return self._apply_vectors(t, defs, stable, bloom)
         used = sorted(self.required_raw(raw), key=raw.index)
         sub = t.select(used)
         if any(sub[c].valid is not None for c in used):
@@ -113,6 +115,25 @@ class EdgeOps:
                 cols[n] = DeviceColumn(o)
         return DeviceTable(cols)
 
+    def _apply_vectors(self, t: DeviceTable, defs: dict, stable: bool, bloom) -> DeviceTable:
+        """A table with vector (2-D) columns: the scan kernel runs over the scalar columns plus a hidden int32 row number, and
+        the vector columns the edge passes on are gathered by the surviving row numbers.  Expressions cannot read a vector."""
+        vec_raw = {c for c, col in t.columns.items() if col.is_vector}
+        read = set(self.pred.columns()) if self.pred is not None else set()
+        for n, e in defs.items():
+            if e.kind != "col":
+                read |= e.columns()
+        bad = sorted(read & vec_raw)
+        if bad:
+            raise NotImplementedError(f"column {bad[0]!r} is a vector column: expressions and predicates cannot read it")
+        moved = [n for n, e in defs.items() if e.kind == "col" and e.value in vec_raw]
+        rest = {n: e for n, e in defs.items() if n not in moved}
+        rows = DeviceColumn(torch.arange(len(t), dtype=torch.int32, device=t.device))
+        plain = t.drop(sorted(vec_raw)).with_column("__row", rows)
+        out = EdgeOps(self.pred, rest | {"__row": E.col("__row")}).apply(plain, stable, bloom)
+        src = sorted({defs[n].value for n in moved})
+        got = t.select(src).gather(out["__row"].data)
+        return DeviceTable({n: got[defs[n].value] if n in moved else out[n] for n in defs})
 
     def _apply_nullable(self, t: DeviceTable, defs: dict, stable: bool) -> DeviceTable:
         """SQL's NULL rules for inputs that carry validity masks (the right side of a left / as-of join): a row whose

@@ -793,6 +793,102 @@ class QuantileFinalExecutor(Executor):
         return self.state
 
 
+# ---------------------------------------------------------------------------------------------- nearest neighbours
+KNN_HIDDEN = ["__knn_probe", "__knn_score", "__knn_key"]
+_KNN_RANK_SHIFT = 56            # final key = rank << 56 | batch sequence << 32 | row
+
+
+class KnnPartialExecutor(Executor):
+    """Per-rank phase of DataStream.vector_nn_join (DFProbeDataStreamNNExecutor1, pyquokka/executors/vector_executors.py:8-52,
+    which keeps every batch's k best rows per probe).  Every batch goes through qk_knn_topk; its <= q * k candidate rows (all
+    columns, vectors included) are gathered and merged by qk_knn_merge into a running state of q * k rows, keyed by arrival
+    (batch sequence << 32 | row).  done() emits the state, slot (p, j) at row p * k + j, with the hidden columns probe id, score
+    and key (rank in the top bits; -1 for an empty slot)."""
+
+    silent_streams = "all"       # execute() only accumulates; the candidates leave in done()
+
+    def __init__(self, vec_column, probes, k) -> None:
+        self.vec_column = vec_column
+        self.probes_host = np.ascontiguousarray(probes, dtype=np.float32)
+        self.k = int(k)
+        self.probes = None
+        self.state = None        # (scores [q, k], keys [q, k], DeviceTable of q * k rows)
+        self.seq = 0
+
+    def execute(self, batches, stream_id, executor_id):
+        for b in _clean(batches):
+            col = b[self.vec_column]
+            if not col.is_vector:
+                raise L.QkError(f"vector_nn_join: column {self.vec_column!r} is not a vector column")
+            if col.data.shape[1] != self.probes_host.shape[1]:
+                raise L.QkError(f"vector_nn_join: column {self.vec_column!r} has dimension {col.data.shape[1]}, the probes "
+                                f"{self.probes_host.shape[1]}")
+            if self.probes is None:
+                self.probes = torch.from_numpy(self.probes_host).to(b.device)
+            scores, rows = ops.knn_topk(col.data, self.probes, self.k)
+            keys = torch.where(rows >= 0, rows | (self.seq << 32), torch.full_like(rows, -1))
+            cand = b.gather(rows.reshape(-1).to(torch.int32))
+            self.seq += 1
+            if self.state is None:
+                self.state = (scores, keys, cand)
+                continue
+            s0, k0, t0 = self.state
+            ms, mk, src = ops.knn_merge(s0, k0, scores, keys, self.k)
+            self.state = (ms, mk, concat_tables([t0, cand]).gather(src.reshape(-1)))
+
+    def done(self, executor_id):
+        if self.state is None:
+            return None
+        scores, keys, t = self.state
+        q = scores.shape[0]
+        dev = scores.device
+        keys = torch.where(keys >= 0, keys | (int(executor_id) << _KNN_RANK_SHIFT), keys)
+        probe = torch.arange(q, dtype=torch.int32, device=dev).repeat_interleave(self.k)
+        return DeviceTable(dict(t.columns) | {"__knn_probe": DeviceColumn(probe), "__knn_score": DeviceColumn(scores.reshape(-1)),
+                                              "__knn_key": DeviceColumn(keys.reshape(-1))})
+
+
+class KnnFinalExecutor(Executor):
+    """Final phase of DataStream.vector_nn_join on one channel (DFProbeDataStreamNNExecutor2): merges the per-rank candidate
+    states with qk_knn_merge (the rank sits in the top bits of every key, so ties between ranks go to the lower rank) and emits,
+    probe by probe in the probe table's order, its min(k, valid rows) rows best first, followed by the probe's columns and, if
+    asked for, the score."""
+
+    silent_streams = "all"       # the result leaves in done()
+
+    def __init__(self, columns, probe_table: pa.Table, q, k, score_column=None) -> None:
+        self.columns = list(columns)
+        self.probe_table = probe_table
+        self.q, self.k = int(q), int(k)
+        self.score_column = score_column
+        self.parts = []
+        self.state = None
+
+    def execute(self, batches, stream_id, executor_id):
+        for b in _clean(batches):
+            n = self.q * self.k
+            for lo in range(0, len(b), n):             # the states of several ranks may arrive in one batch
+                self.parts.append(b.slice(lo, lo + n))
+
+    def done(self, executor_id):
+        if not self.parts:
+            return None
+        q, k = self.q, self.k
+        t = self.parts[0]
+        s, key = t["__knn_score"].data.reshape(q, k), t["__knn_key"].data.reshape(q, k)
+        for p in self.parts[1:]:
+            s, key, src = ops.knn_merge(s, key, p["__knn_score"].data.reshape(q, k), p["__knn_key"].data.reshape(q, k), k)
+            t = concat_tables([t, p]).gather(src.reshape(-1))
+        keep = torch.nonzero(key.reshape(-1) >= 0).flatten().to(torch.int32)
+        t = t.gather(keep)
+        probe_rows = DeviceTable.from_arrow(self.probe_table, t.device).gather(t["__knn_probe"].data)
+        cols = {c: t[c] for c in self.columns} | dict(probe_rows.columns)
+        if self.score_column is not None:
+            cols[self.score_column] = t["__knn_score"]
+        self.state = DeviceTable(cols)
+        return self.state
+
+
 # ---------------------------------------------------------------------------------------------- as-of
 class SortedAsofExecutor(Executor):
     """ts_executors.py:324-383: streaming backward as-of join of two time-sorted streams per symbol.

@@ -12,9 +12,9 @@ from . import _lib as L
 from . import expr as E
 
 _TORCH2QK = {torch.uint8: L.QK_U8, torch.bool: L.QK_U8, torch.int32: L.QK_I32, torch.int64: L.QK_I64,
-             torch.float32: L.QK_F32, torch.float64: L.QK_F64}
+             torch.float32: L.QK_F32, torch.float64: L.QK_F64, torch.float16: L.QK_F16}
 _QK2TORCH = {L.QK_U8: torch.uint8, L.QK_I32: torch.int32, L.QK_I64: torch.int64, L.QK_F32: torch.float32,
-             L.QK_F64: torch.float64}
+             L.QK_F64: torch.float64, L.QK_F16: torch.float16}
 
 
 def qk_dtype(t: torch.Tensor) -> int:
@@ -32,7 +32,10 @@ def _require_cuda(t: torch.Tensor, what: str):
 
 
 def col(t: torch.Tensor, what: str = "column") -> L.qk_column:
+    """A 1-D tensor is a scalar column; a 2-D (n, d) tensor is a vector column of n rows (lanes = d)."""
     _require_cuda(t, what)
+    if t.dim() == 2:
+        return L.qk_column(t.data_ptr() if t.numel() else None, None, t.shape[0], qk_dtype(t), t.shape[1])
     return L.qk_column(t.data_ptr() if t.numel() else None, None, t.numel(), qk_dtype(t), 0)
 
 
@@ -374,7 +377,7 @@ class XchgChannel:
 
 def gather(columns: Sequence[torch.Tensor], idx: torch.Tensor):
     n = idx.numel()
-    outs = [torch.empty(n, dtype=c.dtype, device=c.device) for c in columns]
+    outs = [torch.empty((n,) + tuple(c.shape[1:]), dtype=c.dtype, device=c.device) for c in columns]
     if n == 0:
         return outs
     for lo in range(0, len(columns), L.MAX_COLS):
@@ -741,3 +744,58 @@ def parquet_page_runs(scratch: torch.Tensor, pages: torch.Tensor, n_pages: int, 
 
 def launch_count() -> int:
     return int(L.lib().qk_launch_count())
+
+
+# ------------------------------------------------------------------ K11 nearest neighbours
+KNN_WS_BUDGET = 256 << 20          # bytes of per-CTA candidate lists one qk_knn_topk call may use; larger q is chunked
+
+
+def knn_topk(x: torch.Tensor, probes: torch.Tensor, k: int):
+    """(scores f32 [q, k], rows int64 [q, k]) of the k rows of `x` (n x d, f32 / f16) with the highest cosine similarity to each
+    row of `probes` (q x d fp32, unit norm), best first, ties by smaller row; row -1 / score -inf pad probes with fewer valid
+    rows.  Probes are chunked so that the kernel's workspace stays under KNN_WS_BUDGET."""
+    if x.dim() != 2 or x.dtype not in (torch.float32, torch.float16):
+        raise L.QkError("knn_topk: x must be an (n, d) f32 or f16 tensor")
+    if probes.dim() != 2 or probes.dtype != torch.float32 or probes.shape[1] != x.shape[1]:
+        raise L.QkError("knn_topk: probes must be a (q, d) fp32 tensor with the vectors' d")
+    if not 1 <= k <= L.KNN_MAX_K:
+        raise L.QkError(f"knn_topk: k must be in [1, {L.KNN_MAX_K}]")
+    if not 1 <= x.shape[1] <= L.KNN_MAX_DIM:
+        raise L.QkError(f"knn_topk: dimension {x.shape[1]} outside [1, {L.KNN_MAX_DIM}]")
+    x = x.contiguous()
+    probes = probes.contiguous()
+    n, d = x.shape
+    q = probes.shape[0]
+    scores = torch.empty(q, k, dtype=torch.float32, device=x.device)
+    rows = torch.empty(q, k, dtype=torch.int64, device=x.device)
+    if q == 0:
+        return scores, rows
+    lib = L.lib()
+    chunk = q
+    while chunk > 16 and lib.qk_knn_workspace_bytes(n, d, chunk, k) > KNN_WS_BUDGET:
+        chunk = (chunk + 1) // 2
+    ws = _ws(lib.qk_knn_workspace_bytes(n, d, chunk, k), x.device)
+    xc = col(x, "vectors")
+    for lo in range(0, q, chunk):
+        m = min(chunk, q - lo)
+        L.check(lib.qk_knn_topk(C.byref(xc), probes[lo:lo + m].data_ptr(), m, k, scores[lo:lo + m].data_ptr(),
+                                rows[lo:lo + m].data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "qk_knn_topk")
+    return scores, rows
+
+
+def knn_merge(a_score: torch.Tensor, a_key: torch.Tensor, b_score: torch.Tensor, b_key: torch.Tensor, k: int):
+    """Per probe, the best k of two sorted candidate lists ([q, ka] and [q, kb] scores f32 / keys int64, key -1 = no entry):
+    (scores [q, k], keys [q, k], src int32 [q, k]) with src indexing the concatenation of a's and b's flattened entries."""
+    q = a_score.shape[0]
+    if b_score.shape[0] != q or a_key.shape != a_score.shape or b_key.shape != b_score.shape:
+        raise L.QkError("knn_merge: candidate lists of different shapes")
+    if k < 1:
+        raise L.QkError("knn_merge: k must be >= 1")
+    dev = a_score.device
+    a_score, a_key, b_score, b_key = (t.contiguous() for t in (a_score, a_key, b_score, b_key))
+    os_ = torch.empty(q, k, dtype=torch.float32, device=dev)
+    ok = torch.empty(q, k, dtype=torch.int64, device=dev)
+    src = torch.empty(q, k, dtype=torch.int32, device=dev)
+    L.check(L.lib().qk_knn_merge(q, a_score.data_ptr(), a_key.data_ptr(), a_score.shape[1], b_score.data_ptr(), b_key.data_ptr(),
+                                 b_score.shape[1], k, os_.data_ptr(), ok.data_ptr(), src.data_ptr(), _stream()), "qk_knn_merge")
+    return os_, ok, src

@@ -83,6 +83,10 @@ def plan_batch(units, columns=None):
         names = schema.names
         want = columns if columns is not None else list(arrow_schema.names)
         for name in want:
+            if name in arrow_schema.names and pa.types.is_list(arrow_schema.field(name).type) | \
+                    pa.types.is_large_list(arrow_schema.field(name).type) | pa.types.is_fixed_size_list(arrow_schema.field(name).type):
+                raise L.QkError(f"{path}: column {name!r} is a nested list (vector) column, which the device Parquet decoder "
+                                "does not read; set device_parquet to False to read it through Arrow")
             if name not in names:
                 raise L.QkError(f"{path}: no column {name!r} (nested columns are not supported)")
             ci = names.index(name)

@@ -48,13 +48,45 @@ def rank() -> int:
 
 # ------------------------------------------------------------------ the shuffle
 _DT = {"torch.uint8": torch.uint8, "torch.int32": torch.int32, "torch.int64": torch.int64,
-       "torch.float32": torch.float32, "torch.float64": torch.float64}
+       "torch.float32": torch.float32, "torch.float64": torch.float64, "torch.float16": torch.float16}
+_VALID_FLAG, _WIDTH_MASK = 1 << 32, (1 << 32) - 1     # meta word of a column: row bytes | _VALID_FLAG when it has a mask
+
+
+def _col_dt(t: torch.Tensor) -> str:
+    """Schema string of a column buffer: the dtype, and the row width of a vector column ("torch.float32[768]")."""
+    return str(t.dtype) if t.dim() == 1 else f"{t.dtype}[{t.shape[1]}]"
+
+
+def _parse_dt(dt: str):
+    """(torch dtype, lanes) of a schema string; lanes = 0 for a scalar column."""
+    base, _, lanes = dt.partition("[")
+    return _DT[base], (int(lanes[:-1]) if lanes else 0)
+
+
+def _row_bytes(dt: str) -> int:
+    t, lanes = _parse_dt(dt)
+    return t.itemsize * max(1, lanes)
+
+
+def _empty(n: int, dt: str, device) -> torch.Tensor:
+    t, lanes = _parse_dt(dt)
+    return torch.empty((n, lanes) if lanes else n, dtype=t, device=device)
+
+
+def _as_rows(buf: torch.Tensor, dt: str) -> torch.Tensor:
+    """A received byte / element buffer as the column's rows."""
+    t, lanes = _parse_dt(dt)
+    v = buf.view(t)
+    return v.view(-1, lanes) if lanes else v
 
 
 def _flat(t: torch.Tensor) -> torch.Tensor:
-    """A dense 1-D buffer (a one-row slice of a 2-D state keeps its row stride and reports is_contiguous())."""
+    """A dense buffer: 1-D for a scalar column, (n, d) row-major for a vector column (a one-row slice of a 2-D state keeps its
+    row stride and reports is_contiguous())."""
     if t.dim() == 1 and (t.numel() == 0 or t.stride(0) == 1):
         return t
+    if t.dim() == 2:
+        return t.contiguous()
     out = torch.empty(t.numel(), dtype=t.dtype, device=t.device)      # fresh storage: unit stride guaranteed
     out.copy_(t.reshape(-1))
     return out
@@ -194,9 +226,10 @@ class Exchange:
         maxrecv = max(n_recv)
         src = next(r for r in range(w) if int(allmeta[r, w + 2]) > 0)
         ncols = int(allmeta[src, w + 2])
-        col_w = [int(allmeta[src, w + 3 + i]) & 255 for i in range(ncols)]
-        if any(int(allmeta[r, w + 3 + i]) & 256 for r in range(w) for i in range(ncols)):
-            return None                                           # validity masks: NCCL path
+        col_w = [int(allmeta[src, w + 3 + i]) & _WIDTH_MASK for i in range(ncols)]
+        if any(int(allmeta[r, w + 3 + i]) & _VALID_FLAG for r in range(w) for i in range(ncols)) \
+                or any(_parse_dt(sc[1])[1] for sc in schema or []):
+            return None                                           # validity masks, vector columns: NCCL path
         bases, off = [], 0
         for wd in col_w:
             bases.append(off)
@@ -224,13 +257,13 @@ class Exchange:
             return []
         out = {}
         for i, (name, dt, union, atype, _) in enumerate(schema):
-            view = mb.buf[bases[i]: bases[i] + n_recv[me] * col_w[i]].view(_DT[dt])
+            view = _as_rows(mb.buf[bases[i]: bases[i] + n_recv[me] * col_w[i]], dt)
             out[name] = DeviceColumn(view.clone(), union, atype)   # the mailbox is reused by the next exchange
         return [DeviceTable(out)]
 
     @staticmethod
     def _schema_of(t: DeviceTable):
-        return [(n, str(c.data.dtype), c.dictionary, c.arrow_type, c.valid is not None) for n, c in t.columns.items()]
+        return [(n, _col_dt(c.data), c.dictionary, c.arrow_type, c.valid is not None) for n, c in t.columns.items()]
 
     # ------------------------------------------------------------------ the peer-memory path (csrc/exchange.cu)
     W_COUNTS, W_HASH, W_CACHED, W_NCOLS, W_WIDTHS, MAXC = 0, 16, 17, 18, 20, 24
@@ -320,7 +353,7 @@ class Exchange:
         words[self.W_NCOLS] = len(mine) if mine is not None else 0
         if mine is not None:
             for i, (_, dt, _, _, hv) in enumerate(mine):
-                words[self.W_WIDTHS + i] = _DT[dt].itemsize | (256 if hv else 0)
+                words[self.W_WIDTHS + i] = _row_bytes(dt) | (_VALID_FLAG if hv else 0)
         m = ch.meta(words, doffs if dest is not None else None)
         counts = m[:, :w]                                               # counts[s][d]
         if edge_key is not None:
@@ -356,8 +389,8 @@ class Exchange:
             self.schemas[edge_key] = schema
         src = next(r for r in range(w) if int(m[r, self.W_NCOLS]) > 0)
         ncols = int(m[src, self.W_NCOLS])
-        col_w = [int(m[src, self.W_WIDTHS + i]) & 255 for i in range(ncols)]
-        col_valid = [any(int(m[r, self.W_WIDTHS + i]) & 256 for r in range(w)) for i in range(ncols)]
+        col_w = [int(m[src, self.W_WIDTHS + i]) & _WIDTH_MASK for i in range(ncols)]
+        col_valid = [any(int(m[r, self.W_WIDTHS + i]) & _VALID_FLAG for r in range(w)) for i in range(ncols)]
         widths = col_w + [1 for v in col_valid if v]                     # validity masks travel as extra uint8 columns
         n_recv = [int(counts[:, d].sum()) for d in range(w)]
         bases = []                                                       # bases[d][c]: column c in rank d's mailbox
@@ -398,7 +431,7 @@ class Exchange:
         if n_recv[me] == 0 or schema is None:
             ch.recv([], [])
             return []
-        outs = [torch.empty(n_recv[me], dtype=_DT[schema[i][1]], device=self.device) for i in range(ncols)]
+        outs = [_empty(n_recv[me], schema[i][1], self.device) for i in range(ncols)]
         outs += [torch.empty(n_recv[me], dtype=torch.uint8, device=self.device) for v in col_valid if v]
         ch.recv(bases[me], outs)
         vmap, k = {}, ncols
@@ -502,7 +535,7 @@ class Exchange:
             if len(mine) > MAXC:
                 raise L.QkError(f"exchange: more than {MAXC} columns on one edge")
             for i, (_, dt, _, _, hv) in enumerate(mine):
-                widths[i] = _DT[dt].itemsize | (256 if hv else 0)
+                widths[i] = _row_bytes(dt) | (_VALID_FLAG if hv else 0)
         meta = torch.tensor(counts + [h_mine, h_cached, len(mine) if mine is not None else 0] + widths + [peer_flag],
                             dtype=torch.int64, device=self.device)
         M = w + 3 + MAXC + 1
@@ -539,8 +572,8 @@ class Exchange:
             table = parts.table                                   # NCCL path: group the rows locally first
         src = next(r for r in range(w) if int(allmeta[r, w + 2]) > 0)
         ncols = int(allmeta[src, w + 2])
-        col_w = [int(allmeta[src, w + 3 + i]) & 255 for i in range(ncols)]
-        col_valid = [any(int(allmeta[r, w + 3 + i]) & 256 for r in range(w)) for i in range(ncols)]
+        col_w = [int(allmeta[src, w + 3 + i]) & _WIDTH_MASK for i in range(ncols)]
+        col_valid = [any(int(allmeta[r, w + 3 + i]) & _VALID_FLAG for r in range(w)) for i in range(ncols)]
         recv_counts = [int(allmeta[s_, me]) for s_ in range(w)]
         send_counts = [int(c) for c in counts]
         n_recv, n_send = sum(recv_counts), sum(send_counts)
@@ -557,7 +590,7 @@ class Exchange:
                 if union is not None and c.dictionary != union:
                     c = unify_dictionaries([DeviceColumn(torch.zeros(0, dtype=c.data.dtype, device=c.data.device), union, c.arrow_type), c])[1][1]
                 d = _flat(c.data)
-                send_b = d.view(torch.uint8)
+                send_b = d.reshape(-1).view(torch.uint8)
                 if col_valid[i]:
                     valid_b = c.valid if c.valid is not None else torch.ones(len(c), dtype=torch.uint8, device=self.device)
             # one variable-split all-to-all per column (grouped ncclSend/ncclRecv inside NCCL), straight out of the
@@ -598,7 +631,7 @@ class Exchange:
             roff.append(roff[-1] + c_)
         out_cols = {}
         for (name, dt, union, atype, _), (recv_b, valid_r) in zip(schema, received):
-            out_cols[name] = (recv_b.view(_DT[dt]), union, atype, valid_r)
+            out_cols[name] = (_as_rows(recv_b, dt), union, atype, valid_r)
         tables = []
         for s_ in range(w):
             lo, hi = roff[s_], roff[s_ + 1]
