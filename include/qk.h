@@ -10,7 +10,8 @@
  *     the library never allocates, frees or synchronises: all work is enqueued on `stream`
  *     (a cudaStream_t passed as void*; NULL = legacy default stream);
  *   - return value 0 = ok, negative = QK_ERR_*; qk_last_error() gives a thread-local message;
- *   - no nulls on the hot path: qk_column.validity must be NULL (QK_ERR_UNSUPPORTED otherwise);
+ *   - no nulls on the hot path: qk_column.validity must be NULL (QK_ERR_UNSUPPORTED otherwise), except for the link
+ *     columns of qk_pattern_search;
  *     operators that can produce "no match" report it as index -1;
  *   - row counts fit int32 per call (a batch is < 2^31 rows); totals are int64.
  */
@@ -464,6 +465,33 @@ QK_API int qk_knn_topk(const qk_column* x, const float* probes, int32_t q, int32
 QK_API int qk_knn_merge(int32_t q, const float* a_score, const int64_t* a_key, int32_t ka, const float* b_score,
                         const int64_t* b_key, int32_t kb, int32_t k, float* out_score, int64_t* out_key, int32_t* out_src,
                         void* stream);
+
+/* ---- K12: complex event recognition over a key-segmented, time-sorted stream ---------------------------------------
+ * Replaces the per-batch DuckDB range join and Python DFS of CEPExecutor (pyquokka/executors/cep_executors.py:86-178) behind
+ * OrderedStream.pattern_recognize (pyquokka/orderedstream.py:37-53).  Inputs are in KEY-SEGMENTED order (as for the windows):
+ * time int64, by = dense int32 codes in [0, n_by), seg = device int64[n_by + 1] segment starts.  cand = device uint8[n]: bit e set
+ * when row r satisfies the row-local conjuncts of event e (evaluated before by qk_scan_filter_project).  starts = device int32
+ * rows (each with cand bit 0 set and inside its key's segment, seg[by[s]] <= s < seg[by[s] + 1] <= n; others give no match).  m = 2 .. QK_PATTERN_MAX_EVENTS events.
+ * A match of start r0 is rows r0 < r1 < ... < r(m-1) of r0's segment with time strictly increasing from one event to the next,
+ * t(r(m-1)) <= t(r0) + maxspan, cand bit e of r_e set and links[e] true over the bound rows.  The reported match is the one with
+ * the lexicographically smallest (t1 .. t(m-1)); out_bound[s * m + e] (device int32) = its row for event e, or -1 for every e when
+ * start s has none.
+ * links = HOST array of m programs: links[0] is empty, links[e] (empty = true) is postfix over the link columns with
+ * QK_OP_COL a0 = link column, a1 = the event whose bound row is read (a1 = e: the row being tested); ops: COL, CONST, ADD, SUB,
+ * MUL, DIV, NEG, the six float compares, AND, OR, NOT, SELECT; fp64; at most QK_MAX_EXPR_NODES nodes each, 128 together.
+ * link_cols: nlink <= QK_MAX_COLS scalar columns of n rows.  THIS IS THE ONE ENTRY POINT THAT ACCEPTS qk_column.validity: a
+ * device uint8 per row (0 = NULL); a link program that reads a NULL is false.
+ * budget: the rows one start may test; a start that exceeds it gives -1 and is counted in status.  status = device
+ * uint64[QK_PATTERN_STATUS_WORDS], zeroed by the call: [0] starts over budget, [1] n_starts - (smallest index into starts of such a
+ * start), 0 when none; the other words are the call's own.  rows_tested (device uint64 or NULL) accumulates the rows tested.
+ * Errors: bad arguments or programs: QK_ERR_INVALID; an op outside the subset, more stack or nodes than allowed, a vector link
+ * column: QK_ERR_UNSUPPORTED. */
+#define QK_PATTERN_MAX_EVENTS 8
+#define QK_PATTERN_STATUS_WORDS 4
+QK_API int qk_pattern_search(const qk_column* time, const qk_column* by, const int64_t* seg, int32_t n_by, const uint8_t* cand,
+                             const int32_t* starts, int64_t n_starts, int32_t m, int64_t maxspan, const qk_column* link_cols,
+                             int32_t nlink, const qk_expr* links, int64_t budget, int32_t* out_bound, uint64_t* status,
+                             uint64_t* rows_tested, void* stream);
 
 /* ---- synthetic TPC-H-shaped / SIP-shaped columns, generated in HBM --------------------------
  * Bit-identical to oracle/tpch_gen.py (counter-based hash of (table, column, row)); lets bench.py hold

@@ -10,6 +10,7 @@ LIB_PATH = os.path.join(HERE, "libqk.so")
 
 QK_U8, QK_I32, QK_I64, QK_F32, QK_F64, QK_F16 = 1, 2, 3, 4, 5, 6
 KNN_MAX_DIM, KNN_MAX_K = 4096, 256
+PATTERN_MAX_EVENTS, PATTERN_STATUS_WORDS, PATTERN_MAX_LINK_NODES = 8, 4, 128   # csrc/pattern.cu PT_MAX_NODES
 (OP_COL, OP_CONST, OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_NEG, OP_LT, OP_LE, OP_GT, OP_GE, OP_EQ, OP_NE,
  OP_AND, OP_OR, OP_NOT, OP_CMP_COL_IMM, OP_CMP_COL_COL, OP_RINT, OP_IN_SET, OP_SELECT, OP_EXTRACT, OP_RANGE_COL_IMM) = range(1, 24)
 CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_EQ, CMP_NE = range(6)
@@ -148,6 +149,9 @@ _SIGNATURES = {
                               C.c_void_p]),
     "qk_knn_merge": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "qk_pattern_search": (C.c_int, [_P(qk_column), _P(qk_column), C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                    C.c_int64, _P(qk_column), C.c_int32, _P(qk_expr), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p]),
     "qk_synth_column": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_int64), C.c_int64, C.c_int64, C.c_void_p,
                                   C.c_int32, C.c_void_p]),
     "qk_parquet_walk_chunk": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

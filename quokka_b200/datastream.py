@@ -937,7 +937,8 @@ class DataStream:
             return
         def walk(n, d=0):
             extra = {"filter": lambda: n.pred.sql(), "join": lambda: f"{n.how} {n.left_on}={n.right_on}",
-                     "agg": lambda: f"keys={n.keys}", "topk": lambda: f"{n.by} k={n.k}"}.get(n.kind, lambda: "")()
+                     "agg": lambda: f"keys={n.keys}", "topk": lambda: f"{n.by} k={n.k}",
+                     "stateful": lambda: getattr(n.executor, "explain", lambda: "")()}.get(n.kind, lambda: "")()
             print("  " * d + f"{n.kind} {extra} -> {n.schema}")
             for p in n.parents:
                 walk(p, d + 1)
@@ -1009,3 +1010,27 @@ class OrderedStream(DataStream):
         assert left_by is not None and right_by is not None, "Must specify by or left_by and right_by"
         node = AsofNode(self.node, right.node, left_on, right_on, left_by, right_by, suffix)
         return OrderedStream(self.quokka_context, node, self.sorted_by)
+
+    def pattern_recognize(self, time_col, events, maxspan, by):
+        """Complex event recognition per key (pyquokka/orderedstream.py:37-53).  `events` = [(name, predicate)], 2 to 8 of them;
+        a predicate is a SQL boolean over the row's columns (plain or qualified by the event's own name) that may read the rows
+        bound to earlier events as `name.col`; only the first event may have predicate None (every row).  Within one key, in time
+        order, a match is rows r0, r1, ..., r(m-1) with each r_i satisfying event i, times strictly increasing from one event to
+        the next and t(r(m-1)) <= t(r0) + maxspan (an int in the time column's unit or a datetime.timedelta); rows in between are
+        skipped.  One output row per start row r0 that has a match: `by`, then one column per event holding the time of its row
+        in the match with the lexicographically smallest (t1, ..., t(m-1)); ordered by key, then start time, per channel.  A
+        predicate that reads a NULL is false.
+        Deviations from the reference: the output schema (the reference declares [event_number, first_event_timestamp,
+        last_event_timestamp] and never produces it); consecutive events need strictly increasing times; matches span batch
+        boundaries; a start row is never re-used as a later event."""
+        from .executors import CEPExecutor
+        if by is None:
+            raise Exception("You must specify a key by column for pattern_recognize currently.")
+        assert self.sorted_by is not None and time_col == self.sorted_by, "pattern_recognize: time_col must be the column the stream is sorted by"
+        assert by in self.schema, f"pattern_recognize: by column {by!r} not in schema"
+        ex = CEPExecutor(self.schema, events, time_col, maxspan, by)
+        _reject_vectors(self.node.vectors, ex.touched_columns, "pattern_recognize")
+        src = self.node if ex.prefilter is None else FilterNode(self.node, ex.prefilter)
+        node = StatefulNode({0: src}, ex, [by] + ex.names, {0: sorted(ex.touched_columns)}, {0: HashPartitioner(by)},
+                            CustomChannelsStrategy(1))
+        return OrderedStream(self.quokka_context, node, ex.names[0])

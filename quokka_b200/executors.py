@@ -1224,54 +1224,39 @@ class SortedAsofExecutor(Executor):
 
 
 # ---------------------------------------------------------------------------------------------- time-series windows
-class _WindowExecutor(Executor):
-    """Common part of the three window executors (pyquokka/executors/ts_executors.py:12-288): the stream arrives sorted by
-    time and hash-partitioned by the `by` column; the rows are segmented by key with the stable partition kernel (time order
-    survives inside a key) and the window kernel of the subclass runs over the segments.  The windows are evaluated when the
-    channel's input is complete (done()): the same rows, whatever the batching -- the reference's incremental emission
-    loses rows of hopping windows across batch boundaries (ts_executors.py:41-58 keeps only rows past the last complete
-    window although earlier rows still belong to later windows)."""
+class _KeySegmented(Executor):
+    """Input handling shared by the done-time operators over an OrderedStream hash-partitioned by a key (the windows, the
+    pattern search): batches are kept per source rank in arrival order (ranks hold consecutive time ranges), put back together
+    and checked to be time-sorted, and the rows are segmented by key with the stable partition kernel, so time order survives
+    inside a key."""
 
-    silent_streams = "all"       # windows are evaluated when the channel's input is complete
+    silent_streams = "all"       # the answer is computed when the channel's input is complete
 
-    def __init__(self, time_col, by_col, window, trigger) -> None:
-        from .windowtypes import Trigger, Window
-        assert issubclass(type(window), Window) and issubclass(type(trigger), Trigger)
-        self.time_col, self.by_col, self.window, self.trigger = time_col, by_col, window, trigger
-        self.state = None
-        self._parts = {}             # source rank -> batches in arrival order (ranks hold consecutive time ranges)
+    def _init_segments(self):
+        self._parts = {}             # source rank -> batches in arrival order
         self._codes = SortedAsofExecutor()      # only for its append-only symbol codes
 
     def execute(self, batches, stream_id, executor_id):
         for b in _clean(batches):
             self._parts.setdefault(getattr(b, "src_rank", 0) or 0, []).append(b)
 
-    def _segmented(self):
-        """(time, by codes, seg, n_by, fp64 value columns, aggregate list, decode) in key-segmented order, or None."""
+    def _sorted_input(self, time_col: str, who: str):
+        """(the whole input as one table, its time column as int64), or None when nothing arrived."""
         parts = [b for r in sorted(self._parts) for b in self._parts[r]]
         self._parts = {}
         if not parts:
             return None
         t = concat_tables(parts)
-        tcol = t[self.time_col]
-        time = tcol.data.to(torch.int64)
+        time = t[time_col].data.to(torch.int64)
         if len(time) > 1 and not bool((time[1:] >= time[:-1]).all().item()):
-            raise L.QkError("windowed_transform: the stream is not sorted by " + self.time_col)
-        bycol = t[self.by_col]
-        codes = self._codes._stable_codes(bycol)
+            raise L.QkError(f"{who}: the stream is not sorted by " + time_col)
+        return t, time
+
+    def _segment(self, codes: torch.Tensor, columns: list):
+        """(columns moved into key-segmented order, segment starts int64[n_by + 1], n_by)."""
         n_by = max(1, self._codes._n_by)
-        aggs = self.window.parsed()
-        exprs, vals = [], []
-        for _, op, arg in aggs:                                   # one fp64 column per distinct argument expression
-            if arg is not None and arg.sql() not in exprs:
-                exprs.append(arg.sql())
-                e = EdgeOps(None, {"__v": arg}).apply(t.select(sorted(arg.columns(), key=t.column_names.index)), stable=True)
-                vals.append(to_f64(e["__v"].data))
         dest, seg = ops.partition_plan(codes, n_by, L.PART_CODE)
-        moved = ops.scatter([time, codes] + vals, dest)
-        spec = [(name, op, exprs.index(arg.sql()) if arg is not None else -1) for name, op, arg in aggs]
-        unit = str(tcol.arrow_type.unit) if tcol.arrow_type is not None and pa_is_timestamp(tcol.arrow_type) else None
-        return moved[0], moved[1], seg, n_by, moved[2:], spec, (bycol, tcol, unit)
+        return ops.scatter(columns, dest), seg, n_by
 
     def _by_column(self, codes: torch.Tensor, bycol: DeviceColumn) -> DeviceColumn:
         if self._codes._values is not None:
@@ -1280,6 +1265,43 @@ class _WindowExecutor(Executor):
 
     def _time_column(self, time: torch.Tensor, tcol: DeviceColumn) -> DeviceColumn:
         return DeviceColumn(time.to(tcol.data.dtype), None, tcol.arrow_type)
+
+
+class _WindowExecutor(_KeySegmented):
+    """Common part of the three window executors (pyquokka/executors/ts_executors.py:12-288): the stream arrives sorted by
+    time and hash-partitioned by the `by` column; the rows are segmented by key with the stable partition kernel (time order
+    survives inside a key) and the window kernel of the subclass runs over the segments.  The windows are evaluated when the
+    channel's input is complete (done()): the same rows, whatever the batching -- the reference's incremental emission
+    loses rows of hopping windows across batch boundaries (ts_executors.py:41-58 keeps only rows past the last complete
+    window although earlier rows still belong to later windows)."""
+
+    def __init__(self, time_col, by_col, window, trigger) -> None:
+        from .windowtypes import Trigger, Window
+        assert issubclass(type(window), Window) and issubclass(type(trigger), Trigger)
+        self.time_col, self.by_col, self.window, self.trigger = time_col, by_col, window, trigger
+        self.state = None
+        self._init_segments()
+
+    def _segmented(self):
+        """(time, by codes, seg, n_by, fp64 value columns, aggregate list, decode) in key-segmented order, or None."""
+        got = self._sorted_input(self.time_col, "windowed_transform")
+        if got is None:
+            return None
+        t, time = got
+        tcol = t[self.time_col]
+        bycol = t[self.by_col]
+        codes = self._codes._stable_codes(bycol)
+        aggs = self.window.parsed()
+        exprs, vals = [], []
+        for _, op, arg in aggs:                                   # one fp64 column per distinct argument expression
+            if arg is not None and arg.sql() not in exprs:
+                exprs.append(arg.sql())
+                e = EdgeOps(None, {"__v": arg}).apply(t.select(sorted(arg.columns(), key=t.column_names.index)), stable=True)
+                vals.append(to_f64(e["__v"].data))
+        moved, seg, n_by = self._segment(codes, [time, codes] + vals)
+        spec = [(name, op, exprs.index(arg.sql()) if arg is not None else -1) for name, op, arg in aggs]
+        unit = str(tcol.arrow_type.unit) if tcol.arrow_type is not None and pa_is_timestamp(tcol.arrow_type) else None
+        return moved[0], moved[1], seg, n_by, moved[2:], spec, (bycol, tcol, unit)
 
 
 def pa_is_timestamp(t) -> bool:
@@ -1386,3 +1408,126 @@ class SessionWindowExecutor(_HashedWindow):
         cols = {self.by_col: self._by_column(codes[at], bycol), self.time_col: self._time_column(time[at], tcol)}
         cols.update(out)
         return DeviceTable(cols)
+
+
+# ---------------------------------------------------------------------------------------------- pattern recognition
+class CEPExecutor(_KeySegmented):
+    """OrderedStream.pattern_recognize (pyquokka/executors/cep_executors.py:13-181; the reference's constructor order, plus `by`).
+    Per key, in time order, every row r0 satisfying event 0 that starts at least one match -- rows r0 < r1 < ... < r(m-1) with
+    strictly increasing times, t(r(m-1)) <= t(r0) + max_span and event i's predicate true with r0 .. r(i-1) bound to the earlier
+    names -- gives one output row: the key and the times of the match whose (t1 .. t(m-1)) is lexicographically smallest.
+    Done-time: the channel's rows are segmented by key, the row-local conjuncts of every event are evaluated by the scan kernel
+    into a candidate mask, and qk_pattern_search runs the search.  A predicate that reads a NULL is false.
+    `touched_columns` and `prefilter` (the OR of the events' row-local parts, pushed to the scan by the planner) as in the reference."""
+
+    BUDGET = 1 << 24             # rows one start may test before the search gives up on it and the query fails
+
+    def __init__(self, schema, events, time_col, max_span, by) -> None:
+        import datetime
+        if isinstance(max_span, bool) or not isinstance(max_span, (int, datetime.timedelta)):
+            raise E.ExprError("maxspan must be an int in the time column's unit or a datetime.timedelta")
+        if (max_span.total_seconds() if isinstance(max_span, datetime.timedelta) else max_span) < 0:
+            raise E.ExprError("maxspan must be >= 0")
+        assert time_col in schema and by in schema
+        self.time_col, self.by_col, self.max_span = time_col, by, max_span
+        self.preds = E.split_pattern(events, schema, by)
+        self.names = list(self.preds.names)
+        self.touched_columns = set(self.preds.columns) | {time_col, by}
+        self.prefilter = E.pattern_prefilter(self.preds)
+        E.compile_links(self.preds)              # the link programs' errors while the plan is built, not after the input is read
+        self._init_segments()
+
+    def explain(self) -> str:
+        ev = ", ".join(f"{n}: {'*' if lo is None and li is None else ' and '.join(x.sql() for x in (lo, li) if x is not None)}"
+                       for n, lo, li in zip(self.names, self.preds.local, self.preds.link))
+        return f"pattern_recognize [{ev}] maxspan={self.max_span} by={self.by_col}"
+
+    def _ticks(self, tcol: DeviceColumn) -> int:
+        import datetime
+        from .windowtypes import Window
+        if isinstance(self.max_span, datetime.timedelta) and tcol.arrow_type is not None and pa.types.is_date32(tcol.arrow_type):
+            days = self.max_span / datetime.timedelta(days=1)
+            if not float(days).is_integer():
+                raise E.ExprError("maxspan over a date column must be a whole number of days")
+            return int(days)
+        unit = str(tcol.arrow_type.unit) if tcol.arrow_type is not None and pa_is_timestamp(tcol.arrow_type) else None
+        return Window.ticks(self.max_span, unit)
+
+    def _empty(self, tcol: DeviceColumn, bycol: DeviceColumn, dev) -> DeviceTable:
+        none = torch.empty(0, dtype=torch.int64, device=dev)
+        return DeviceTable({self.by_col: self._by_column(none.to(torch.int32), bycol)} |
+                           {n: self._time_column(none, tcol) for n in self.names})
+
+    def search_inputs(self, t: DeviceTable, time: torch.Tensor) -> dict:
+        """The arguments of ops.pattern_search for the rows of `t` (time = its time column as int64): the rows segmented by key,
+        the candidate mask from the row-local conjuncts, the start rows and the link programs.  None when no row starts a match."""
+        tcol, bycol = t[self.time_col], t[self.by_col]
+        codes = self._codes._stable_codes(bycol)
+        read = sorted(self.preds.columns, key=t.column_names.index)
+        plain, mask_of = t.select(read).split_validity()
+        hidden = sorted(set(mask_of.values()))
+        names = read + hidden
+        moved, seg, n_by = self._segment(codes, [time, codes] + [plain[c].data for c in names])
+        stime, scodes = moved[0], moved[1]
+        seg_t = DeviceTable({c: DeviceColumn(d, plain[c].dictionary, plain[c].arrow_type) for c, d in zip(names, moved[2:])})
+        dev, m, n = stime.device, len(self.names), len(stime)
+        # ---- row-local conjuncts: one scan projection per event, packed into the candidate mask (bit e: may bind event e)
+        cand = torch.zeros(n, dtype=torch.uint8, device=dev)
+        local = {}
+        for e, node in enumerate(self.preds.local):
+            if node is None:
+                cand |= 1 << e
+                continue
+            nulls = sorted({mask_of[c] for c in node.columns() if c in mask_of})
+            local[e] = E.and_all([node] + [E.binop("!=", E.col(h), E.num(0)) for h in nulls])
+        if local and n:
+            used = sorted(set().union(*[x.columns() for x in local.values()]), key=names.index)
+            sub = seg_t.select(used)
+            sch = sub.schema_info()
+            progs = {e: E.compile_expr(x, sch) for e, x in local.items()}
+            groups, cur = [], []
+            for e in progs:                                   # as many projections per scan call as its limits take
+                if cur and sum(len(progs[k]) for k in cur) + len(progs[e]) > L.MAX_TOTAL_NODES:
+                    groups.append(cur)
+                    cur = []
+                cur.append(e)
+            groups.append(cur)
+            for g in groups:
+                outs, _ = ops.scan_filter_project([sub[c].data for c in used], None, [progs[e] for e in g], stable=True)
+                for e, o in zip(g, outs):
+                    cand |= (o != 0).to(torch.uint8) << e
+        starts = torch.nonzero(cand & 1).flatten().to(torch.int32)
+        if starts.numel() == 0:
+            return None
+        # ---- link conjuncts: one program per event over the columns they read
+        lcols, links = E.compile_links(self.preds, seg_t.schema_info())
+        return dict(time=stime, by=scodes, seg=seg, n_by=n_by, cand=cand, starts=starts, m=m, maxspan=self._ticks(tcol),
+                    link_cols=[seg_t[c].data for c in lcols], link_valid=[seg_t[mask_of[c]].data if c in mask_of else None for c in lcols],
+                    links=links, budget=self.BUDGET)
+
+    def done(self, executor_id):
+        got = self._sorted_input(self.time_col, "pattern_recognize")
+        if got is None:
+            return None
+        t, time = got
+        tcol, bycol = t[self.time_col], t[self.by_col]
+        a = self.search_inputs(t, time)
+        if a is None:
+            return self._empty(tcol, bycol, time.device)
+        starts, stime, scodes = a["starts"], a["time"], a["by"]
+        try:
+            bound = ops.pattern_search(**a)
+        except ops.PatternBudgetError as err:
+            r = int(starts[err.index].item())
+            code = int(scodes[r].item())
+            key = self._codes._values[code] if self._codes._values is not None else code
+            raise L.QkError(f"pattern_recognize: the search from the row of key {key!r} at time {int(stime[r].item())} tested more "
+                            f"than {self.BUDGET} rows; narrow the pattern (maxspan, more selective predicates)") from err
+        keep = torch.nonzero(bound[:, 0] >= 0).flatten()
+        bound = bound[keep]
+        if bound.shape[0] == 0:
+            return self._empty(tcol, bycol, time.device)
+        out = {self.by_col: self._by_column(ops.gather([scodes], bound[:, 0].contiguous())[0], bycol)}
+        for e, name in enumerate(self.names):
+            out[name] = self._time_column(ops.gather([stime], bound[:, e].contiguous())[0], tcol)
+        return DeviceTable(out)

@@ -646,3 +646,142 @@ def check_call(ncols: int, pred, exprs, who: str = "scan") -> None:
                 raise ExprError(f"{who}: column slot out of range in expression {k}")
     if total > L.MAX_TOTAL_NODES:
         raise ExprError(f"{who}: programs hold {total} nodes in total; one kernel call takes at most {L.MAX_TOTAL_NODES}")
+
+
+# ------------------------------------------------------------------ pattern predicates (OrderedStream.pattern_recognize)
+@dataclass
+class PatternPredicates:
+    """The events of a pattern, split the way the search runs them.  local[e]: the conjuncts of event e that read only the row
+    being bound (plain column names), or None = every row; link[e]: the conjuncts that read an earlier event's row, whose columns
+    are `name.col` (that event's bound row) or `col` (the row being bound), or None."""
+    names: list
+    local: list
+    link: list
+    columns: set
+
+
+def split_pattern(events, schema, by: str) -> PatternPredicates:
+    """Resolves the `name.col` qualifiers of every event predicate (the event's own name = the row being bound, an earlier
+    event's name = that event's bound row) and splits each predicate into row-local and link conjuncts (the reference's
+    event_prefilters / event_dependent_filters, pyquokka/executors/cep_executors.py:35-75).  A reference to a later event, an
+    unknown event or column, a repeated or malformed name, or a missing predicate after the first event is an ExprError."""
+    events = list(events)
+    if not 2 <= len(events) <= L.PATTERN_MAX_EVENTS:
+        raise ExprError(f"a pattern has 2 to {L.PATTERN_MAX_EVENTS} events, got {len(events)}")
+    names = []
+    for ev in events:
+        if not (isinstance(ev, (tuple, list)) and len(ev) == 2):
+            raise ExprError("every event is a (name, predicate) pair")
+        name = ev[0]
+        if not isinstance(name, str) or not re.fullmatch(r"[A-Za-z_][A-Za-z_0-9]*", name):
+            raise ExprError(f"event name {name!r} must be an identifier without '.'")
+        if name in names:
+            raise ExprError(f"event name {name!r} is used for two events")
+        if name == by:
+            raise ExprError(f"event name {name!r} equals the `by` column")
+        names.append(name)
+    schema = set(schema)
+    local, link, columns = [], [], set()
+    for i, (name, pred) in enumerate(events):
+        if pred is None:
+            if i > 0:
+                raise ExprError(f"event {name!r}: only the first event may have no predicate")
+            local.append(None)
+            link.append(None)
+            continue
+        node = parse(pred) if isinstance(pred, str) else getattr(pred, "node", pred)
+        if not isinstance(node, Node):
+            raise ExprError(f"event {name!r}: a predicate is a SQL string or an Expression")
+
+        def resolve(n):
+            if n.kind != "col":
+                return Node(n.kind, n.value, tuple(resolve(a) for a in n.args)) if n.args else n
+            q, c = n.value.split(".", 1) if "." in n.value else (None, n.value)
+            if q is not None and q != name:
+                if q not in names:
+                    raise ExprError(f"event {name!r}: {n.value!r} names no event")
+                if names.index(q) > i:
+                    raise ExprError(f"event {name!r}: {n.value!r} refers to the later event {q!r}")
+            if c not in schema:
+                raise ExprError(f"event {name!r}: unknown column {c!r}")
+            columns.add(c)
+            return col(c if q is None or q == name else f"{q}.{c}")
+
+        terms = conjuncts(resolve(node))
+        loc = [t for t in terms if not any("." in c for c in t.columns())]
+        lnk = [t for t in terms if any("." in c for c in t.columns())]
+        local.append(and_all(loc))
+        link.append(and_all(lnk))
+    return PatternPredicates(names, local, link, columns)
+
+
+def pattern_prefilter(p: PatternPredicates):
+    """The OR of the events' row-local parts (cep_executors.py:77-81): a row it rejects can bind no event.  None when an event
+    has no row-local part, or when the parts read different columns -- a filter over a column that may hold NULLs drops every
+    row where it reads one, which is only right when every event would read that column too."""
+    if any(x is None for x in p.local) or len({frozenset(x.columns()) for x in p.local}) != 1:
+        return None
+    out = None
+    for x in p.local:
+        out = x if out is None else binop("or", out, x)
+    return out
+
+
+def compile_link(e: Node, ev: int, names: list, slots: dict, schema: dict) -> list:
+    """Postfix program of event `ev`'s link conjuncts for qk_pattern_search: QK_OP_COL a0 = slots[column], a1 = the event whose
+    bound row is read (ev for the row being bound).  Only arithmetic, NEG, the float compares, AND / OR / NOT and CASE, in fp64;
+    string columns and literals are rejected."""
+    out: list = []
+
+    def emit(n: Node):
+        k = n.kind
+        if k == "col":
+            q, c = n.value.split(".", 1) if "." in n.value else (names[ev], n.value)
+            if names.index(q) > ev:
+                raise ExprError(f"event {names[ev]!r}: {n.value!r} refers to a later event")
+            info = schema[c]
+            if info.dictionary is not None:
+                raise ExprError(f"event {names[ev]!r}: string column {c!r} cannot be read across events")
+            out.append((L.OP_COL, slots[c], names.index(q), 0.0, 0))
+        elif k in ("num", "date"):
+            out.append((L.OP_CONST, 0, 0, float(n.value), 0))
+        elif k == "un":
+            emit(n.args[0])
+            out.append((L.OP_NEG if n.value == "neg" else L.OP_NOT, 0, 0, 0.0, 0))
+        elif k == "bin" and n.value in _ARITH:
+            emit(n.args[0]); emit(n.args[1])
+            out.append((_ARITH[n.value], 0, 0, 0.0, 0))
+        elif k == "bin" and n.value in _FCMP:
+            emit(n.args[0]); emit(n.args[1])
+            out.append((_FCMP[n.value], 0, 0, 0.0, 0))
+        elif k == "bin" and n.value in ("and", "or"):
+            emit(n.args[0]); emit(n.args[1])
+            out.append((L.OP_AND if n.value == "and" else L.OP_OR, 0, 0, 0.0, 0))
+        elif k == "func" and n.value == "case":
+            for a in n.args:
+                emit(a)
+            out.append((L.OP_SELECT, 0, 0, 0.0, 0))
+        else:
+            raise ExprError(f"event {names[ev]!r}: {n.sql()} is not supported in a predicate that reads an earlier event "
+                            "(arithmetic, comparisons, AND / OR / NOT and CASE over numeric columns)")
+
+    emit(e)
+    check_program(out, f"event {names[ev]!r}")
+    return out
+
+
+def compile_links(p: PatternPredicates, schema: dict | None = None):
+    """(link columns, one program per event) for qk_pattern_search, with the limits the kernel enforces: at most QK_MAX_COLS link
+    columns and PATTERN_MAX_LINK_NODES nodes over all programs.  schema = None checks a plan before any row has arrived: every
+    column is taken as numeric, so only a string column is left to be found when the rows' types are known."""
+    lcols = sorted({c.split(".", 1)[-1] for x in p.link if x is not None for c in x.columns()})
+    if len(lcols) > L.MAX_COLS:
+        raise ExprError(f"pattern: predicates that read earlier events read {len(lcols)} columns; at most {L.MAX_COLS}")
+    if schema is None:
+        schema = {c: ColumnInfo(i, L.QK_F64) for i, c in enumerate(lcols)}
+    slots = {c: i for i, c in enumerate(lcols)}
+    links = [compile_link(x, e, p.names, slots, schema) if x is not None else [] for e, x in enumerate(p.link)]
+    total = sum(len(x) for x in links)
+    if total > L.PATTERN_MAX_LINK_NODES:
+        raise ExprError(f"pattern: predicates that read earlier events compile to {total} nodes; at most {L.PATTERN_MAX_LINK_NODES}")
+    return lcols, links

@@ -799,3 +799,56 @@ def knn_merge(a_score: torch.Tensor, a_key: torch.Tensor, b_score: torch.Tensor,
     L.check(L.lib().qk_knn_merge(q, a_score.data_ptr(), a_key.data_ptr(), a_score.shape[1], b_score.data_ptr(), b_key.data_ptr(),
                                  b_score.shape[1], k, os_.data_ptr(), ok.data_ptr(), src.data_ptr(), _stream()), "qk_knn_merge")
     return os_, ok, src
+
+
+# ------------------------------------------------------------------ K12 pattern search
+class PatternBudgetError(L.QkError):
+    """A start tested more rows than the step budget of qk_pattern_search allows; `index` is its position in `starts`."""
+
+    def __init__(self, msg: str, index: int):
+        super().__init__(msg)
+        self.index = int(index)
+
+
+def pattern_search(time: torch.Tensor, by: torch.Tensor, seg: torch.Tensor, n_by: int, cand: torch.Tensor, starts: torch.Tensor, m: int,
+                   maxspan: int, link_cols: Sequence[torch.Tensor], link_valid: Sequence[torch.Tensor | None], links: Sequence[Program],
+                   budget: int, rows_tested: torch.Tensor | None = None) -> torch.Tensor:
+    """qk_pattern_search over key-segmented rows: int32 [len(starts), m], the rows of each start's lexicographically smallest
+    match (-1 rows: no match).  link_valid[c]: a uint8 row mask (0 = NULL) of link column c, or None.  links: m programs, the
+    first empty.  rows_tested: a device int64[1] that accumulates the rows tested.  Raises PatternBudgetError when a start
+    tests more than `budget` rows."""
+    n_starts = starts.numel()
+    dev = time.device
+    out = torch.empty((n_starts, m), dtype=torch.int32, device=dev)
+    status = torch.empty(L.PATTERN_STATUS_WORDS, dtype=torch.int64, device=dev)
+    lc = cols(link_cols, "link column")
+    for i, v in enumerate(link_valid):
+        if v is not None:
+            _require_cuda(v, "link validity")
+            if v.dtype != torch.uint8 or v.numel() != link_cols[i].numel():
+                raise L.QkError("pattern_search: a validity mask must be uint8 with one entry per row")
+            lc[i].validity = v.data_ptr()
+    if len(links) != m:
+        raise L.QkError(f"pattern_search: {len(links)} link programs for {m} events")
+    for k, prog in enumerate(links):
+        E.check_program(prog or [], f"pattern_search: link program {k}")
+    progs = _Progs(list(links), dev)
+    tc, bc = col(time, "time"), col(by, "key")
+    for t, what in ((seg, "segments"), (cand, "candidate mask"), (starts, "starts")):
+        _require_cuda(t, what)
+    if seg.dtype != torch.int64 or cand.dtype != torch.uint8 or starts.dtype != torch.int32:
+        raise L.QkError("pattern_search: seg must be int64, cand uint8 and starts int32")
+    n = time.numel()
+    if by.numel() != n or cand.numel() != n:
+        raise L.QkError(f"pattern_search: time has {n} rows, the key {by.numel()} and the candidate mask {cand.numel()}")
+    if seg.numel() != int(n_by) + 1:
+        raise L.QkError(f"pattern_search: {seg.numel()} segment offsets for {n_by} keys (expected n_by + 1)")
+    L.check(L.lib().qk_pattern_search(C.byref(tc), C.byref(bc), seg.data_ptr(), int(n_by), cand.data_ptr() if cand.numel() else None,
+                                      starts.data_ptr() if n_starts else None, n_starts, int(m), int(maxspan), lc, len(link_cols),
+                                      progs.arr, int(budget), out.data_ptr() if n_starts else None, status.data_ptr(),
+                                      rows_tested.data_ptr() if rows_tested is not None else None, _stream()), "qk_pattern_search")
+    over, first = (int(x) for x in status[:2].tolist())
+    if over:
+        idx = n_starts - first
+        raise PatternBudgetError(f"pattern_search: {over} start(s) tested more than {budget} rows; the first is start {idx}", idx)
+    return out
