@@ -231,15 +231,6 @@ QK_API size_t qk_partition_workspace_bytes(int64_t nrows, int32_t nparts);
 QK_API int qk_partition_plan(const qk_column* key, int32_t nparts, int32_t mode, int32_t* dest,
                       int64_t* part_offsets, void* workspace, size_t ws_bytes, void* stream);
 QK_API int qk_scatter(const qk_column* cols, int32_t ncols, const int32_t* dest, qk_column* out, void* stream);
-/* Fused partition-scatter + shuffle over peer memory (replaces qk_scatter + the all-to-all of
- * TaskManager.push, pyquokka/core.py:276-376, when the ranks' mailboxes are mapped into each other's address
- * space): row i is stored directly into peer p's receive column at row peer_row_off[p] + (dest[i] -
- * part_offsets[p]), p being the partition dest[i] falls in.  peer_col_ptrs = HOST array [nparts][ncols] of device
- * pointers (peer-mapped, e.g. symmetric memory); peer_row_off = HOST array [nparts].  The caller separates
- * successive uses of a mailbox with a cross-rank barrier. */
-#define QK_MAX_PEERS 16
-QK_API int qk_scatter_peer(const qk_column* cols, int32_t ncols, const int32_t* dest, const int64_t* part_offsets, int32_t nparts,
-                           const uint64_t* peer_col_ptrs, const int64_t* peer_row_off, void* stream);
 /* ---- K6: the shuffle over peer-mapped memory ------------------------------------------------------
  * Replaces TaskManager.push -> Flight do_put / do_get (pyquokka/core.py:276-376, pyquokka/flight.py:44-264): one
  * process per GPU, every rank owns a CHANNEL = a control block (qk_xchg_ctrl_bytes(), zeroed once) + a mailbox, both
@@ -263,7 +254,8 @@ QK_API int qk_scatter_peer(const qk_column* cols, int32_t ncols, const int32_t* 
  * qk_xchg_recv: waits until every peer's rows of this epoch have landed, then copies column c (out[c].length
  *   rows from byte offset src_byte_off[c] of the own mailbox, 16-byte aligned) into out[c].
  * A row of column c is size(dtype) * max(1, lanes) bytes: qk_xchg_push and qk_xchg_recv move vector columns (lanes > 1);
- * qk_xchg_push_scatter returns QK_ERR_UNSUPPORTED for them. */
+ * qk_xchg_push_scatter returns QK_ERR_UNSUPPORTED for them.  A link has at most QK_MAX_PEERS ranks. */
+#define QK_MAX_PEERS 16
 #define QK_XCHG_META_WORDS 48
 #define QK_XCHG_CTRL_BYTES 16384
 typedef struct qk_xchg {

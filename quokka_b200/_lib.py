@@ -108,7 +108,6 @@ _SIGNATURES = {
     "qk_partition_plan": (C.c_int, [_P(qk_column), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_size_t, C.c_void_p]),
     "qk_scatter": (C.c_int, [_P(qk_column), C.c_int32, C.c_void_p, _P(qk_column), C.c_void_p]),
-    "qk_scatter_peer": (C.c_int, [_P(qk_column), C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, _P(C.c_uint64), _P(C.c_int64), C.c_void_p]),
     "qk_xchg_ctrl_bytes": (C.c_size_t, []),
     "qk_xchg_meta": (C.c_int, [_P(qk_xchg), C.c_uint64, C.c_void_p, _P(C.c_int64), C.c_void_p, C.c_void_p, C.c_void_p]),
     "qk_xchg_push": (C.c_int, [_P(qk_xchg), C.c_uint64, _P(qk_column), C.c_int32, _P(C.c_int64), _P(C.c_int64), _P(C.c_int64), C.c_void_p]),

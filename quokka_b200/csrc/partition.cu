@@ -225,37 +225,6 @@ __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ MoveArgs
     }
 }
 
-// Scatter straight into the receivers' memory: row i of this rank goes to partition p (found from its
-// position `dest[i]` in the partition-ordered output), i.e. to peer p, at row peer_row_off[p] + rank-in-partition
-// of that peer's receive column.  One pass over the payload does the local re-ordering AND the transfer: the
-// stores travel over NVLink (or stay local for p == my rank).  Replaces qk_scatter + an NCCL all-to-all.
-struct PeerArgs {
-    const void* src[QK_MAX_COLS];
-    unsigned long long dst[QK_MAX_PEERS][QK_MAX_COLS];   // device-mapped pointers into every peer's mailbox
-    long long row_off[QK_MAX_PEERS];
-    int8_t width[QK_MAX_COLS];
-    int32_t ncols, nparts;
-};
-
-__global__ void __launch_bounds__(256) k_scatter_peer(const __grid_constant__ PeerArgs P, const int32_t* dest, const int64_t* part_offsets, int64_t n) {
-    __shared__ long long off[QK_MAX_PEERS + 1];
-    if (threadIdx.x <= P.nparts) off[threadIdx.x] = part_offsets[threadIdx.x];
-    __syncthreads();
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const long long d = dest[i];
-        int p = 0;
-        while (p + 1 < P.nparts && d >= off[p + 1]) ++p;
-        const long long r = d - off[p] + P.row_off[p];
-        for (int c = 0; c < P.ncols; ++c) {
-            switch (P.width[c]) {
-                case 1: ((uint8_t*)P.dst[p][c])[r] = ((const uint8_t*)P.src[c])[i]; break;
-                case 4: ((uint32_t*)P.dst[p][c])[r] = ((const uint32_t*)P.src[c])[i]; break;
-                default: ((uint64_t*)P.dst[p][c])[r] = ((const uint64_t*)P.src[c])[i]; break;
-            }
-        }
-    }
-}
-
 int fill_move(MoveArgs& M, const qk_column* cols, int ncols, qk_column* out, int64_t n_src, int64_t n_dst, const char* who) {
     if (ncols < 0 || ncols > QK_MAX_COLS) QK_FAIL(QK_ERR_INVALID, "%s: ncols out of range", who);
     M.ncols = ncols;
@@ -454,31 +423,5 @@ extern "C" int qk_gather(const qk_column* cols, int32_t ncols, const int32_t* id
     if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
     k_gather<<<(unsigned)nb, 256, 0, st>>>(M, idx, n_idx);
     QK_LAUNCH_CHECK("k_gather");
-    return QK_OK;
-}
-
-extern "C" int qk_scatter_peer(const qk_column* cols, int32_t ncols, const int32_t* dest, const int64_t* part_offsets, int32_t nparts,
-                               const uint64_t* peer_col_ptrs, const int64_t* peer_row_off, void* stream) {
-    const char* who = "qk_scatter_peer";
-    if (ncols < 1 || ncols > QK_MAX_COLS || nparts < 1 || nparts > QK_MAX_PEERS) QK_FAIL(QK_ERR_INVALID, "%s: ncols / nparts out of range", who);
-    if (!cols || !part_offsets || !peer_col_ptrs || !peer_row_off) QK_FAIL(QK_ERR_INVALID, "%s: null arguments", who);
-    static thread_local PeerArgs P;
-    const int64_t n = cols[0].length;
-    for (int c = 0; c < ncols; ++c) {
-        if (int rc = check_col(&cols[c], who)) return rc;
-        if (cols[c].length != n) QK_FAIL(QK_ERR_INVALID, "%s: column %d length mismatch", who, c);
-        P.src[c] = cols[c].data; P.width[c] = (int8_t)dtype_size(cols[c].dtype);
-    }
-    for (int p = 0; p < nparts; ++p) {
-        P.row_off[p] = peer_row_off[p];
-        for (int c = 0; c < ncols; ++c) P.dst[p][c] = peer_col_ptrs[(size_t)p * ncols + c];
-    }
-    P.ncols = ncols; P.nparts = nparts;
-    if (n == 0) return QK_OK;
-    if (!dest) QK_FAIL(QK_ERR_INVALID, "%s: null dest", who);
-    int64_t nb = (n + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_scatter_peer<<<(unsigned)nb, 256, 0, (cudaStream_t)stream>>>(P, dest, part_offsets, n);
-    QK_LAUNCH_CHECK("k_scatter_peer");
     return QK_OK;
 }

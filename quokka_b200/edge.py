@@ -460,8 +460,9 @@ class PartialAgg:
 # ------------------------------------------------------------------ partitioners
 class Parts:
     """Output of a hash partition: the rows of one table grouped by target channel.  The grouping is kept
-    LAZY -- `pending` = (unpartitioned table, dest, device offsets) -- so that the exchange can either scatter
-    locally and send slices (NCCL path) or scatter straight into the peers' memory (peer path)."""
+    LAZY -- `pending` = (unpartitioned table, dest, device offsets) -- so that the exchange can scatter the rows
+    straight into the peers' memory while it sends them (peer-memory link), or group them locally and send one
+    contiguous run per rank (torch.distributed all-to-all)."""
 
     def __init__(self, table: DeviceTable | None, offsets: list | None, pending=None, doffs=None):
         self._table, self._offsets, self.pending = table, offsets, pending
@@ -469,15 +470,11 @@ class Parts:
 
     @property
     def offsets(self) -> list:
-        """Partition boundaries on the HOST.  Read lazily: the peer-memory exchange takes the counts from the device and
-        learns them back with everybody else's (one round trip for both); only the other paths pay this sync."""
+        """Partition boundaries on the HOST.  Read lazily: the peer-memory exchange sends the counts from the device and
+        never reads them here; only the other paths pay this sync."""
         if self._offsets is None:
             self._offsets = self.doffs.cpu().tolist()
         return self._offsets
-
-    @offsets.setter
-    def offsets(self, v):
-        self._offsets = list(v)
 
     @property
     def table(self) -> DeviceTable | None:

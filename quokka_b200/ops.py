@@ -299,16 +299,6 @@ def scatter(columns: Sequence[torch.Tensor], dest: torch.Tensor):
     return outs
 
 
-def scatter_peer(columns: Sequence[torch.Tensor], dest: torch.Tensor, part_offsets: torch.Tensor, peer_col_ptrs: Sequence[Sequence[int]],
-                 peer_row_off: Sequence[int]):
-    """Partition-scatter straight into the peers' mailboxes (qk_scatter_peer)."""
-    nparts, ncols = len(peer_col_ptrs), len(columns)
-    flat = (C.c_uint64 * (nparts * ncols))(*[int(p) for row in peer_col_ptrs for p in row])
-    roff = (C.c_int64 * nparts)(*[int(x) for x in peer_row_off])
-    L.check(L.lib().qk_scatter_peer(cols(columns), ncols, dest.data_ptr(), part_offsets.data_ptr(), nparts, flat, roff, _stream()),
-            "qk_scatter_peer")
-
-
 class XchgChannel:
     """One channel of the peer-memory shuffle (include/qk.h "K6"): this rank's control block + mailbox and the
     peer-mapped addresses of everybody else's.  All ranks call meta / push / recv in the same order on a channel."""

@@ -73,13 +73,6 @@ def _empty(n: int, dt: str, device) -> torch.Tensor:
     return torch.empty((n, lanes) if lanes else n, dtype=t, device=device)
 
 
-def _as_rows(buf: torch.Tensor, dt: str) -> torch.Tensor:
-    """A received byte / element buffer as the column's rows."""
-    t, lanes = _parse_dt(dt)
-    v = buf.view(t)
-    return v.view(-1, lanes) if lanes else v
-
-
 def _flat(t: torch.Tensor) -> torch.Tensor:
     """A dense buffer: 1-D for a scalar column, (n, d) row-major for a vector column (a one-row slice of a 2-D state keeps its
     row stride and reports is_contiguous())."""
@@ -92,42 +85,34 @@ def _flat(t: torch.Tensor) -> torch.Tensor:
     return out
 
 
-class PeerMailbox:
-    """A receive buffer per rank, mapped into every other rank's address space (CUDA IPC / fabric handles
-    through torch symmetric memory), so that the partition kernel of a producer can store rows directly into
-    the consumer's HBM over NVLink: compute (partition-scatter) and collective (all-to-all) in ONE kernel."""
-
-    def __init__(self, device, nbytes: int):
-        import torch.distributed._symmetric_memory as symm
-        self.nbytes = int(nbytes)
-        self.buf = symm.empty(self.nbytes, dtype=torch.uint8, device=device)
-        self.hdl = symm.rendezvous(self.buf, dist.group.WORLD)
-        self.ptrs = [int(p) for p in self.hdl.buffer_ptrs]
-
-    def barrier(self):
-        self.hdl.barrier(channel=0)
+def _checksum(schema) -> int:
+    return (zlib.crc32(repr(schema).encode()) | 1) if schema is not None else 0
 
 
 class NativeLink:
     """The process-wide symmetric allocation behind the peer-memory shuffle (csrc/exchange.cu): `nchannels` channels,
-    each a control block + a mailbox.  Channel 0 belongs to the driver thread, channel 1 + i to pipeline lane i, so
-    that chunks in flight on different CUDA streams never share flags or mailbox space and every channel sees the
-    same sequence of exchanges on every rank."""
+    each a control block + a mailbox.  Every rank's allocation is mapped into every other rank's address space (CUDA IPC
+    / fabric handles through torch symmetric memory), so a producer's kernels store rows straight into the consumers' HBM.
+    Channel 0 belongs to the driver thread, channel 1 + i to pipeline lane i, so that chunks in flight on different CUDA
+    streams never share flags or mailbox space and every channel sees the same sequence of exchanges on every rank."""
 
     CTRL = L.XCHG_CTRL_BYTES
 
     def __init__(self, device, nchannels: int, mailbox_bytes: int):
+        import torch.distributed._symmetric_memory as symm
         mailbox_bytes = (int(mailbox_bytes) + 4095) // 4096 * 4096
         head = (nchannels * self.CTRL + 65535) // 65536 * 65536
-        self.box = PeerMailbox(device, head + nchannels * mailbox_bytes)
-        self.box.buf[:head].zero_()
+        self.buf = symm.empty(head + nchannels * mailbox_bytes, dtype=torch.uint8, device=device)
+        self.hdl = symm.rendezvous(self.buf, dist.group.WORLD)
+        ptrs = [int(p) for p in self.hdl.buffer_ptrs]
+        self.buf[:head].zero_()
         torch.cuda.synchronize(device)
-        self.box.barrier()                                   # every control block is zero before anybody posts
+        self.hdl.barrier(channel=0)                          # every control block is zero before anybody posts
         torch.cuda.synchronize(device)
         w, me = world_size(), rank()
         tmo = int(float(os.environ.get("QK_XCHG_TIMEOUT_S", "120")) * 1000)     # a rank may lag by a first-touch allocation of tens of GB
-        self.channels = [ops.XchgChannel(w, me, [p + i * self.CTRL for p in self.box.ptrs],
-                                         [p + head + i * mailbox_bytes for p in self.box.ptrs], mailbox_bytes, device, tmo)
+        self.channels = [ops.XchgChannel(w, me, [p + i * self.CTRL for p in ptrs],
+                                         [p + head + i * mailbox_bytes for p in ptrs], mailbox_bytes, device, tmo)
                          for i in range(nchannels)]
         self.mailbox_bytes = mailbox_bytes
 
@@ -175,98 +160,160 @@ def native_link(device):
     return _link["obj"]
 
 
-_mailbox = {"obj": None, "failed": False}
+# ------------------------------------------------------------------ the exchange protocol, shared by both transports
+class _SendPlan:
+    """Which rows this rank sends where: rows [lo[d], hi[d]) of `table` go to rank d (a broadcast names the same rows for
+    every rank), or -- `dest` set -- `table` is a hash partition not yet materialised: row i has position dest[i] in the
+    partition order, and `doffs` (device int64[world + 1]) holds where each destination's rows start."""
+
+    def __init__(self, parts, single_owner, w: int):
+        self.table = self.dest = self.doffs = None
+        self.lo, self.hi = [0] * w, [0] * w
+        if isinstance(parts, Parts):
+            if single_owner is None and parts.pending is not None and parts.doffs.numel() == w + 1:
+                if len(parts.pending[0]) > 0:
+                    self.table, self.dest, self.doffs = parts.pending
+            else:
+                t = parts.table
+                if t is not None and len(t) > 0:
+                    self.table = t
+                    if single_owner is not None:
+                        self.hi[single_owner] = len(t)
+                    else:
+                        offs = parts.offsets
+                        for d in range(min(w, len(offs) - 1)):
+                            self.lo[d], self.hi[d] = offs[d], offs[d + 1]
+        else:
+            owner = (lambda c_: single_owner) if single_owner is not None else (lambda c_: c_)
+            by_rank = {}
+            for c_, p_ in sorted(parts.items()):
+                if p_ is not None and len(p_) > 0:
+                    by_rank.setdefault(owner(c_), []).append(p_)
+            flat = [p_ for r in sorted(by_rank) for p_ in by_rank[r]]
+            if flat and all(p_ is flat[0] for p_ in flat) and all(len(v) == 1 for v in by_rank.values()):
+                self.table = flat[0]                              # broadcast / single owner: the same rows to every destination
+                for r in by_rank:
+                    self.hi[r] = len(self.table)
+            elif flat:
+                self.table = concat_tables(flat)
+                pos = 0
+                for r in sorted(by_rank):
+                    self.lo[r] = pos
+                    pos = self.hi[r] = pos + sum(len(p_) for p_ in by_rank[r])
+        self.schema = Exchange._schema_of(self.table) if self.table is not None else None
+
+    @property
+    def counts(self) -> list:
+        """Rows for each destination (zeros for an unmaterialised hash partition: its counts are on the device)."""
+        return [h - l for l, h in zip(self.lo, self.hi)]
 
 
-def peer_mailbox(device, nbytes: int):
-    """Round 1's mailbox for qk_scatter_peer, kept for the collective (NCCL) path's opt-in QK_P2P_LEGACY=1."""
-    if os.environ.get("QK_P2P_LEGACY", "0") != "1" or _mailbox["failed"] or device.type != "cuda" or world_size() == 1:
-        return None
-    if dist.get_backend() != "nccl":
-        return None
-    if _mailbox["obj"] is None:
-        ok = 1
-        try:
-            _mailbox["obj"] = PeerMailbox(device, nbytes)
-        except Exception:
-            ok = 0
-        flag = torch.tensor([ok], device=device, dtype=torch.int32)
-        dist.all_reduce(flag, op=dist.ReduceOp.MIN)              # a rank-local failure must not leave the others in rendezvous
-        if int(flag.item()) == 0:
-            _mailbox["failed"], _mailbox["obj"] = True, None
-            return None
-    return _mailbox["obj"]
+class _Meta:
+    """Every rank's meta row, in one layout for both transports: rows for each destination rank in words [0, w), then
+    from word `head` the header: the checksum of the sender's schema (0: no table), the checksum of the schema it has
+    cached for the edge, the column count and every column's row bytes | _VALID_FLAG when it has a validity mask.  On the
+    link `head` is 16 (qk_xchg_meta may overwrite words [0, w) with the device counts, and the link takes at most
+    QK_MAX_PEERS = 16 ranks); the collective path puts the header after max(16, w) counts."""
+
+    HASH, CACHED, NCOLS, WIDTHS, MAXC = 0, 1, 2, 4, 24
+
+    @classmethod
+    def row(cls, counts: list, mine, cached, head: int) -> list:
+        if mine is not None and len(mine) > cls.MAXC:
+            raise L.QkError(f"exchange: more than {cls.MAXC} columns on one edge")
+        words = [0] * (head + cls.WIDTHS + cls.MAXC)
+        words[:len(counts)] = counts
+        words[head + cls.HASH], words[head + cls.CACHED] = _checksum(mine), _checksum(cached)
+        for i, (_, dt, _, _, hv) in enumerate(mine or []):
+            words[head + cls.WIDTHS + i] = _row_bytes(dt) | (_VALID_FLAG if hv else 0)
+        words[head + cls.NCOLS] = len(mine or [])
+        return words
+
+    def __init__(self, m, w: int, head: int):
+        """m: everybody's row, an integer array [world][words]."""
+        self.counts = m[:, :w]                                    # counts[s][d]: rows rank s sends to rank d
+        self.total = int(self.counts.sum())
+        self.n_recv = [int(self.counts[:, d].sum()) for d in range(w)]
+        self.hash = [int(x) for x in m[:, head + self.HASH]]
+        self.cached = [int(x) for x in m[:, head + self.CACHED]]
+        src = next((r for r in range(w) if int(m[r, head + self.NCOLS]) > 0), None)      # a rank that has a table
+        ncols = int(m[src, head + self.NCOLS]) if src is not None else 0
+        flags = m[:, head + self.WIDTHS: head + self.WIDTHS + ncols]
+        self.col_valid = [bool((flags[:, i] & _VALID_FLAG).any()) for i in range(ncols)]
+        # validity masks travel as extra uint8 columns after the data columns
+        self.widths = [int(flags[src, i]) & _WIDTH_MASK for i in range(ncols)] + [1 for v in self.col_valid if v]
+
+    def sent_bytes(self, me: int) -> int:
+        """Bytes rank `me` sends to other ranks."""
+        return (int(self.counts[me].sum()) - int(self.counts[me, me])) * sum(self.widths)
+
+
+def _recode(c: DeviceColumn, union) -> DeviceColumn:
+    """`c` with its codes re-mapped onto the agreed union dictionary."""
+    if union is None or c.dictionary == union:
+        return c
+    return unify_dictionaries([DeviceColumn(torch.zeros(0, dtype=c.data.dtype, device=c.data.device), union, c.arrow_type), c])[1][1]
+
+
+def _send_columns(table: DeviceTable, schema, col_valid) -> list:
+    """The buffers that cross ranks, one per width of the meta: the columns of `table` in schema order, re-coded onto the
+    agreed dictionaries, then the validity mask of every column that has one on any rank (all ones where this rank's
+    column has none)."""
+    cols, masks = [], []
+    for (name, _, union, _, _), v in zip(schema, col_valid):
+        c = _recode(table[name], union)
+        cols.append(_flat(c.data))
+        if v:
+            masks.append(c.valid if c.valid is not None else torch.ones(len(c), dtype=torch.uint8, device=c.data.device))
+    return cols + masks
+
+
+def _recv_buffers(n: int, schema, col_valid, device) -> list:
+    return [_empty(n, dt, device) for _, dt, _, _, _ in schema] + [torch.empty(n, dtype=torch.uint8, device=device) for v in col_valid if v]
+
+
+def _split(outs: list, schema, col_valid, rows_from) -> list:
+    """The received buffers (in _send_columns order; the rows of rank s after those of ranks < s, rows_from[s] of them)
+    as one DeviceTable per source rank that sent rows."""
+    masks = iter(outs[len(schema):])
+    valid = [next(masks) if v else None for v in col_valid]
+    tables, r0 = [], 0
+    for s_, n in enumerate(rows_from):
+        r1 = r0 + int(n)
+        if r1 > r0:
+            t = DeviceTable({name: DeviceColumn(o[r0:r1], union, atype, None if v is None else v[r0:r1])
+                             for (name, _, union, atype, _), o, v in zip(schema, outs, valid)})
+            t.src_rank = s_              # ordered consumers put the ranks' time ranges back in order with this
+            tables.append(t)
+        r0 = r1
+    return tables
 
 
 class Exchange:
     """All-to-all of partitioned column buffers (the reference's push -> Flight do_put / do_get,
-    core.py:276-376, flight.py:44-264).
+    core.py:276-376, flight.py:44-264), over one of two transports:
 
-    Per call: one small all-gather of the per-destination row counts (+ schema checksums), then one
-    variable-split all-to-all per column (grouped ncclSend / ncclRecv) that moves every column slice straight
-    out of the partition kernel's output -- rows of one destination are already contiguous there, so nothing
-    is packed or concatenated.  Column names / dtypes / dictionaries
-    travel (pickled) only when an edge is first used or a dictionary changes."""
+      * the peer-memory link (csrc/exchange.cu, `native_link`): one meta round, then every rank stores its rows straight
+        into the receivers' mailboxes -- one host round trip per exchange, no library collective;
+      * torch.distributed (gloo on CPU; NCCL when there is no link): an all-gather of the meta rows, then one
+        variable-split all_to_all_single per column.
 
-    def __init__(self, device, mailbox_bytes: int = 6 << 30):
+    Both speak one protocol: every rank posts a meta row (`_Meta`: rows per destination, schema checksums, column widths);
+    column names / dtypes / dictionaries travel (pickled) only when an edge is first used or a dictionary changes
+    (`_agree`); dictionary columns are re-coded onto the union dictionary and validity masks travel as extra uint8
+    columns (`_send_columns`); a receiver gets one table per source rank that sent rows (`_split`)."""
+
+    def __init__(self, device):
         self.device = device
-        self.bytes_sent = 0
+        self.bytes_sent = 0        # payload bytes this rank sent to other ranks, validity masks included
         self.calls = 0
-        self.peer_calls = 0
+        self.peer_calls = 0        # exchanges (and rounds of one) that moved their rows over the link
         self.schemas = {}          # edge key -> [(name, dtype str, dictionary, arrow type, has_valid)]
         self.recv_totals = {}      # edge key -> rows every rank has RECEIVED on that edge so far (known to all ranks from the counts)
-        self.mailbox_bytes = mailbox_bytes
-
-    def _peer_path(self, parts, allmeta, schema, w, me):
-        """Hash-partitioned rows go straight into the receivers' mailboxes (qk_scatter_peer): every rank knows
-        the whole counts matrix, hence where its rows start inside each receiver's columns.  Returns None (all
-        ranks alike) when the payload does not fit the mailbox."""
-        counts = allmeta[:, :w]                                   # counts[s][d]
-        n_recv = [int(counts[:, d].sum()) for d in range(w)]
-        maxrecv = max(n_recv)
-        src = next(r for r in range(w) if int(allmeta[r, w + 2]) > 0)
-        ncols = int(allmeta[src, w + 2])
-        col_w = [int(allmeta[src, w + 3 + i]) & _WIDTH_MASK for i in range(ncols)]
-        if any(int(allmeta[r, w + 3 + i]) & _VALID_FLAG for r in range(w) for i in range(ncols)) \
-                or any(_parse_dt(sc[1])[1] for sc in schema or []):
-            return None                                           # validity masks, vector columns: NCCL path
-        bases, off = [], 0
-        for wd in col_w:
-            bases.append(off)
-            off += (maxrecv * wd + 255) // 256 * 256
-        mb = peer_mailbox(self.device, self.mailbox_bytes)
-        if off > mb.nbytes:
-            return None
-        table, dest, doffs = parts.pending if parts is not None and parts.pending is not None else (None, None, None)
-        mb.barrier()                                              # every rank is done reading the previous contents
-        if table is not None and len(table) > 0:
-            cols_ = []
-            for i in range(ncols):
-                c = table[schema[i][0]]
-                union = schema[i][2]
-                if union is not None and c.dictionary != union:
-                    c = unify_dictionaries([DeviceColumn(torch.zeros(0, dtype=c.data.dtype, device=c.data.device), union, c.arrow_type), c])[1][1]
-                cols_.append(_flat(c.data))
-            row_off = [int(counts[:me, d].sum()) for d in range(w)]
-            ptrs = [[mb.ptrs[d] + bases[i] for i in range(ncols)] for d in range(w)]
-            ops.scatter_peer(cols_, dest, doffs, ptrs, row_off)
-            self.bytes_sent += sum((int(counts[me].sum()) - int(counts[me, me])) * wd for wd in col_w)
-        mb.barrier()                                              # every row addressed to me has landed
-        self.peer_calls += 1
-        if n_recv[me] == 0 or schema is None:
-            return []
-        out = {}
-        for i, (name, dt, union, atype, _) in enumerate(schema):
-            view = _as_rows(mb.buf[bases[i]: bases[i] + n_recv[me] * col_w[i]], dt)
-            out[name] = DeviceColumn(view.clone(), union, atype)   # the mailbox is reused by the next exchange
-        return [DeviceTable(out)]
 
     @staticmethod
     def _schema_of(t: DeviceTable):
         return [(n, _col_dt(c.data), c.dictionary, c.arrow_type, c.valid is not None) for n, c in t.columns.items()]
-
-    # ------------------------------------------------------------------ the peer-memory path (csrc/exchange.cu)
-    W_COUNTS, W_HASH, W_CACHED, W_NCOLS, W_WIDTHS, MAXC = 0, 16, 17, 18, 20, 24
 
     def allgather_words(self, words: list) -> list:
         """[[words of rank 0], [words of rank 1], ...]: a handful of integers from every rank.  On the peer-memory link
@@ -276,13 +323,58 @@ class Exchange:
             return [list(words)]
         link = native_link(self.device)
         if link is not None:
-            m = link.channels[lane_channel()].meta([0] * 16 + [int(x) for x in words])
-            return [[int(x) for x in m[r, 16:16 + len(words)]] for r in range(w)]
+            m = link.channels[lane_channel()].meta([0] * L.MAX_PEERS + [int(x) for x in words])
+            return [[int(x) for x in m[r, L.MAX_PEERS:L.MAX_PEERS + len(words)]] for r in range(w)]
         t = torch.tensor([int(x) for x in words], dtype=torch.int64, device=self.device)
         out = torch.empty(w * len(words), dtype=torch.int64, device=self.device)
         dist.all_gather_into_tensor(out, t)
         return out.cpu().view(w, len(words)).tolist()
 
+    def __call__(self, parts, n_target: int, single_owner: int | None = None, edge_key=None) -> list:
+        """parts: {target_channel: DeviceTable} or edge.Parts.  Target channel c lives on rank c (or on
+        `single_owner` when the consumer has a single channel).  Returns the tables received by this rank,
+        one per source rank that sent rows."""
+        if world_size() == 1:
+            if isinstance(parts, Parts):
+                return parts.tables()
+            return [p for _, p in sorted(parts.items()) if p is not None and len(p) > 0]
+        link = native_link(self.device)
+        if link is not None:
+            return self._native_call(link, parts, single_owner, edge_key)
+        return self._collective_call(parts, single_owner, edge_key)
+
+    # ------------------------------------------------------------------ what both transports do with the meta rows
+    def _count_received(self, edge_key, counts):
+        if edge_key is not None:
+            tot = self.recv_totals.setdefault(edge_key, [0] * counts.shape[1])
+            for d in range(len(tot)):
+                tot[d] += int(counts[:, d].sum())
+
+    def _agree(self, m: _Meta, mine, cached, edge_key, share) -> list | None:
+        """The schema the rows are sent and decoded with (None: this rank neither sends nor receives).  Every rank
+        published a checksum of its table's schema and of the schema it has cached for this edge; the schemas themselves
+        travel -- `share(obj)` returns every rank's object -- only when the checksums disagree (a dictionary grew) or when
+        a rank that will RECEIVE rows has neither a table nor a matching cached schema.  Dictionaries are merged into
+        their sorted union."""
+        hashes = set(h for h in m.hash if h != 0)
+        negotiate = len(hashes) != 1
+        if not negotiate:
+            common = next(iter(hashes))
+            negotiate = any(m.hash[r] == 0 and m.n_recv[r] > 0 and m.cached[r] != common for r in range(len(m.hash)))
+        if negotiate:
+            known = [h for h in share(mine) if h is not None]
+            schema = []
+            for i, (name, dt, _, atype, _) in enumerate(known[0]):
+                dicts = [h[i][2] for h in known if h[i][2] is not None]
+                union = sorted(set().union(*[set(d_) for d_ in dicts])) if dicts else None
+                schema.append((name, dt, union, atype, any(h[i][4] for h in known)))
+        else:
+            schema = mine if mine is not None else (cached if _checksum(cached) == common else None)
+        if edge_key is not None and schema is not None:
+            self.schemas[edge_key] = schema
+        return schema
+
+    # ------------------------------------------------------------------ transport 1: the peer-memory link (csrc/exchange.cu)
     def _share_objects(self, ch, obj):
         """Every rank's `obj` (pickled) to every rank over the link: used only when schemas disagree."""
         w, me = ch.world, ch.rank
@@ -297,349 +389,127 @@ class Exchange:
         out = torch.empty(sum(sizes), dtype=torch.uint8, device=self.device)
         ch.recv([0], [out])
         host = out.cpu().numpy().tobytes()
+        ch.meta([0])        # the objects used this channel's epoch and mailbox: the payload gets a fresh epoch (and the barrier)
         return [pickle.loads(host[off[s_]:off[s_] + sizes[s_]]) for s_ in range(w)]
 
     def _native_call(self, link, parts, single_owner, edge_key) -> list:
-        """One exchange over the link.  Host round trips: ONE (the meta matrix); collectives: none."""
+        """One exchange over the link.  Host round trips: ONE (the meta matrix); collectives: none.  A hash partition's
+        counts go into the meta row from the device (qk_xchg_meta) and its rows are scattered while they are sent."""
         ch = link.channels[lane_channel()]
         w, me = ch.world, ch.rank
-        # ---- what do I send?  mode "scatter": an unmaterialised hash partition (dest / device offsets);
-        #      mode "ranges": a table + one contiguous row range per destination rank
-        table, dest, doffs, lo, hi = None, None, None, [0] * w, [0] * w
-        if isinstance(parts, Parts):
-            if single_owner is None and parts.pending is not None and parts.doffs is not None and parts.doffs.numel() == w + 1:
-                table, dest, doffs = parts.pending
-                if len(table) == 0:
-                    table = dest = doffs = None
-            else:
-                t = parts.table
-                if t is not None and len(t) > 0:
-                    table = t
-                    if single_owner is not None:
-                        hi[single_owner] = len(t)
-                    else:
-                        offs = parts.offsets
-                        for d in range(min(w, len(offs) - 1)):
-                            lo[d], hi[d] = offs[d], offs[d + 1]
-        else:
-            owner = (lambda c_: single_owner) if single_owner is not None else (lambda c_: c_)
-            by_rank = {}
-            for c_, p_ in sorted(parts.items()):
-                if p_ is not None and len(p_) > 0:
-                    by_rank.setdefault(owner(c_), []).append(p_)
-            flat = [p_ for r in sorted(by_rank) for p_ in by_rank[r]]
-            if flat and all(p_ is flat[0] for p_ in flat) and all(len(v) == 1 for v in by_rank.values()):
-                table = flat[0]                                   # broadcast / single owner: the same rows to every destination
-                for r in by_rank:
-                    hi[r] = len(table)
-            elif flat:
-                table = concat_tables(flat)
-                pos = 0
-                for r in sorted(by_rank):
-                    n_r = sum(len(p_) for p_ in by_rank[r])
-                    lo[r], hi[r] = pos, pos + n_r
-                    pos += n_r
+        plan = _SendPlan(parts, single_owner, w)
         self.calls += 1
-        # ---- meta round: counts (from the device in scatter mode), schema checksums, column widths
-        cached = self.schemas.get(edge_key) if edge_key is not None else None
-        mine = self._schema_of(table) if table is not None else None
-        if mine is not None and len(mine) > self.MAXC:
-            raise L.QkError(f"exchange: more than {self.MAXC} columns on one edge")
-        words = [0] * ops.XchgChannel.META
-        for d in range(w):
-            words[d] = hi[d] - lo[d]
-        words[self.W_HASH] = (zlib.crc32(repr(mine).encode()) | 1) if mine is not None else 0
-        words[self.W_CACHED] = (zlib.crc32(repr(cached).encode()) | 1) if cached is not None else 0
-        words[self.W_NCOLS] = len(mine) if mine is not None else 0
-        if mine is not None:
-            for i, (_, dt, _, _, hv) in enumerate(mine):
-                words[self.W_WIDTHS + i] = _row_bytes(dt) | (_VALID_FLAG if hv else 0)
-        m = ch.meta(words, doffs if dest is not None else None)
-        counts = m[:, :w]                                               # counts[s][d]
-        if edge_key is not None:
-            tot = self.recv_totals.setdefault(edge_key, [0] * w)
-            for d in range(w):
-                tot[d] += int(counts[:, d].sum())
-        if dest is not None:
-            offs = [0]
-            for d in range(w):
-                offs.append(offs[-1] + int(counts[me, d]))
-            parts.offsets = offs                                        # my own counts came back with everybody's
-        if int(counts.sum()) == 0:
+        cached = self.schemas.get(edge_key)
+        m = _Meta(ch.meta(_Meta.row(plan.counts, plan.schema, cached, L.MAX_PEERS), plan.doffs), w, L.MAX_PEERS)
+        self._count_received(edge_key, m.counts)
+        if m.total == 0:
             return []
-        # ---- schema agreement (objects travel only when the checksums disagree)
-        hashes = set(int(x) for x in m[:, self.W_HASH] if x != 0)
-        negotiate = len(hashes) != 1
-        if not negotiate:
-            common = next(iter(hashes))
-            for r in range(w):
-                if int(m[r, self.W_HASH]) == 0 and int(counts[:, r].sum()) > 0 and int(m[r, self.W_CACHED]) != common:
-                    negotiate = True
-        if negotiate:
-            known = [h for h in self._share_objects(ch, mine) if h is not None]
-            schema = []
-            for i, (name, dt, _, atype, _) in enumerate(known[0]):
-                dicts = [h[i][2] for h in known]
-                union = sorted(set().union(*[set(d_) for d_ in dicts if d_ is not None])) if any(d_ is not None for d_ in dicts) else None
-                schema.append((name, dt, union, atype, any(h[i][4] for h in known)))
-            ch.meta([0])        # the objects used this channel's epoch and mailbox: the payload gets a fresh epoch (and the barrier)
-        else:
-            schema = mine if mine is not None else (cached if words[self.W_CACHED] == next(iter(hashes)) else None)
-        if edge_key is not None and schema is not None:
-            self.schemas[edge_key] = schema
-        src = next(r for r in range(w) if int(m[r, self.W_NCOLS]) > 0)
-        ncols = int(m[src, self.W_NCOLS])
-        col_w = [int(m[src, self.W_WIDTHS + i]) & _WIDTH_MASK for i in range(ncols)]
-        col_valid = [any(int(m[r, self.W_WIDTHS + i]) & _VALID_FLAG for r in range(w)) for i in range(ncols)]
-        widths = col_w + [1 for v in col_valid if v]                     # validity masks travel as extra uint8 columns
-        n_recv = [int(counts[:, d].sum()) for d in range(w)]
+        schema = self._agree(m, plan.schema, cached, edge_key, lambda obj: self._share_objects(ch, obj))
         bases = []                                                       # bases[d][c]: column c in rank d's mailbox
         for d in range(w):
             row, off = [], 0
-            for wd in widths:
+            for wd in m.widths:
                 row.append(off)
-                off += (n_recv[d] * wd + 255) // 256 * 256
+                off += (m.n_recv[d] * wd + 255) // 256 * 256
             bases.append(row)
             if off > ch.mailbox_bytes:
-                if edge_key is not None:                       # the rounds below count their own rows
-                    tot = self.recv_totals[edge_key]
-                    for d2 in range(w):
-                        tot[d2] -= int(counts[:, d2].sum())
-                return self._native_oversize(link, parts, table, lo, hi, single_owner, edge_key, off, ch.mailbox_bytes)
-        # ---- payload
-        send = []
-        if table is not None:
-            valids = []
-            for i in range(ncols):
-                c = table[schema[i][0]]
-                union = schema[i][2]
-                if union is not None and c.dictionary != union:
-                    c = unify_dictionaries([DeviceColumn(torch.zeros(0, dtype=c.data.dtype, device=c.data.device), union, c.arrow_type), c])[1][1]
-                d_ = _flat(c.data)
-                send.append(d_.view(torch.uint8) if d_.dtype == torch.bool else d_)
-                if col_valid[i]:
-                    valids.append(c.valid if c.valid is not None else torch.ones(len(c), dtype=torch.uint8, device=self.device))
-            send += valids
-        row_off = [int(counts[:me, d].sum()) for d in range(w)]
-        dst_off = [[bases[d][c] + row_off[d] * widths[c] for c in range(len(send))] for d in range(w)]
-        if dest is not None and table is not None:
-            ch.push_scatter(send, dest, doffs, dst_off)
+                self._count_received(edge_key, -m.counts)                # the rounds count their own rows
+                return self._native_oversize(link, plan, edge_key, off, ch.mailbox_bytes)
+        send = _send_columns(plan.table, schema, m.col_valid) if plan.table is not None else []
+        row_off = [int(m.counts[:me, d].sum()) for d in range(w)]
+        dst_off = [[bases[d][c] + row_off[d] * m.widths[c] for c in range(len(send))] for d in range(w)]
+        if plan.dest is not None:
+            ch.push_scatter(send, plan.dest, plan.doffs, dst_off)
         else:
-            ch.push(send, lo, hi, dst_off)
+            ch.push(send, plan.lo, plan.hi, dst_off)
         self.peer_calls += 1
-        self.bytes_sent += (int(counts[me].sum()) - int(counts[me, me])) * sum(widths)
-        if n_recv[me] == 0 or schema is None:
+        self.bytes_sent += m.sent_bytes(me)
+        if m.n_recv[me] == 0 or schema is None:
             ch.recv([], [])
             return []
-        outs = [_empty(n_recv[me], schema[i][1], self.device) for i in range(ncols)]
-        outs += [torch.empty(n_recv[me], dtype=torch.uint8, device=self.device) for v in col_valid if v]
+        outs = _recv_buffers(m.n_recv[me], schema, m.col_valid, self.device)
         ch.recv(bases[me], outs)
-        vmap, k = {}, ncols
-        for i, v in enumerate(col_valid):
-            if v:
-                vmap[i] = outs[k]
-                k += 1
-        tables, r0 = [], 0
-        for s_ in range(w):
-            r1 = r0 + int(counts[s_, me])
-            if r1 > r0:
-                tables.append(DeviceTable({schema[i][0]: DeviceColumn(outs[i][r0:r1], schema[i][2], schema[i][3],
-                                                                      None if i not in vmap else vmap[i][r0:r1])
-                                           for i in range(ncols)}))
-                tables[-1].src_rank = s_         # ordered consumers put the ranks' time ranges back in order with this
-            r0 = r1
-        return tables
+        return _split(outs, schema, m.col_valid, m.counts[:, me])
 
-    def _native_oversize(self, link, parts, table, lo, hi, single_owner, edge_key, need, have) -> list:
+    def _native_oversize(self, link, plan: _SendPlan, edge_key, need, have) -> list:
         """Somebody's share does not fit its mailbox (every rank sees that in the same meta matrix): the rows go in R
         rounds, each a complete exchange of a slice of every sender's rows."""
         R = -(-int(need) // int(have)) * 2
         out = []
-        w = world_size()
-        if isinstance(parts, Parts) and parts.pending is not None and single_owner is None:
+        w = len(plan.lo)
+        if plan.dest is not None:
             # an unmaterialised hash partition: every round is the fused scatter push of a slice of the INPUT rows; the
             # slice's own plan comes from the destinations the full plan already assigned (no local scatter, no copy)
-            t, dest, doffs = parts.pending
-            n = len(t)
-            inner = doffs[1:w].contiguous()
+            n = len(plan.table)
+            inner = plan.doffs[1:w].contiguous()
             for r in range(R):
                 a, b = n * r // R, n * (r + 1) // R
                 if b > a:
-                    which = torch.bucketize(dest[a:b].long(), inner, right=True).to(torch.int32)
+                    which = torch.bucketize(plan.dest[a:b].long(), inner, right=True).to(torch.int32)
                     d_r, o_r = ops.partition_plan(which, w, L.PART_CODE)
-                    sub = Parts(None, None, (t.slice(a, b), d_r, o_r))
+                    sub = Parts(None, None, (plan.table.slice(a, b), d_r, o_r))
                 else:
                     sub = {}
                 out += self._native_call(link, sub, None, edge_key)
             return out
         for r in range(R):
             sub = {}
-            if table is not None:
+            if plan.table is not None:
                 for d in range(w):
-                    n_d = hi[d] - lo[d]
-                    a, b = lo[d] + n_d * r // R, lo[d] + n_d * (r + 1) // R
+                    n_d = plan.hi[d] - plan.lo[d]
+                    a, b = plan.lo[d] + n_d * r // R, plan.lo[d] + n_d * (r + 1) // R
                     if b > a:
-                        sub[d] = table.slice(a, b)
+                        sub[d] = plan.table.slice(a, b)
             out += self._native_call(link, sub, None, edge_key)
         return out
 
-    def __call__(self, parts, n_target: int, single_owner: int | None = None, edge_key=None) -> list:
-        """parts: {target_channel: DeviceTable} or edge.Parts.  Target channel c lives on rank c (or on
-        `single_owner` when the consumer has a single channel).  Returns the tables received by this rank,
-        one per source rank that sent rows."""
-        w = world_size()
-        if w > 1:
-            link = native_link(self.device)
-            if link is not None:
-                return self._native_call(link, parts, single_owner, edge_key)
-        if isinstance(parts, Parts):
-            if w == 1:
-                return parts.tables()
-            peer_flag = 1 if (single_owner is None and parts.pending is not None and len(parts.offsets) == w + 1) else 0
-            table, counts = (parts.pending[0] if peer_flag else parts.table), [0] * w
-            if table is not None and len(table) > 0:
-                if single_owner is not None:
-                    counts[single_owner] = len(table)
-                else:
-                    for ch in range(len(parts.offsets) - 1):
-                        counts[ch] += parts.offsets[ch + 1] - parts.offsets[ch]
-            else:
-                table = None
-        else:
-            if w == 1:
-                return [p for _, p in sorted(parts.items()) if p is not None and len(p) > 0]
-            # nothing to send: this rank can follow whichever path the others take
-            peer_flag = 1 if (single_owner is None and not any(p is not None and len(p) > 0 for p in parts.values())) else 0
-            owner = (lambda ch: single_owner) if single_owner is not None else (lambda ch: ch)
-            by_rank = {}
-            for ch, p in sorted(parts.items()):
-                if p is not None and len(p) > 0:
-                    by_rank.setdefault(owner(ch), []).append(p)
-            counts = [sum(len(p) for p in by_rank.get(r, [])) for r in range(w)]
-            ordered = [p for r in range(w) for p in by_rank.get(r, [])]
-            table = concat_tables(ordered) if ordered else None
-        me = rank()
+    # ------------------------------------------------------------------ transport 2: torch.distributed collectives
+    @staticmethod
+    def _gather_objects(obj):
+        out = [None] * world_size()
+        dist.all_gather_object(out, obj)
+        return out
+
+    def _collective_call(self, parts, single_owner, edge_key) -> list:
+        """One exchange over torch.distributed: an all-gather of the meta rows, then one variable-split all_to_all_single
+        per column, which takes each destination's rows as one contiguous run of the send buffer, in rank order."""
+        w, me = world_size(), rank()
+        plan = _SendPlan(parts, single_owner, w)
         self.calls += 1
-        # Schema agreement without pickling: every rank publishes a checksum of its table's schema (0 = no
-        # table), of the schema it has cached for this edge, and the column widths.  Names / dtypes /
-        # dictionaries are exchanged as objects only when the checksums disagree (a dictionary grew) or when a
-        # rank that will RECEIVE rows has neither a table nor a matching cached schema.  Payload moves as bytes,
-        # so a rank that neither sends nor receives can take part in the collectives knowing only the widths.
-        MAXC = 24
-        cached = self.schemas.get(edge_key) if edge_key is not None else None
-        mine = self._schema_of(table) if table is not None else None
-        h_mine = (zlib.crc32(repr(mine).encode()) | 1) if mine is not None else 0
-        h_cached = (zlib.crc32(repr(cached).encode()) | 1) if cached is not None else 0
-        widths = [0] * MAXC
-        if mine is not None:
-            if len(mine) > MAXC:
-                raise L.QkError(f"exchange: more than {MAXC} columns on one edge")
-            for i, (_, dt, _, _, hv) in enumerate(mine):
-                widths[i] = _row_bytes(dt) | (_VALID_FLAG if hv else 0)
-        meta = torch.tensor(counts + [h_mine, h_cached, len(mine) if mine is not None else 0] + widths + [peer_flag],
-                            dtype=torch.int64, device=self.device)
-        M = w + 3 + MAXC + 1
-        allmeta = torch.empty(w * M, dtype=torch.int64, device=self.device)
-        dist.all_gather_into_tensor(allmeta, meta)
-        allmeta = allmeta.cpu().view(w, M)
-        if int(allmeta[:, :w].sum()) == 0:
+        counts = plan.counts
+        if plan.dest is not None:
+            offs = plan.doffs.cpu().tolist()
+            counts = [offs[d + 1] - offs[d] for d in range(w)]
+        head = max(L.MAX_PEERS, w)
+        cached = self.schemas.get(edge_key)
+        row = torch.tensor(_Meta.row(counts, plan.schema, cached, head), dtype=torch.int64, device=self.device)
+        allm = torch.empty(w * row.numel(), dtype=torch.int64, device=self.device)
+        dist.all_gather_into_tensor(allm, row)
+        m = _Meta(allm.cpu().view(w, -1).numpy(), w, head)
+        self._count_received(edge_key, m.counts)
+        if m.total == 0:
             return []
-        hashes = set(int(x) for x in allmeta[:, w].tolist() if x != 0)
-        negotiate = len(hashes) != 1
-        if not negotiate:
-            common = next(iter(hashes))
-            for r in range(w):
-                if int(allmeta[r, w]) == 0 and int(allmeta[:, r].sum()) > 0 and int(allmeta[r, w + 1]) != common:
-                    negotiate = True
-        if negotiate:
-            headers = [None] * w
-            dist.all_gather_object(headers, mine)
-            known = [h for h in headers if h is not None]
-            schema = []
-            for i, (name, dt, _, atype, has_valid) in enumerate(known[0]):
-                dicts = [h[i][2] for h in known]
-                union = sorted(set().union(*[set(d) for d in dicts if d is not None])) if any(d is not None for d in dicts) else None
-                schema.append((name, dt, union, atype, any(h[i][4] for h in known)))
-        else:
-            schema = mine if mine is not None else (cached if h_cached == next(iter(hashes)) else None)
-        if edge_key is not None and schema is not None:
-            self.schemas[edge_key] = schema
-        if int(allmeta[:, M - 1].sum()) == w and peer_mailbox(self.device, self.mailbox_bytes) is not None:
-            got = self._peer_path(parts if isinstance(parts, Parts) else None, allmeta, schema, w, me)
-            if got is not None:
-                return got
-        if isinstance(parts, Parts) and table is not None and parts.pending is not None:
-            table = parts.table                                   # NCCL path: group the rows locally first
-        src = next(r for r in range(w) if int(allmeta[r, w + 2]) > 0)
-        ncols = int(allmeta[src, w + 2])
-        col_w = [int(allmeta[src, w + 3 + i]) & _WIDTH_MASK for i in range(ncols)]
-        col_valid = [any(int(allmeta[r, w + 3 + i]) & _VALID_FLAG for r in range(w)) for i in range(ncols)]
-        recv_counts = [int(allmeta[s_, me]) for s_ in range(w)]
-        send_counts = [int(c) for c in counts]
-        n_recv, n_send = sum(recv_counts), sum(send_counts)
-        received = []
-        grouped = os.environ.get("QK_EXCHANGE") == "grouped"        # opt-in: ONE grouped send/recv call for all columns
-        pending_ops, sent_keep = [], []
-        for i in range(ncols):
-            send_b = torch.zeros(0, dtype=torch.uint8, device=self.device)
-            valid_b = torch.zeros(0, dtype=torch.uint8, device=self.device)
-            if table is not None:
-                name = schema[i][0]
-                c = table[name]
-                union = schema[i][2]
-                if union is not None and c.dictionary != union:
-                    c = unify_dictionaries([DeviceColumn(torch.zeros(0, dtype=c.data.dtype, device=c.data.device), union, c.arrow_type), c])[1][1]
-                d = _flat(c.data)
-                send_b = d.reshape(-1).view(torch.uint8)
-                if col_valid[i]:
-                    valid_b = c.valid if c.valid is not None else torch.ones(len(c), dtype=torch.uint8, device=self.device)
-            # one variable-split all-to-all per column (grouped ncclSend/ncclRecv inside NCCL), straight out of the
-            # partition kernel's output: rows of one destination are contiguous there
-            wd = col_w[i]
-            recv_b = torch.empty(n_recv * wd, dtype=torch.uint8, device=self.device)
-            valid_r = torch.empty(n_recv, dtype=torch.uint8, device=self.device) if col_valid[i] else None
-            if grouped:
-                # every rank knows the whole counts matrix, so both ends of each transfer agree on which ones are empty
-                for buf_s, buf_r, unit in ((send_b, recv_b, wd),) + (((valid_b, valid_r, 1),) if col_valid[i] else ()):
-                    so = ro = 0
-                    for r in range(w):
-                        ns, nr = send_counts[r] * unit, recv_counts[r] * unit
-                        if r == me:
-                            if ns:
-                                buf_r[ro:ro + nr].copy_(buf_s[so:so + ns])
-                        else:
-                            if ns:
-                                pending_ops.append(dist.P2POp(dist.isend, buf_s[so:so + ns], r))
-                            if nr:
-                                pending_ops.append(dist.P2POp(dist.irecv, buf_r[ro:ro + nr], r))
-                        so, ro = so + ns, ro + nr
-                    sent_keep.append(buf_s)
+        schema = self._agree(m, plan.schema, cached, edge_key, self._gather_objects)
+        nothing = torch.empty(0, dtype=torch.uint8, device=self.device)
+        send = [nothing] * len(m.widths)
+        if plan.table is not None:
+            send = _send_columns(plan.table, schema, m.col_valid)
+            if plan.dest is not None:                            # the hash partition, grouped locally
+                send = ops.scatter(send, plan.dest)
+            elif any(n and lo != sum(counts[:d]) for d, (lo, n) in enumerate(zip(plan.lo, counts))):
+                send = [torch.cat([c[lo:hi] for lo, hi in zip(plan.lo, plan.hi)]) for c in send]     # a broadcast: one copy per rank
             else:
-                dist.all_to_all_single(recv_b, send_b, [c_ * wd for c_ in recv_counts], [c_ * wd for c_ in send_counts])
-                if col_valid[i]:
-                    dist.all_to_all_single(valid_r, valid_b, recv_counts, send_counts)
-            self.bytes_sent += (n_send - send_counts[me]) * wd
-            received.append((recv_b, valid_r))
-        if pending_ops:
-            for req in dist.batch_isend_irecv(pending_ops):
-                req.wait()
-        del sent_keep
+                send = [c[:sum(counts)] for c in send]
+        n_recv = m.n_recv[me]
+        recv = _recv_buffers(n_recv, schema, m.col_valid, self.device) if schema is not None else [nothing] * len(m.widths)
+        recv_counts = [int(x) for x in m.counts[:, me]]
+        for s_b, r_b, wd in zip(send, recv, m.widths):
+            dist.all_to_all_single(r_b.reshape(-1).view(torch.uint8), s_b.reshape(-1).view(torch.uint8),
+                                   [c_ * wd for c_ in recv_counts], [c_ * wd for c_ in counts])
+        self.bytes_sent += m.sent_bytes(me)
         if n_recv == 0 or schema is None:
             return []
-        roff = [0]
-        for c_ in recv_counts:
-            roff.append(roff[-1] + c_)
-        out_cols = {}
-        for (name, dt, union, atype, _), (recv_b, valid_r) in zip(schema, received):
-            out_cols[name] = (_as_rows(recv_b, dt), union, atype, valid_r)
-        tables = []
-        for s_ in range(w):
-            lo, hi = roff[s_], roff[s_ + 1]
-            if hi > lo:
-                tables.append(DeviceTable({n: DeviceColumn(d[lo:hi], u, a, None if v is None else v[lo:hi])
-                                           for n, (d, u, a, v) in out_cols.items()}))
-                tables[-1].src_rank = s_
-        return tables
+        return _split(recv, schema, m.col_valid, recv_counts)
 
 
 # ------------------------------------------------------------------ the graph

@@ -1,10 +1,8 @@
-"""Multi-GPU parity of the peer-memory shuffle (csrc/exchange.cu through runtime.Exchange), launched with
+"""Multi-GPU parity of runtime.Exchange, launched with
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P tests/dist_xchg_check.py
-Every rank draws the SAME global table from a seed, keeps its shard, runs the exchange and checks what it received
-against numpy: rows with key % world == rank, per source rank in source order (the partition is stable), bit-exact.
-Covers: hash-partitioned edges (fused scatter push), broadcast, single owner, ranks with nothing to send, validity
-masks, dictionaries that differ across ranks, payloads larger than the mailbox (rounds), the small all-gather, and
-the exchange driven from two lanes (threads + streams) at once."""
+Runs the checks of tests/xchg_cases.py over the peer-memory shuffle (csrc/exchange.cu), or over NCCL all_to_all_single with
+QK_P2P=0.  On the link it also checks payloads larger than the mailbox (rounds, with QK_MAILBOX_MB set) and the exchange
+driven from two lanes (threads + streams) at once."""
 import os
 import sys
 import threading
@@ -13,7 +11,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.dirname(HERE))
 
-import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -23,107 +20,41 @@ def main():
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     dist.init_process_group("nccl", device_id=dev)
+    import xchg_cases as XC
     from quokka_b200 import runtime as RT
-    from quokka_b200.columns import DeviceColumn, DeviceTable
-    from quokka_b200.edge import apply_partitioner
-    from quokka_b200.target_info import HashPartitioner
     w, me = dist.get_world_size(), dist.get_rank()
     link = RT.native_link(dev)
-    assert link is not None, "peer-memory link unavailable"
+    want_link = os.environ.get("QK_P2P", "1") != "0"
+    assert (link is not None) == want_link, "the peer-memory link must be present exactly when QK_P2P is not 0"
     ex = RT.Exchange(dev)
+    XC.run_all(ex, dev)
 
-    def table_of(cols, lo, hi, dicts=None, valid=None):
-        out = {}
-        for n, v in cols.items():
-            out[n] = DeviceColumn(torch.from_numpy(np.ascontiguousarray(v[lo:hi])).to(dev), (dicts or {}).get(n), None,
-                                  None if valid is None or n not in valid else torch.from_numpy(np.ascontiguousarray(valid[n][lo:hi])).to(dev))
-        return DeviceTable(out)
+    # two lanes at once: different channels, different streams, interleaved in whatever order the threads run (the link
+    # only: library collectives issued from two threads would not come in the same order on every rank)
+    if link is not None:
+        errors = []
 
-    def shard(n, r):
-        return n * r // w, n * (r + 1) // w
-
-    def check_hash(n, seed, empty_ranks=(), tag=""):
-        rng = np.random.default_rng(seed)
-        cols = {"k": rng.integers(0, 1 << 40, n), "a": rng.random(n), "b": rng.integers(-100, 100, n).astype(np.int32),
-                "c": rng.integers(0, 200, n).astype(np.uint8)}
-        lo, hi = shard(n, me)
-        if me in empty_ranks:
-            hi = lo
-        t = table_of(cols, lo, hi)
-        parts = apply_partitioner(HashPartitioner("k"), t, me, w) if hi > lo else {}
-        got = ex(parts, w, edge_key=("hash", tag))
-        exp = []
-        for s in range(w):
-            a, b = shard(n, s)
-            if s in empty_ranks:
-                b = a
-            sel = np.nonzero(cols["k"][a:b] % w == me)[0] + a
-            if len(sel):
-                exp.append(sel)
-        # one table per source rank, or several per source when the payload went in rounds: rows per source, in order
-        srcs = sorted(set(g.src_rank for g in got))
-        assert len(srcs) == len(exp), (tag, me, len(got), len(exp))
-        for s_, sel in zip(srcs, exp):
-            for name, v in cols.items():
-                have = np.concatenate([g[name].data.cpu().numpy() for g in got if g.src_rank == s_])
-                assert np.array_equal(have, v[sel]), (tag, me, name)
-
-    for n, seed in ((0, 1), (1, 2), (5, 3), (2047, 4), (2049, 5), (100_003, 6), (3_000_017, 7)):
-        check_hash(n, seed, tag=f"hash{n}")
-    check_hash(50_000, 8, empty_ranks=(0,), tag="empty0")
-    check_hash(50_000, 9, empty_ranks=tuple(range(1, w)), tag="only0")
-
-    # broadcast and single owner, with a validity mask on one column and per-rank dictionaries
-    rng = np.random.default_rng(20)
-    n = 10_007
-    words = [f"w{i}" for i in range(50)]
-    mydict = [words[(i * 7 + me * 3) % 50] for i in range(50)]                   # a different code assignment on every rank
-    codes = rng.integers(0, 50, n)
-    lo, hi = shard(n, me)
-    cols = {"x": rng.random(n), "s": codes.astype(np.int32)}
-    valid = {"x": (rng.random(n) < 0.7).astype(np.uint8)}
-    t = table_of(cols, lo, hi, {"s": mydict}, valid)
-    got = ex({r: t for r in range(w)}, w, edge_key=("bcast",))
-    assert sorted(set(g.src_rank for g in got)) == list(range(w))
-    for s in range(w):
-        a, b = shard(n, s)
-        mine_ = [g for g in got if g.src_rank == s]
-        assert np.array_equal(np.concatenate([g["x"].data.cpu().numpy() for g in mine_]), cols["x"][a:b])
-        assert np.array_equal(np.concatenate([g["x"].valid.cpu().numpy() for g in mine_]), valid["x"][a:b])
-        sdict = [words[(i * 7 + s * 3) % 50] for i in range(50)]
-        assert [g["s"].dictionary[c] for g in mine_ for c in g["s"].data.cpu().numpy()] == [sdict[c] for c in cols["s"][a:b]], "values survive the re-coding"
-    got = ex({0: t}, 1, single_owner=0, edge_key=("single",))
-    assert (sorted(set(g.src_rank for g in got)) == list(range(w))) if me == 0 else (got == [])
-    if me == 0:
-        assert np.array_equal(np.concatenate([g["x"].data.cpu().numpy() for g in got]), cols["x"])
-
-    # the small all-gather
-    rows = ex.allgather_words([me * 10 + 1, 7])
-    assert rows == [[r * 10 + 1, 7] for r in range(w)]
-
-    # two lanes at once: different channels, different streams, interleaved in whatever order the threads run
-    errors = []
-
-    def lane(li):
-        try:
-            torch.cuda.set_device(dev)
-            RT._lane.index = li
-            with torch.cuda.stream(torch.cuda.Stream(dev)):
-                for rep in range(6):
-                    check_hash(200_003 + li, 100 + 10 * li + rep, tag=f"lane{li}")
-        except BaseException as e:
-            errors.append(e)
-    ts = [threading.Thread(target=lane, args=(li,)) for li in range(min(2, RT.N_LANES))]
-    [t_.start() for t_ in ts]
-    [t_.join() for t_ in ts]
-    if errors:
-        raise errors[0]
+        def lane(li):
+            try:
+                torch.cuda.set_device(dev)
+                RT._lane.index = li
+                with torch.cuda.stream(torch.cuda.Stream(dev)):
+                    for rep in range(6):
+                        XC.check_hash(ex, dev, 200_003 + li, 100 + 10 * li + rep, tag=f"lane{li}")
+            except BaseException as e:
+                errors.append(e)
+        ts = [threading.Thread(target=lane, args=(li,)) for li in range(min(2, RT.N_LANES))]
+        [t_.start() for t_ in ts]
+        [t_.join() for t_ in ts]
+        if errors:
+            raise errors[0]
     torch.cuda.synchronize()
     peer_calls = ex.peer_calls
+    assert link is not None or peer_calls == 0
 
     # payload larger than the mailbox: rounds
     if os.environ.get("QK_MAILBOX_MB"):
-        check_hash(1_500_000, 40, tag="oversize")
+        XC.check_hash(ex, dev, 1_500_000, 40, tag="oversize")
     dist.barrier()
     dist.destroy_process_group()
     if me == 0:

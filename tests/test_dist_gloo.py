@@ -43,10 +43,6 @@ def _worker(rank, world, port, case_names, out_dir):
             qc = QuokkaContext()
             qc.set_config("broadcast_rows", 100)    # shuffle (and Bloom-reduce) every join even at test sizes
             qc.set_config("broadcast_cost_based", False)    # ... unless the case asks for cost-based replication ("cb:")
-            os.environ.pop("QK_EXCHANGE", None)
-            if name.startswith("grp:"):             # one grouped send/recv call per exchange instead of one all-to-all per column
-                os.environ["QK_EXCHANGE"] = "grouped"
-                name = name[4:]
             if name.startswith("hash:"):            # as-of joins the reference's way: both streams hash-shuffled by symbol
                 qc.set_config("asof_time_ranges", False)
                 name = name[5:]
@@ -100,8 +96,8 @@ def _worker(rank, world, port, case_names, out_dir):
 @pytest.mark.parametrize("cases", [["case_q1_sql", "case_q1_dict_api", "case_q3"], ["case_q5", "case_join_kinds"],
                                    ["case_q3", "cb:case_q3", "cbmix:case_q3", "cb:case_q5", "cbmix:case_q10_q18", "cb:case_join_kinds"],
                                    ["case_parquet_q1", "case_parquet_device", "case_csv_q1"],
-                                   ["grp:case_q3", "grp:case_q5", "grp:case_asof", "grp:case_join_kinds", "grp:case_scalar_aggs"],
-                                   ["random_programs:31", "cb:random_programs:32", "grp:random_programs:33", "random_asof:34", "grp:random_asof:35", "bench_legs"],
+                                   ["random_programs:33", "random_asof:35"],
+                                   ["random_programs:31", "cb:random_programs:32", "random_asof:34", "bench_legs"],
                                    ["hash:case_asof", "hash:random_asof:36", "hash:case_asof_reference_result", "asof_rank_shards:41", "hash:asof_rank_shards:42"],
                                    ["case_q9_q11_q13", "case_q15_q16_q20_q22", "case_q2_q21", "case_string_funcs_and_nulls"],
                                    ["case_asof", "case_executor_protocol", "case_misc_ops", "case_scalar_aggs", "case_q6_and_semi_anti", "case_q10_q18", "case_case_like_extract", "case_custom_host_executor", "case_q14_q17_q19", "case_q4_q12",
