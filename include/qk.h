@@ -138,6 +138,8 @@ QK_API int qk_sm_count(void);
  * `payload[sorted(projection)]` (core.py:190-193), in one pass.
  * proj[i]: a single QK_OP_COL node copies the column verbatim in its own dtype (keys stay bit-exact);
  * anything else is evaluated in fp64 and written as QK_F64.
+ * pred and every proj[i]: at most QK_MAX_EXPR_NODES nodes and QK_MAX_STACK stack slots each, 112 nodes together
+ * (QK_ERR_UNSUPPORTED beyond).
  * out[i].data must hold `nrows` elements; *out_rows (device int64) receives the surviving row count.
  * stable != 0 keeps input row order (two passes over the predicate columns, needs
  * qk_scan_workspace_bytes(nrows) bytes of device workspace); stable == 0 compacts in arrival order

@@ -10,6 +10,7 @@ SUM / AVG / MIN / MAX / COUNT(*) with aliases.
 from __future__ import annotations
 
 import datetime as _dt
+import math
 import re
 from dataclasses import dataclass
 from typing import Any
@@ -433,8 +434,31 @@ _ARITH = {"+": L.OP_ADD, "-": L.OP_SUB, "*": L.OP_MUL, "/": L.OP_DIV}
 _INT_DTYPES = (L.QK_U8, L.QK_I32, L.QK_I64)
 
 
-def _is_int_literal(n: Node) -> bool:
-    return n.kind == "date" or (n.kind == "num" and float(n.value).is_integer() and isinstance(n.value, int))
+_I64_MIN, _I64_MAX = -(1 << 63), (1 << 63) - 1
+_ALWAYS, _NEVER = (L.CMP_GE, _I64_MIN), (L.CMP_LT, _I64_MIN)     # x >= INT64_MIN, x < INT64_MIN: true / false for every x
+
+
+def lower_int_cmp(op: str, v) -> tuple:
+    """(compare code, int64 immediate) of `x <op> v` for an integer column x and a numeric literal v (Python int or float),
+    decided exactly, as Python compares an int with an int or a float: a fractional bound becomes the integer bound that
+    selects the same rows (x < 2.5 is x <= 2), a literal outside int64 or a NaN / inf decides every row at once (NaN: every
+    compare false, != true), and the result always fits the node's int64 immediate.  Without this an int64 column would be
+    compared in fp64 (1.7e18 + 1 rounds to 1.7e18) or against a literal that wraps when it is stored."""
+    if isinstance(v, float):
+        if math.isnan(v):
+            return _ALWAYS if op == "!=" else _NEVER
+        if math.isinf(v):
+            v = _I64_MAX + 1 if v > 0 else _I64_MIN - 1      # beyond every x, like any literal outside int64
+        elif not v.is_integer():
+            if op in ("=", "!="):
+                return _ALWAYS if op == "!=" else _NEVER
+            op, v = ("<=", math.floor(v)) if op in ("<", "<=") else (">=", math.ceil(v))
+    v = int(v)
+    if v > _I64_MAX:
+        return _ALWAYS if op in ("<", "<=", "!=") else _NEVER
+    if v < _I64_MIN:
+        return _ALWAYS if op in (">", ">=", "!=") else _NEVER
+    return _CMP[op], v
 
 
 def compile_expr(e: Node, schema: dict) -> list:
@@ -540,10 +564,12 @@ def compile_expr(e: Node, schema: dict) -> list:
             if info.dictionary is not None and all(it.kind == "str" for it in items):
                 emit_set(info, [info.dictionary.index(it.value) for it in items if it.value in info.dictionary])
                 return
-            if info.dtype in _INT_DTYPES and all(_is_int_literal(it) for it in items) \
-                    and all(0 <= int(it.value) < (1 << 16) for it in items):
-                emit_set(info, [int(it.value) for it in items])
-                return
+            if info.dtype in _INT_DTYPES and all(it.kind in ("num", "date") for it in items):
+                # the integers the column can equal: a fractional, NaN, infinite or out-of-int64 literal matches no row
+                vals = [v for c, v in (lower_int_cmp("=", it.value) for it in items) if c == L.CMP_EQ]
+                if vals and all(0 <= v < (1 << 16) for v in vals):
+                    emit_set(info, vals)
+                    return
         for j, it in enumerate(items):
             emit_cmp("=", a, it)
             if j:
@@ -562,8 +588,9 @@ def compile_expr(e: Node, schema: dict) -> list:
                 code = info.dictionary.index(b.value) if b.value in info.dictionary else -1
                 out.append((L.OP_CMP_COL_IMM, info.slot, _CMP[op], 0.0, code))
                 return
-            if info.dtype in _INT_DTYPES and _is_int_literal(b):
-                out.append((L.OP_CMP_COL_IMM, info.slot, _CMP[op], 0.0, int(b.value)))
+            if info.dtype in _INT_DTYPES and b.kind in ("num", "date"):
+                cmp, v = lower_int_cmp(op, b.value)
+                out.append((L.OP_CMP_COL_IMM, info.slot, cmp, 0.0, v))
                 return
             if info.dtype in _INT_DTYPES and b.kind == "col" and ci(b.value).dtype in _INT_DTYPES:
                 out.append((L.OP_CMP_COL_COL, info.slot, _CMP[op] | (ci(b.value).slot << 8), 0.0, 0))
@@ -574,9 +601,6 @@ def compile_expr(e: Node, schema: dict) -> list:
     emit(e)
     check_program(out)
     return out
-
-
-_I64_MIN, _I64_MAX = -(1 << 63), (1 << 63) - 1
 
 
 def _as_range(node):
@@ -615,7 +639,13 @@ def check_program(prog, what: str = "expression") -> None:
     if len(prog) > L.MAX_EXPR_NODES:
         raise ExprError(f"{what} compiles to {len(prog)} nodes; the scan kernels take at most {L.MAX_EXPR_NODES}")
     depth = 0
-    for op, *_ in prog:
+    for op, _a0, _a1, imm, imm_i in prog:
+        # an integer immediate is stored in an int64 field, which would wrap a larger one silently (lower_int_cmp keeps the
+        # compiler's inside it); a range's upper bound travels in the fp64 immediate, exact up to 2^53
+        if op in (L.OP_CMP_COL_IMM, L.OP_RANGE_COL_IMM) and not _I64_MIN <= int(imm_i) <= _I64_MAX:
+            raise ExprError(f"{what}: integer immediate {imm_i} outside int64")
+        if op == L.OP_RANGE_COL_IMM and not -(1 << 53) <= imm <= (1 << 53):
+            raise ExprError(f"{what}: range upper bound {imm} outside +-2^53")
         if op in (L.OP_COL, L.OP_CONST, L.OP_CMP_COL_IMM, L.OP_CMP_COL_COL, L.OP_IN_SET, L.OP_RANGE_COL_IMM):
             depth += 1
         elif op == L.OP_SELECT:
