@@ -256,8 +256,12 @@ QK_API int qk_scatter(const qk_column* cols, int32_t ncols, const int32_t* dest,
  * qk_xchg_recv: waits until every peer's rows of this epoch have landed, then copies column c (out[c].length
  *   rows from byte offset src_byte_off[c] of the own mailbox, 16-byte aligned) into out[c].
  * A row of column c is size(dtype) * max(1, lanes) bytes: qk_xchg_push and qk_xchg_recv move vector columns (lanes > 1);
- * qk_xchg_push_scatter returns QK_ERR_UNSUPPORTED for them.  A link has at most QK_MAX_PEERS ranks. */
+ * qk_xchg_push_scatter returns QK_ERR_UNSUPPORTED for them.  A link has at most QK_MAX_PEERS ranks.
+ * One push / recv takes at most QK_XCHG_MAX_BUFS buffers (24 columns + a validity mask for each, as uint8 buffers), more
+ * than QK_MAX_COLS: every buffer of an edge must go in ONE push, because the push releases the peers' "data landed" flag
+ * after its last store and a receiver may copy out as soon as it sees that flag. */
 #define QK_MAX_PEERS 16
+#define QK_XCHG_MAX_BUFS 48
 #define QK_XCHG_META_WORDS 48
 #define QK_XCHG_CTRL_BYTES 16384
 typedef struct qk_xchg {

@@ -50,7 +50,7 @@ class qk_bloom(C.Structure):
     _fields_ = [("bits", C.c_void_p), ("words_per_part", C.c_int64), ("nparts", C.c_int32), ("key_proj", C.c_int32)]
 
 
-MAX_PEERS, XCHG_META_WORDS, XCHG_CTRL_BYTES = 16, 48, 16384
+MAX_PEERS, XCHG_MAX_BUFS, XCHG_META_WORDS, XCHG_CTRL_BYTES = 16, 48, 48, 16384
 
 
 class qk_xchg(C.Structure):

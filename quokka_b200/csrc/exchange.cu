@@ -107,15 +107,20 @@ __global__ void __launch_bounds__(64) k_xchg_meta(const __grid_constant__ Chan C
 constexpr int X_NT = 256;
 constexpr int X_TILE = 2048;             // rows per tile
 
+constexpr int X_BUFS = QK_XCHG_MAX_BUFS;
+
 struct PushArgs {
-    const void* src[QK_MAX_COLS];
-    unsigned long long dst[QK_MAX_PEERS][QK_MAX_COLS];   // peer-mapped address of the FIRST element this rank writes for (dest, column)
+    const void* src[X_BUFS];
+    unsigned long long dst[QK_MAX_PEERS][X_BUFS];        // peer-mapped address of the FIRST element this rank writes for (dest, column)
     long long send_lo[QK_MAX_PEERS], send_hi[QK_MAX_PEERS];   // contiguous mode: source row range per destination
     long long tile_base[QK_MAX_PEERS + 1];                    // contiguous mode: prefix sums of tiles per destination
-    int8_t width[QK_MAX_COLS];                                // element bytes
-    int32_t lanes[QK_MAX_COLS];                               // elements per row (1: scalar column)
+    int8_t width[X_BUFS];                                     // element bytes
+    int32_t lanes[X_BUFS];                                    // elements per row (1: scalar column)
     int32_t ncols;
 };
+// every buffer of an edge goes in ONE push, so that the data-landed flag is released once, after the last of them: the
+// argument block is ~7 KB of __grid_constant__ parameters (sm_90 with CUDA >= 12.1 takes 32 764 bytes; 4 KB before)
+static_assert(sizeof(Chan) + sizeof(PushArgs) + 3 * sizeof(void*) <= 32764, "push kernel parameters exceed 32 764 bytes");
 
 template <class T>
 __device__ __forceinline__ void copy_rows(const void* src, void* dst, long long first_row, long long r0, long long n, int lanes) {
@@ -255,11 +260,12 @@ __global__ void __launch_bounds__(32) k_xchg_wait_data(const __grid_constant__ C
 }
 
 struct CopyArgs {
-    const void* src[QK_MAX_COLS];
-    void* dst[QK_MAX_COLS];
-    long long bytes[QK_MAX_COLS];
+    const void* src[X_BUFS];
+    void* dst[X_BUFS];
+    long long bytes[X_BUFS];
     int32_t ncols;
 };
+static_assert(sizeof(CopyArgs) <= 4096, "copy-out kernel parameters");
 // mailbox columns -> caller's columns (both 16-byte aligned: mailbox column bases are 256-byte aligned)
 __global__ void __launch_bounds__(256) k_xchg_copy_out(const __grid_constant__ CopyArgs A) {
     for (int c = 0; c < A.ncols; ++c) {
@@ -308,7 +314,7 @@ extern "C" int qk_xchg_meta(const qk_xchg* x, uint64_t epoch, const int64_t* par
 
 static int fill_push(PushArgs& A, const qk_xchg* x, const qk_column* cols, int32_t ncols, const int64_t* dst_byte_off,
                      int64_t* nrows_out, bool vectors_ok, const char* who) {
-    if (ncols < 0 || ncols > QK_MAX_COLS) QK_FAIL(QK_ERR_INVALID, "%s: ncols out of range", who);
+    if (ncols < 0 || ncols > QK_XCHG_MAX_BUFS) QK_FAIL(QK_ERR_INVALID, "%s: ncols out of range (%d buffers, at most %d)", who, ncols, QK_XCHG_MAX_BUFS);
     if (ncols > 0 && (!cols || !dst_byte_off)) QK_FAIL(QK_ERR_INVALID, "%s: null columns / offsets", who);
     int64_t n = ncols > 0 ? cols[0].length : 0;
     for (int c = 0; c < ncols; ++c) {
@@ -386,11 +392,9 @@ extern "C" int qk_xchg_recv(const qk_xchg* x, uint64_t epoch, const int64_t* src
     const char* who = "qk_xchg_recv";
     Chan C;
     if (int rc = fill_chan(C, x, epoch, who)) return rc;
-    if (ncols < 0 || ncols > QK_MAX_COLS) QK_FAIL(QK_ERR_INVALID, "%s: ncols out of range", who);
-    k_xchg_wait_data<<<1, 32, 0, (cudaStream_t)stream>>>(C);
-    QK_LAUNCH_CHECK("k_xchg_wait_data");
-    if (ncols == 0) return QK_OK;
-    if (!src_byte_off || !out) QK_FAIL(QK_ERR_INVALID, "%s: null arguments", who);
+    if (ncols < 0 || ncols > QK_XCHG_MAX_BUFS) QK_FAIL(QK_ERR_INVALID, "%s: ncols out of range (%d buffers, at most %d)", who, ncols, QK_XCHG_MAX_BUFS);
+    if (ncols > 0 && (!src_byte_off || !out)) QK_FAIL(QK_ERR_INVALID, "%s: null arguments", who);
+    // every argument is checked before the wait is launched: a rejected call leaves nothing on the stream
     CopyArgs A;
     long long total = 0;
     for (int c = 0; c < ncols; ++c) {
@@ -404,6 +408,8 @@ extern "C" int qk_xchg_recv(const qk_xchg* x, uint64_t epoch, const int64_t* src
         total += bytes;
     }
     A.ncols = ncols;
+    k_xchg_wait_data<<<1, 32, 0, (cudaStream_t)stream>>>(C);
+    QK_LAUNCH_CHECK("k_xchg_wait_data");
     if (total == 0) return QK_OK;
     long long nb = (total / 16 + 255) / 256 / 4 + 1;
     const long long cap = (long long)sm_count() * 8;

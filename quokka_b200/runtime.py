@@ -215,7 +215,8 @@ class _Meta:
     link `head` is 16 (qk_xchg_meta may overwrite words [0, w) with the device counts, and the link takes at most
     QK_MAX_PEERS = 16 ranks); the collective path puts the header after max(16, w) counts."""
 
-    HASH, CACHED, NCOLS, WIDTHS, MAXC = 0, 1, 2, 4, 24
+    HASH, CACHED, NCOLS, WIDTHS = 0, 1, 2, 4
+    MAXC = L.XCHG_MAX_BUFS // 2      # columns of an edge: with a validity mask each, one push of QK_XCHG_MAX_BUFS buffers
 
     @classmethod
     def row(cls, counts: list, mine, cached, head: int) -> list:
@@ -415,6 +416,9 @@ class Exchange:
             if off > ch.mailbox_bytes:
                 self._count_received(edge_key, -m.counts)                # the rounds count their own rows
                 return self._native_oversize(link, plan, edge_key, off, ch.mailbox_bytes)
+        if len(m.widths) > L.XCHG_MAX_BUFS:
+            raise L.QkError(f"exchange: {len(m.widths)} buffers on one edge (columns + validity masks); the link moves at most "
+                            f"{L.XCHG_MAX_BUFS} in one push")
         send = _send_columns(plan.table, schema, m.col_valid) if plan.table is not None else []
         row_off = [int(m.counts[:me, d].sum()) for d in range(w)]
         dst_off = [[bases[d][c] + row_off[d] * m.widths[c] for c in range(len(send))] for d in range(w)]
