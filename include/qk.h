@@ -184,12 +184,13 @@ QK_API int qk_scan_filter_agg_dense(const qk_column* cols, int32_t ncols, int64_
                              const qk_expr* agg_expr, const int32_t* agg_op, int32_t nagg,
                              double* acc, int64_t* cnt, void* workspace, size_t ws_bytes,
                              int32_t variant, void* stream);
-/* variant: 0 = auto, 1 = generic interpreter, 2 = fused template (vector LDG), 3 = fused template
- * with cp.async.bulk (TMA engine) staging of column tiles into shared memory. Returns
- * QK_ERR_UNSUPPORTED if a forced fused variant has no instantiation for the plan. */
+/* variant: 0 = auto (3, else the interpreter), 1 = generic interpreter, 3 = a typed fused plan with
+ * cp.async.bulk (TMA engine) staging of column tiles into shared memory, else the runtime-described
+ * fused plan over the same tile ring, 7 = the runtime-described plan only.  Any other value is
+ * QK_ERR_INVALID.  Returns QK_ERR_UNSUPPORTED if a forced fused variant has no plan for the request. */
 /* name of the kernel variant the last qk_scan_filter_agg_dense call on this thread dispatched to */
 QK_API const char* qk_last_variant(void);
-/* launch shape of that kernel, e.g. "nt512v2s2" = 512 threads, 2 rows/thread/tile, 2 TMA stages */
+/* launch shape of that kernel, e.g. "nt256v2s3" = 256 threads, 2 rows/thread/tile, 3 TMA stages */
 QK_API const char* qk_last_variant_config(void);
 
 /* ---- K2 (high cardinality): hash aggregate -------------------------------------------------

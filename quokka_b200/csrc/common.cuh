@@ -68,6 +68,35 @@ static inline int check_col(const qk_column* c, const char* what) {
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// An integer-range predicate node (QK_OP_CMP_COL_IMM or QK_OP_RANGE_COL_IMM) as the branch-free test
+// ((lo <= x) & (x <= hi)) != neg, its bounds clamped to 32 bits when the column is QK_I32 (a kernel that compares in
+// 32 bits must not truncate a bound beyond int32) and to 64 bits otherwise.  An empty range is lo = 1, hi = 0.
+struct IntRange { int64_t lo, hi; bool neg; };
+static inline IntRange int_range(const qk_expr_node& nd, int dtype) {
+    const int64_t tmin = dtype == QK_I32 ? INT32_MIN : INT64_MIN, tmax = dtype == QK_I32 ? INT32_MAX : INT64_MAX;
+    IntRange r{tmin, tmax, false};
+    bool empty = false;
+    if (nd.op == QK_OP_RANGE_COL_IMM) {
+        r.neg = nd.a1 != 0;
+        const int64_t lo = nd.imm_i, hi = (int64_t)nd.imm;
+        empty = lo > tmax || hi < tmin || lo > hi;
+        if (lo > tmin) r.lo = lo;
+        if (hi < tmax) r.hi = hi;
+    } else {
+        const int64_t imm = nd.imm_i;
+        switch (nd.a1) {
+            case QK_CMP_LT: if (imm <= tmin) empty = true; else r.hi = imm > tmax ? tmax : imm - 1; break;
+            case QK_CMP_LE: if (imm < tmin) empty = true; else r.hi = imm > tmax ? tmax : imm; break;
+            case QK_CMP_GT: if (imm >= tmax) empty = true; else r.lo = imm < tmin ? tmin : imm + 1; break;
+            case QK_CMP_GE: if (imm > tmax) empty = true; else r.lo = imm < tmin ? tmin : imm; break;
+            case QK_CMP_EQ: if (imm < tmin || imm > tmax) empty = true; else r.lo = r.hi = imm; break;
+            default: r.neg = true; if (imm < tmin || imm > tmax) empty = true; else r.lo = r.hi = imm; break;   // !=
+        }
+    }
+    if (empty) { r.lo = 1; r.hi = 0; }
+    return r;
+}
+
 // ---------------------------------------------------------------- device side
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
     x ^= x >> 30; x *= 0xBF58476D1CE4E5B9ULL;

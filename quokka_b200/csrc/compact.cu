@@ -429,21 +429,8 @@ int try_filter_compact_tma(const qk_column* cols, int ncols, int64_t nrows, cons
         const qk_column& c = cols[nd.a0];
         if (!al16(c.data)) return 1;
         A.pred_col = (const unsigned char*)c.data; A.pred_width = dtype_size(c.dtype);
-        const long long imm = nd.imm_i;
-        long long lo = INT64_MIN, hi = INT64_MAX;
-        bool empty = false;
-        A.pred_neg = 0;
-        if (nd.op == QK_OP_RANGE_COL_IMM) { lo = nd.imm_i; hi = (long long)nd.imm; A.pred_neg = nd.a1 != 0; empty = lo > hi; }
-        else switch (nd.a1) {
-            case QK_CMP_LT: if (imm == INT64_MIN) empty = true; else hi = imm - 1; break;
-            case QK_CMP_LE: hi = imm; break;
-            case QK_CMP_GT: if (imm == INT64_MAX) empty = true; else lo = imm + 1; break;
-            case QK_CMP_GE: lo = imm; break;
-            case QK_CMP_EQ: lo = hi = imm; break;
-            default: lo = hi = imm; A.pred_neg = 1; break;
-        }
-        if (empty) { lo = 1; hi = 0; }
-        A.pred_lo = lo; A.pred_hi = hi;
+        const IntRange r = int_range(nd, QK_I64);          // the kernel compares in 64 bits whatever the column width
+        A.pred_lo = r.lo; A.pred_hi = r.hi; A.pred_neg = r.neg;
     }
     // tile size: 3 CTAs per SM (so one CTA's output-reservation atomic overlaps the others' work), each with a
     // 3-stage ring inside ~72 KB; QK_COMPACT_CTAS overrides the CTAs-per-SM target for experiments

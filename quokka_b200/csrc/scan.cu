@@ -3,11 +3,12 @@
 // Three code paths, all HBM-bound by design (no tensor cores: there is no dense contraction):
 //   variant 1  generic: a postfix interpreter per row (any predicate / expression the host compiler
 //              emits); stack in local memory, columns read straight from global memory.
-//   variant 2  fused template: the plan shape (typed column slots, affine-product aggregates) is a
-//              C++ type, so every operand lives in a statically named register; 4 rows per thread,
-//              128-bit global loads (32-bit for the 1-byte code columns).
-//   variant 3  the same fused plan with the column tiles staged into shared memory by the TMA engine
-//              (cp.async.bulk + mbarrier complete_tx), 3-stage ring, one elected producer thread.
+//   variant 3  typed plan: the plan shape (typed column slots, affine-product aggregates) is a C++ type,
+//              so every operand lives in a statically named register; the column tiles are staged into
+//              shared memory by the TMA engine (cp.async.bulk + mbarrier complete_tx), 3-stage ring, one
+//              elected producer thread.  A request no typed plan matches takes variant 7.
+//   variant 7  runtime-described plan: any aggregate of a small grammar over the same TMA tile ring.
+// Variant 0 (auto) tries 3, then 7, then 1.
 // The dense aggregate keeps LANE-PRIVATE partial states in shared memory (acc[slot][thread]), so the
 // inner loop has no atomics and no bank conflicts; each CTA then reduces its copies with warp shuffles
 // and writes one partial per slot; a last tiny kernel folds the per-CTA partials in a FIXED order, which
@@ -403,7 +404,7 @@ __global__ void k_dense_finalize_cnt(const long long* part_cnt, int nblocks, int
     }
 }
 
-// ---------------------------------------------------------------- fused template plans (variants 2, 3)
+// ---------------------------------------------------------------- typed fused plan (variant 3)
 // Operand kinds of an aggregate argument written as a product of affine factors of fp64 columns:
 //   Col<S>        v[S]
 //   KMinus<S,P>   par[P] - v[S]          (e.g. 1 - l_discount)
@@ -446,169 +447,54 @@ template <class... As> struct AggList {
     }
 };
 
-// A dense plan: optional predicate `icol <cmp> imm` on one integer column (dtype PRED_DT, 0 = none),
-// NG group code columns (u8), NF fp64 measure columns, SUM aggregates from AggList.
-template <int PRED_DT_, int NG_, int NF_, class Aggs_, int NPAR_>
+// A dense plan: predicate `icol <cmp> imm` on one int32 column, NG group code columns (u8), NF fp64 measure columns,
+// SUM aggregates from AggList.
+template <int NG_, int NF_, class Aggs_, int NPAR_>
 struct DensePlan {
-    static constexpr int PRED_DT = PRED_DT_, NG = NG_, NF = NF_, NAGG = Aggs_::N;
+    static constexpr int NG = NG_, NF = NF_, NAGG = Aggs_::N;
     static_assert(NPAR_ >= 0 && NPAR_ <= 8, "at most 8 constants");
     using Aggs = Aggs_;
 };
 
 struct FusedArgs {
-    const void* pred_col;
+    const int32_t* pred_col;
     const uint8_t* gcol[2];
     const double* fcol[8];
     int32_t gstride[2];
     int32_t pred_neg;              // predicate = ((lo <= x) & (x <= hi)) != neg   (branch-free form of col <cmp> imm)
-    int64_t pred_lo, pred_hi;
+    int64_t pred_lo, pred_hi;      // clamped to int32 (int_range)
     double par[8];
 };
 
-// col <cmp> imm  ->  closed range [lo, hi] (+ negation for !=), clamped to the column's integer width
-void range_of(int cmp, int64_t imm, int dt, FusedArgs& F) {
-    const int64_t tmin = dt == QK_I32 ? INT32_MIN : INT64_MIN, tmax = dt == QK_I32 ? INT32_MAX : INT64_MAX;
-    int64_t lo = tmin, hi = tmax;
-    bool empty = false;
-    F.pred_neg = 0;
-    switch (cmp) {
-        case QK_CMP_LT: if (imm <= tmin) empty = true; else hi = imm > tmax ? tmax : imm - 1; break;
-        case QK_CMP_LE: if (imm < tmin) empty = true; else hi = imm > tmax ? tmax : imm; break;
-        case QK_CMP_GT: if (imm >= tmax) empty = true; else lo = imm < tmin ? tmin : imm + 1; break;
-        case QK_CMP_GE: if (imm > tmax) empty = true; else lo = imm < tmin ? tmin : imm; break;
-        case QK_CMP_EQ: if (imm < tmin || imm > tmax) empty = true; else lo = hi = imm; break;
-        default: F.pred_neg = 1; if (imm < tmin || imm > tmax) empty = true; else lo = hi = imm; break;   // !=
-    }
-    if (empty) { lo = 1; hi = 0; }
-    F.pred_lo = lo; F.pred_hi = hi;
-}
-
-// closed range [lo, hi] (+ negation), clamped to the column's integer width
-void range_closed(int64_t lo, int64_t hi, bool neg, int dt, FusedArgs& F) {
-    const int64_t tmin = dt == QK_I32 ? INT32_MIN : INT64_MIN, tmax = dt == QK_I32 ? INT32_MAX : INT64_MAX;
-    if (lo > tmax || hi < tmin || lo > hi) { lo = 1; hi = 0; }
-    else { if (lo < tmin) lo = tmin; if (hi > tmax) hi = tmax; }
-    F.pred_lo = lo; F.pred_hi = hi; F.pred_neg = neg ? 1 : 0;
-}
-
 template <int NF> struct RowVals { double f[NF]; };
 
-constexpr int F_NT = 256;      // threads per CTA
-constexpr int F_V = 4;         // rows per thread per tile
-constexpr int F_TILE = F_NT * F_V;
+constexpr int F_NT = 256;          // threads per CTA
+constexpr int F_STAGES = 3;        // tiles in flight per CTA
 
-__device__ __forceinline__ int4 ldg_nc_v4(const void* p) {
-    int4 r;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-    return r;
-}
-__device__ __forceinline__ unsigned ldg_nc_u32(const void* p) {
-    unsigned r;
-    asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(r) : "l"(p));
-    return r;
-}
-
-template <class Plan>
 __device__ __forceinline__ bool pred_i32(int x, const FusedArgs& F) {
     return ((x >= (int)F.pred_lo) & (x <= (int)F.pred_hi)) != (F.pred_neg != 0);
-}
-template <class Plan>
-__device__ __forceinline__ bool pred_i64(long long x, const FusedArgs& F) {
-    return ((x >= F.pred_lo) & (x <= F.pred_hi)) != (F.pred_neg != 0);
 }
 
 // Branch-free: a row that fails the predicate adds 0.0 / 0 to its group, so the rows of a tile form one
 // basic block and their loads are issued together.
-template <class Plan, int NT>
+template <class Plan>
 __device__ __forceinline__ void accumulate_row(bool pass, int g, const RowVals<Plan::NF>& v, const FusedArgs& F,
                                                double* acc, unsigned* cnt) {
     Plan::Aggs::for_each(v, F.par, [&](int j, double x) {
-        double* a = &acc[(g * Plan::NAGG + j) * NT + threadIdx.x];
+        double* a = &acc[(g * Plan::NAGG + j) * F_NT + threadIdx.x];
         *a += pass ? x : 0.0;
     });
-    cnt[g * NT + threadIdx.x] += pass ? 1u : 0u;
+    cnt[g * F_NT + threadIdx.x] += pass ? 1u : 0u;
 }
 
-// variant 2: direct vector loads, 4 consecutive rows per thread
-template <class Plan>
-__global__ void __launch_bounds__(F_NT, 3) k_dense_agg_fused_ldg(const __grid_constant__ FusedArgs F, const __grid_constant__ DenseArgs A,
-                                                                  int64_t nrows, double* part_acc, long long* part_cnt) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    double* acc = (double*)smem_raw;
-    unsigned* cnt = (unsigned*)(acc + (size_t)A.n_groups * Plan::NAGG * F_NT);
-    cta_init<F_NT>(acc, cnt, A);
-    const int64_t ntiles = (nrows + F_TILE - 1) / F_TILE;
-    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const int64_t base = tile * F_TILE + (int64_t)threadIdx.x * F_V;
-        if (base + F_V <= nrows) {
-            // ---- full vector path: issue every load before the first use
-            int4 pv = make_int4(0, 0, 0, 0);
-            int4 pw[2];
-            if constexpr (Plan::PRED_DT == QK_I32) pv = ldg_nc_v4((const int32_t*)F.pred_col + base);
-            if constexpr (Plan::PRED_DT == QK_I64) {
-                pw[0] = ldg_nc_v4((const int64_t*)F.pred_col + base);
-                pw[1] = ldg_nc_v4((const int64_t*)F.pred_col + base + 2);
-            }
-            unsigned gv[Plan::NG > 0 ? Plan::NG : 1];
-#pragma unroll
-            for (int k = 0; k < Plan::NG; ++k) gv[k] = ldg_nc_u32(F.gcol[k] + base);
-            int4 fv[Plan::NF][2];
-#pragma unroll
-            for (int s = 0; s < Plan::NF; ++s) {
-                fv[s][0] = ldg_nc_v4(F.fcol[s] + base);
-                fv[s][1] = ldg_nc_v4(F.fcol[s] + base + 2);
-            }
-#pragma unroll
-            for (int r = 0; r < F_V; ++r) {
-                bool pass = true;
-                if constexpr (Plan::PRED_DT == QK_I32) pass = pred_i32<Plan>(r == 0 ? pv.x : r == 1 ? pv.y : r == 2 ? pv.z : pv.w, F);
-                if constexpr (Plan::PRED_DT == QK_I64) {
-                    const int4 q = pw[r >> 1];
-                    const long long x = (r & 1) ? (((long long)(unsigned)q.w << 32) | (unsigned)q.z) : (((long long)(unsigned)q.y << 32) | (unsigned)q.x);
-                    pass = pred_i64<Plan>(x, F);
-                }
-                int g = 0;
-#pragma unroll
-                for (int k = 0; k < Plan::NG; ++k) g += (int)((gv[k] >> (8 * r)) & 0xffu) * F.gstride[k];
-                g = min(g, A.n_groups - 1);
-                RowVals<Plan::NF> v;
-#pragma unroll
-                for (int s = 0; s < Plan::NF; ++s) {
-                    const int4 q = fv[s][r >> 1];
-                    v.f[s] = (r & 1) ? __hiloint2double(q.w, q.z) : __hiloint2double(q.y, q.x);
-                }
-                accumulate_row<Plan, F_NT>(pass, g, v, F, acc, cnt);
-            }
-        } else {
-            for (int r = 0; r < F_V; ++r) {
-                const int64_t row = base + r;
-                if (row >= nrows) break;
-                bool pass = true;
-                if constexpr (Plan::PRED_DT == QK_I32) pass = pred_i32<Plan>(((const int32_t*)F.pred_col)[row], F);
-                if constexpr (Plan::PRED_DT == QK_I64) pass = pred_i64<Plan>(((const int64_t*)F.pred_col)[row], F);
-                int g = 0;
-#pragma unroll
-                for (int k = 0; k < Plan::NG; ++k) g += (int)F.gcol[k][row] * F.gstride[k];
-                g = min(g, A.n_groups - 1);
-                RowVals<Plan::NF> v;
-#pragma unroll
-                for (int s = 0; s < Plan::NF; ++s) v.f[s] = F.fcol[s][row];
-                accumulate_row<Plan, F_NT>(pass, g, v, F, acc, cnt);
-            }
-        }
-    }
-    cta_flush<F_NT>(acc, cnt, A, part_acc, part_cnt);
-}
-
-// variant 3+: TMA-engine (cp.async.bulk) staging of column tiles into shared memory.
-// Shared-memory tile of TILE rows: fp64 columns first (8-byte aligned), then the predicate column, then
+// TMA-engine (cp.async.bulk) staging of column tiles into shared memory.
+// Shared-memory tile of TILE rows: fp64 columns first (8-byte aligned), then the int32 predicate column, then
 // the 1-byte group-code columns.  Every sub-array starts on a 16-byte boundary (TILE is a multiple of 16).
 template <class Plan, int TILE> struct TileLayout {
-    static constexpr int pred_bytes = Plan::PRED_DT == QK_I32 ? 4 : Plan::PRED_DT == QK_I64 ? 8 : 0;
-    static constexpr int row_bytes = pred_bytes + Plan::NG + 8 * Plan::NF;
+    static constexpr int row_bytes = 4 + Plan::NG + 8 * Plan::NF;
     static constexpr int off_f = 0;
     static constexpr int off_pred = 8 * Plan::NF * TILE;
-    static constexpr int off_g = off_pred + pred_bytes * TILE;
+    static constexpr int off_g = off_pred + 4 * TILE;
     static constexpr int stage_bytes = row_bytes * TILE;
     static_assert(TILE % 16 == 0, "bulk copies need 16-byte multiples");
 };
@@ -620,16 +506,15 @@ __device__ __forceinline__ void tma_issue_tile(const FusedArgs& F, int64_t tile,
     mbar_expect_tx(bar, (unsigned)L::stage_bytes);
 #pragma unroll
     for (int s = 0; s < Plan::NF; ++s) bulk_g2s(smem_u32(stage + L::off_f + s * 8 * TILE), F.fcol[s] + base, 8 * TILE, bar);
-    if constexpr (L::pred_bytes > 0)
-        bulk_g2s(smem_u32(stage + L::off_pred), (const unsigned char*)F.pred_col + base * L::pred_bytes, L::pred_bytes * TILE, bar);
+    bulk_g2s(smem_u32(stage + L::off_pred), F.pred_col + base, 4 * TILE, bar);
 #pragma unroll
     for (int k = 0; k < Plan::NG; ++k) bulk_g2s(smem_u32(stage + L::off_g + k * TILE), F.gcol[k] + base, TILE, bar);
 }
 
-template <class Plan, int NT, int V, int STAGES>
-__global__ void __launch_bounds__(NT, 1) k_dense_agg_fused_tma(const __grid_constant__ FusedArgs F, const __grid_constant__ DenseArgs A,
-                                                               int64_t nrows, double* part_acc, long long* part_cnt) {
-    constexpr int TILE = NT * V;
+template <class Plan, int V>
+__global__ void __launch_bounds__(F_NT, 1) k_dense_agg_fused_tma(const __grid_constant__ FusedArgs F, const __grid_constant__ DenseArgs A,
+                                                                 int64_t nrows, double* part_acc, long long* part_cnt) {
+    constexpr int NT = F_NT, STAGES = F_STAGES, TILE = NT * V;
     using L = TileLayout<Plan, TILE>;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) unsigned long long bars[STAGES];
@@ -661,9 +546,7 @@ __global__ void __launch_bounds__(NT, 1) k_dense_agg_fused_tma(const __grid_cons
 #pragma unroll
         for (int r = 0; r < V; ++r) {
             const int t = r * NT + threadIdx.x;
-            pass[r] = true;
-            if constexpr (Plan::PRED_DT == QK_I32) pass[r] = pred_i32<Plan>(((const int32_t*)(st + L::off_pred))[t], F);
-            if constexpr (Plan::PRED_DT == QK_I64) pass[r] = pred_i64<Plan>(((const int64_t*)(st + L::off_pred))[t], F);
+            pass[r] = pred_i32(((const int32_t*)(st + L::off_pred))[t], F);
             int gg = 0;
 #pragma unroll
             for (int k = 0; k < Plan::NG; ++k) gg += (int)st[L::off_g + k * TILE + t] * F.gstride[k];
@@ -672,7 +555,7 @@ __global__ void __launch_bounds__(NT, 1) k_dense_agg_fused_tma(const __grid_cons
             for (int q = 0; q < Plan::NF; ++q) v[r].f[q] = ((const double*)(st + L::off_f + q * 8 * TILE))[t];
         }
 #pragma unroll
-        for (int r = 0; r < V; ++r) accumulate_row<Plan, NT>(pass[r], g[r], v[r], F, acc, cnt);
+        for (int r = 0; r < V; ++r) accumulate_row<Plan>(pass[r], g[r], v[r], F, acc, cnt);
         __syncthreads();                                   // every thread is done with stage s
         if (threadIdx.x == 0 && it + STAGES < my_n)
             tma_issue_tile<Plan, TILE>(F, blockIdx.x + (it + STAGES) * gridDim.x, stages + (size_t)s * L::stage_bytes, smem_u32(&bars[s]));
@@ -681,9 +564,7 @@ __global__ void __launch_bounds__(NT, 1) k_dense_agg_fused_tma(const __grid_cons
     // ragged tail (< TILE rows): plain loads, handled by CTA 0
     if (blockIdx.x == 0) {
         for (int64_t row = nfull * TILE + threadIdx.x; row < nrows; row += NT) {
-            bool pass = true;
-            if constexpr (Plan::PRED_DT == QK_I32) pass = pred_i32<Plan>(((const int32_t*)F.pred_col)[row], F);
-            if constexpr (Plan::PRED_DT == QK_I64) pass = pred_i64<Plan>(((const int64_t*)F.pred_col)[row], F);
+            const bool pass = pred_i32(F.pred_col[row], F);
             int g = 0;
 #pragma unroll
             for (int k = 0; k < Plan::NG; ++k) g += (int)F.gcol[k][row] * F.gstride[k];
@@ -691,7 +572,7 @@ __global__ void __launch_bounds__(NT, 1) k_dense_agg_fused_tma(const __grid_cons
             RowVals<Plan::NF> v;
 #pragma unroll
             for (int q = 0; q < Plan::NF; ++q) v.f[q] = F.fcol[q][row];
-            accumulate_row<Plan, NT>(pass, g, v, F, acc, cnt);
+            accumulate_row<Plan>(pass, g, v, F, acc, cnt);
         }
     }
     cta_flush<NT>(acc, cnt, A, part_acc, part_cnt);
@@ -709,17 +590,13 @@ template <class Plan>
 bool match_plan(const Request& R, FusedArgs& F) {
     if (R.nagg != Plan::NAGG || R.ngroup_cols != Plan::NG) return false;
     for (int j = 0; j < R.nagg; ++j) if (R.agg_op[j] != QK_AGG_SUM) return false;
-    // predicate: none, or exactly one CMP_COL_IMM on a column of the plan's predicate dtype
-    const int npred = R.pred ? R.pred->n_nodes : 0;
-    if (Plan::PRED_DT == 0) { if (npred != 0) return false; }
-    else {
-        if (npred != 1 || (R.pred->nodes[0].op != QK_OP_CMP_COL_IMM && R.pred->nodes[0].op != QK_OP_RANGE_COL_IMM)) return false;
-        const qk_expr_node& nd = R.pred->nodes[0];
-        if (R.cols[nd.a0].dtype != Plan::PRED_DT) return false;
-        F.pred_col = R.cols[nd.a0].data;
-        if (nd.op == QK_OP_CMP_COL_IMM) range_of(nd.a1, nd.imm_i, Plan::PRED_DT, F);
-        else range_closed(nd.imm_i, (int64_t)nd.imm, nd.a1 != 0, Plan::PRED_DT, F);
-    }
+    // predicate: exactly one integer-range test on an int32 column
+    if (!R.pred || R.pred->n_nodes != 1 || (R.pred->nodes[0].op != QK_OP_CMP_COL_IMM && R.pred->nodes[0].op != QK_OP_RANGE_COL_IMM)) return false;
+    const qk_expr_node& nd = R.pred->nodes[0];
+    if (R.cols[nd.a0].dtype != QK_I32) return false;
+    F.pred_col = (const int32_t*)R.cols[nd.a0].data;
+    const IntRange r = int_range(nd, QK_I32);
+    F.pred_lo = r.lo; F.pred_hi = r.hi; F.pred_neg = r.neg;
     int stride = 1;
     for (int k = Plan::NG - 1; k >= 0; --k) {      // row-major group id: first key most significant
         const qk_column& c = R.cols[R.group_cols[k]];
@@ -745,9 +622,9 @@ bool match_plan(const Request& R, FusedArgs& F) {
         }
     }
     for (int s = 0; s < Plan::NF; ++s) { if (slot_col[s] < 0) return false; F.fcol[s] = (const double*)R.cols[slot_col[s]].data; }
-    // vector loads need 16-byte aligned column bases
+    // bulk copies need 16-byte aligned column bases
     auto al = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
-    if (Plan::PRED_DT && !al(F.pred_col)) return false;
+    if (!al(F.pred_col)) return false;
     for (int k = 0; k < Plan::NG; ++k) if (!al(F.gcol[k])) return false;
     for (int s = 0; s < Plan::NF; ++s) if (!al(F.fcol[s])) return false;
     return true;
@@ -756,70 +633,46 @@ bool match_plan(const Request& R, FusedArgs& F) {
 // --- the instantiated plans -------------------------------------------------------------------
 // Q1 (apps/tpc-h/tpch.py:108-117 after de-duplicating the AVG partial sums): pred on a date32 column,
 // 2 code keys, fp64 slots {0: qty, 1: extendedprice, 2: discount, 3: tax}
-using PlanQ1 = DensePlan<QK_I32, 2, 4,
+using PlanQ1 = DensePlan<2, 4,
     AggList<Prod<Col<0>>, Prod<Col<1>>, Prod<Col<1>, KMinus<2, 0>>, Prod<Col<1>, KMinus<2, 1>, KPlus<3, 2>>, Prod<Col<2>>>, 3>;
-// sum(a * (k - b)) by one code key, optional date predicate (Q5 / Q3-style revenue by a dictionary key)
-using PlanRev1 = DensePlan<QK_I32, 1, 2, AggList<Prod<Col<0>, KMinus<1, 0>>>, 1>;
-// sum(a * b) ungrouped with a date predicate is Q6-like; grouped by one key here
-using PlanMul1 = DensePlan<QK_I32, 1, 2, AggList<Prod<Col<0>, Col<1>>>, 0>;
+// sum(a * (k - b)) by one code key with a date predicate (Q5 / Q3-style revenue by a dictionary key): the runtime-described
+// plan takes the same request 6 % slower (SF-100 on H100, DESIGN.md section 4)
+using PlanRev1 = DensePlan<1, 2, AggList<Prod<Col<0>, KMinus<1, 0>>>, 1>;
+// sum(a * b) by one key with a date predicate (Q6's product, grouped); same margin over the runtime-described plan
+using PlanMul1 = DensePlan<1, 2, AggList<Prod<Col<0>, Col<1>>>, 0>;
 
 thread_local std::string g_variant, g_variant_cfg;
 
-template <class Plan, int NT, int V, int STAGES>
+template <class Plan, int V>
 int launch_tma(const FusedArgs& F, const DenseArgs& A, int64_t nrows, double* part_acc, long long* part_cnt,
                int* nblocks_out, cudaStream_t st, const char* name) {
-    using L = TileLayout<Plan, NT * V>;
-    const size_t acc_bytes = (size_t)A.n_groups * (Plan::NAGG * 8 + 4) * NT;
-    const size_t smem = (size_t)STAGES * L::stage_bytes + acc_bytes;
+    using L = TileLayout<Plan, F_NT * V>;
+    const size_t acc_bytes = (size_t)A.n_groups * (Plan::NAGG * 8 + 4) * F_NT;
+    const size_t smem = (size_t)F_STAGES * L::stage_bytes + acc_bytes;
     if (smem > 227 * 1024 - 64) return 1;     // does not fit: caller tries the next configuration
-    auto kern = k_dense_agg_fused_tma<Plan, NT, V, STAGES>;
+    auto kern = k_dense_agg_fused_tma<Plan, V>;
     QK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int sms = sm_count();
-    const int64_t nfull = nrows / (NT * V);
+    const int64_t nfull = nrows / (F_NT * V);
     int nb = (int)(nfull < sms ? (nfull > 0 ? nfull : 1) : sms);       // persistent: one CTA per SM
-    kern<<<nb, NT, smem, st>>>(F, A, nrows, part_acc, part_cnt);
+    kern<<<nb, F_NT, smem, st>>>(F, A, nrows, part_acc, part_cnt);
     QK_LAUNCH_CHECK("k_dense_agg_fused_tma");
     *nblocks_out = nb;
     char buf[96];
     snprintf(buf, sizeof buf, "fused_tma:%s", name);
     g_variant = buf;
-    g_variant_cfg = std::string("nt") + std::to_string(NT) + "v" + std::to_string(V) + "s" + std::to_string(STAGES);
+    g_variant_cfg = std::string("nt") + std::to_string(F_NT) + "v" + std::to_string(V) + "s" + std::to_string(F_STAGES);
     return 0;
 }
 
+// 4 rows per thread per tile; groupings whose partial states leave no room for that ring take 2, then 1 (1 = nothing fits)
 template <class Plan>
-int launch_fused(const FusedArgs& F, const DenseArgs& A, int64_t nrows, int variant, double* part_acc,
-                 long long* part_cnt, int* nblocks_out, cudaStream_t st, const char* name) {
-    // variant 3 = default TMA configuration; 4..6 = alternative (threads, rows/thread, stages) shapes kept
-    // selectable for profiling
-    switch (variant) {
-        case 3: {   // default shape: 256 threads x 4 rows, 3 stages
-            int rc = launch_tma<Plan, 256, 4, 3>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
-            if (rc == 1) rc = launch_tma<Plan, 256, 2, 3>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
-            if (rc == 1) rc = launch_tma<Plan, 256, 1, 3>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
-            return rc;
-        }
-        case 4: return launch_tma<Plan, 512, 2, 2>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
-        case 5: return launch_tma<Plan, 512, 1, 4>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
-        case 6: return launch_tma<Plan, 256, 2, 6>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
-        default: break;
-    }
-    const size_t acc_bytes = (size_t)A.n_groups * (Plan::NAGG * 8 + 4) * F_NT;
-    const int sms = sm_count();
-    if (acc_bytes > 110 * 1024) return 1;
-    auto kern = k_dense_agg_fused_ldg<Plan>;
-    QK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)acc_bytes));
-    const int64_t ntiles = (nrows + F_TILE - 1) / F_TILE;
-    int per_sm = (int)((220 * 1024) / (acc_bytes + 1024));      // resident CTAs per SM (shared-memory bound)
-    if (per_sm > 3) per_sm = 3;
-    if (per_sm < 1) per_sm = 1;
-    int nb = (int)(ntiles < (int64_t)per_sm * sms ? (ntiles > 0 ? ntiles : 1) : per_sm * sms);
-    kern<<<nb, F_NT, acc_bytes, st>>>(F, A, nrows, part_acc, part_cnt);
-    QK_LAUNCH_CHECK("k_dense_agg_fused_ldg");
-    *nblocks_out = nb;
-    g_variant = std::string("fused_ldg:") + name;
-    g_variant_cfg = "nt256v4";
-    return 0;
+int launch_fused(const FusedArgs& F, const DenseArgs& A, int64_t nrows, double* part_acc, long long* part_cnt,
+                 int* nblocks_out, cudaStream_t st, const char* name) {
+    int rc = launch_tma<Plan, 4>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
+    if (rc == 1) rc = launch_tma<Plan, 2>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
+    if (rc == 1) rc = launch_tma<Plan, 1>(F, A, nrows, part_acc, part_cnt, nblocks_out, st, name);
+    return rc;
 }
 
 
@@ -864,28 +717,20 @@ struct DyArgs {
 __device__ __forceinline__ const unsigned char* dy_base(const DyArgs& D, const unsigned char* stage, int c) {
     return stage ? stage + D.off[c] : D.src[c];
 }
-// FAST = the column types every TPC-H-shaped plan has (int32 range terms, fp64 compare terms and factors, uint8 code columns for
-// sets and group keys): typed loads instead of a dtype switch per access.
-template <bool FAST = false>
 __device__ __forceinline__ bool dy_term(const DyArgs& D, const DyTerm& T, const unsigned char* stage, int64_t i) {
     const unsigned char* p = dy_base(D, stage, T.col);
     const int dt = D.dtype[T.col];
     bool r;
     if (T.kind == 0) {
-        if constexpr (FAST) {
-            const int x = ((const int*)p)[i];
-            r = (x >= (int)T.ilo) & (x <= (int)T.ihi);
-        } else {
-            const long long x = load_i64(p, dt, i);
-            r = (x >= T.ilo) & (x <= T.ihi);
-        }
+        const long long x = load_i64(p, dt, i);
+        r = (x >= T.ilo) & (x <= T.ihi);
     } else if (T.kind == 1) {
-        const double v = FAST ? ((const double*)p)[i] : load_f64(p, dt, i);
+        const double v = load_f64(p, dt, i);
         r = (T.lo_open ? v > T.flo : v >= T.flo) & (T.hi_open ? v < T.fhi : v <= T.fhi);
     } else if (T.kind == 3) {
         r = cmp_i64(load_i64(p, dt, i), T.cmp, load_i64(dy_base(D, stage, T.col2), D.dtype[T.col2], i));
     } else {
-        const long long code = FAST ? (long long)p[i] : load_i64(p, dt, i);
+        const long long code = load_i64(p, dt, i);
         r = false;
         if (code >= 0 && code < (long long)T.nbits)
             r = T.nbits <= 64 ? ((T.bits >> code) & 1ull) != 0 : ((__ldg((const unsigned*)(uintptr_t)T.bits + (code >> 5)) >> (code & 31)) & 1u) != 0;
@@ -893,39 +738,11 @@ __device__ __forceinline__ bool dy_term(const DyArgs& D, const DyTerm& T, const 
     return r != (T.neg != 0);
 }
 
-template <int NT>
-__device__ __forceinline__ void dy_row(const DyArgs& D, const DenseArgs& A, const unsigned char* stage, int64_t i, double* acc, unsigned* cnt) {
-    bool pass = true;
-    for (int k = 0; k < D.nterms; ++k) pass &= dy_term(D, D.term[k], stage, i);
-    int g = 0;
-    for (int k = 0; k < A.ngroup_cols; ++k)
-        g += (int)load_i64(dy_base(D, stage, D.gcol[k]), D.dtype[D.gcol[k]], i) * A.group_stride[k];
-    g = min(max(g, 0), A.n_groups - 1);
-    for (int j = 0; j < A.nagg; ++j) {
-        const DyAgg& G = D.agg[j];
-        double x = 1.0;
-        for (int f = 0; f < G.nfact; ++f) {
-            const DyFactor& F = G.f[f];
-            double v = F.k0;
-            if (F.col >= 0) {
-                const double c = load_f64(dy_base(D, stage, F.col), D.dtype[F.col], i);
-                v = (F.k0 == 0.0 && F.k1 == 1.0) ? c : F.k0 + F.k1 * c;
-            }
-            x = f == 0 ? v : x * v;
-        }
-        if (G.gate >= 0 && !dy_term(D, D.term[G.gate], stage, i)) x = 0.0;
-        double* a = &acc[(g * A.nagg + j) * NT + threadIdx.x];
-        const int op = A.agg_op[j];
-        if (op == QK_AGG_SUM) *a += pass ? x : 0.0;
-        else if (pass) *a = agg_combine(op, *a, x);
-    }
-    cnt[g * NT + threadIdx.x] += pass ? 1u : 0u;
-}
-
 // V rows of one thread at once, every step over all V rows before the next step: the loads of a step (one per row) are
 // independent, so V of them are in flight per thread instead of one dependent chain per row (with 8 warps per SM and a
-// serial per-row walk the kernel is bound by shared-memory latency, not by HBM).  Rows are idx0 + r * stride.
-template <int NT, int V, bool FAST>
+// serial per-row walk the kernel is bound by shared-memory latency, not by HBM).  Rows are idx0 + r * stride.  Any column
+// type: the walk of plans the typed tile walk does not take, and (V = 1, unstaged) the ragged tail of every plan.
+template <int NT, int V>
 __device__ __forceinline__ void dy_rows(const DyArgs& D, const DenseArgs& A, const unsigned char* stage, int64_t idx0, int64_t stride,
                                         double* acc, unsigned* cnt) {
     bool pass[V];
@@ -934,13 +751,13 @@ __device__ __forceinline__ void dy_rows(const DyArgs& D, const DenseArgs& A, con
     for (int r = 0; r < V; ++r) { pass[r] = true; g[r] = 0; }
     for (int k = 0; k < D.nterms; ++k) {
 #pragma unroll
-        for (int r = 0; r < V; ++r) pass[r] &= dy_term<FAST>(D, D.term[k], stage, idx0 + r * stride);
+        for (int r = 0; r < V; ++r) pass[r] &= dy_term(D, D.term[k], stage, idx0 + r * stride);
     }
     for (int k = 0; k < A.ngroup_cols; ++k) {
         const unsigned char* p = dy_base(D, stage, D.gcol[k]);
         const int dt = D.dtype[D.gcol[k]], gs = A.group_stride[k];
 #pragma unroll
-        for (int r = 0; r < V; ++r) g[r] += (FAST ? (int)p[idx0 + r * stride] : (int)load_i64(p, dt, idx0 + r * stride)) * gs;
+        for (int r = 0; r < V; ++r) g[r] += (int)load_i64(p, dt, idx0 + r * stride) * gs;
     }
 #pragma unroll
     for (int r = 0; r < V; ++r) g[r] = min(max(g[r], 0), A.n_groups - 1);
@@ -956,7 +773,7 @@ __device__ __forceinline__ void dy_rows(const DyArgs& D, const DenseArgs& A, con
             for (int r = 0; r < V; ++r) {
                 double v = F.k0;
                 if (p) {
-                    const double c = FAST ? ((const double*)p)[idx0 + r * stride] : load_f64(p, dt, idx0 + r * stride);
+                    const double c = load_f64(p, dt, idx0 + r * stride);
                     v = plain ? c : F.k0 + F.k1 * c;
                 }
                 x[r] = f == 0 ? v : x[r] * v;
@@ -964,7 +781,7 @@ __device__ __forceinline__ void dy_rows(const DyArgs& D, const DenseArgs& A, con
         }
         if (G.gate >= 0) {
 #pragma unroll
-            for (int r = 0; r < V; ++r) if (!dy_term<FAST>(D, D.term[G.gate], stage, idx0 + r * stride)) x[r] = 0.0;
+            for (int r = 0; r < V; ++r) if (!dy_term(D, D.term[G.gate], stage, idx0 + r * stride)) x[r] = 0.0;
         }
         const int op = A.agg_op[j];
 #pragma unroll
@@ -1149,13 +966,13 @@ __global__ void __launch_bounds__(NT, 1) k_dense_agg_dyn_tma(const __grid_consta
         mbar_wait(smem_u32(&bars[s]), parity);
         const unsigned char* st = stages + (size_t)s * D.stage_bytes;
         if constexpr (FAST) dy_tile_fast<NT, V>(D, A, smem_u32(st), acc, cnt);
-        else dy_rows<NT, V, false>(D, A, st, threadIdx.x, NT, acc, cnt);
+        else dy_rows<NT, V>(D, A, st, threadIdx.x, NT, acc, cnt);
         __syncthreads();
         if (threadIdx.x == 0 && it + STAGES < my_n) issue(blockIdx.x + (it + STAGES) * gridDim.x, s);
         if (++s == STAGES) { s = 0; parity ^= 1u; }
     }
     if (blockIdx.x == 0)
-        for (int64_t row = nfull * TILE + threadIdx.x; row < nrows; row += NT) dy_row<NT>(D, A, nullptr, row, acc, cnt);
+        for (int64_t row = nfull * TILE + threadIdx.x; row < nrows; row += NT) dy_rows<NT, 1>(D, A, nullptr, row, NT, acc, cnt);
     cta_flush<NT>(acc, cnt, A, part_acc, part_cnt);
 }
 
@@ -1211,21 +1028,13 @@ struct DyBuilder {
             out.neg = !out.neg;
             return true;
         }
-        if (x.op == QK_OP_CMP_COL_IMM) {
+        if (x.op == QK_OP_CMP_COL_IMM || x.op == QK_OP_RANGE_COL_IMM) {
             const int s = slot(x.a0);
             if (s < 0) return false;
-            FusedArgs F{};
-            range_of(x.a1, x.imm_i, R.cols[x.a0].dtype == QK_I32 ? QK_I32 : QK_I64, F);
-            if (R.cols[x.a0].dtype == QK_U8) { if (F.pred_lo < 0) F.pred_lo = 0; }
-            out.col = (int8_t)s; out.kind = 0; out.neg = (int8_t)F.pred_neg; out.ilo = F.pred_lo; out.ihi = F.pred_hi;
-            return true;
-        }
-        if (x.op == QK_OP_RANGE_COL_IMM) {
-            const int s = slot(x.a0);
-            if (s < 0) return false;
-            FusedArgs F{};
-            range_closed(x.imm_i, (int64_t)x.imm, x.a1 != 0, R.cols[x.a0].dtype == QK_I32 ? QK_I32 : QK_I64, F);
-            out.col = (int8_t)s; out.kind = 0; out.neg = (int8_t)F.pred_neg; out.ilo = F.pred_lo; out.ihi = F.pred_hi;
+            const qk_expr_node nd{x.op, x.a0, x.a1, 0, x.imm, x.imm_i};
+            IntRange r = int_range(nd, R.cols[x.a0].dtype);
+            if (x.op == QK_OP_CMP_COL_IMM && R.cols[x.a0].dtype == QK_U8 && r.lo < 0) r.lo = 0;
+            out.col = (int8_t)s; out.kind = 0; out.neg = (int8_t)r.neg; out.ilo = r.lo; out.ihi = r.hi;
             return true;
         }
         if (x.op == QK_OP_CMP_COL_COL) {
@@ -1543,6 +1352,9 @@ extern "C" int qk_scan_filter_agg_dense(const qk_column* cols, int32_t ncols, in
                                         int32_t variant, void* stream) {
     static thread_local Programs P;
     const char* who = "qk_scan_filter_agg_dense";
+    if (variant != 0 && variant != 1 && variant != 3 && variant != 7)
+        QK_FAIL(QK_ERR_INVALID, "%s: variant %d is not 0 (auto), 1 (interpreter), 3 (typed plan, else runtime-described) or 7 "
+                "(runtime-described plan)", who, variant);
     if (ngroup_cols < 0 || ngroup_cols > 4 || nagg < 0 || nagg > QK_MAX_AGGS) QK_FAIL(QK_ERR_INVALID, "%s: ngroup_cols / nagg out of range", who);
     if (!cnt || (nagg > 0 && (!acc || !agg_expr || !agg_op))) QK_FAIL(QK_ERR_INVALID, "%s: null output / aggregate arguments", who);
     if (int rc = pack_programs(P, cols, ncols, nrows, pred, agg_expr, nagg, who)) return rc;
@@ -1571,27 +1383,20 @@ extern "C" int qk_scan_filter_agg_dense(const qk_column* cols, int32_t ncols, in
     if (variant != 1) {
         Request R{cols, ncols, nrows, pred, group_cols, group_card, ngroup_cols, agg_expr, agg_op, nagg};
         FusedArgs F{};
-        // auto: TMA-staged fused kernel first (measured faster), then the LDG one, then the interpreter
-        const int order[2] = {variant == 0 ? 3 : variant, variant == 0 ? 2 : -1};
+        // a typed plan first (variants 0, 3), then the runtime-described plan, then (variant 0 only) the interpreter
         int rc = 1;
-        for (int a = 0; a < 2 && rc == 1 && order[a] > 0 && variant != 7; ++a) {
-            const int v = order[a];
-            if (match_plan<PlanQ1>(R, F)) rc = launch_fused<PlanQ1>(F, A, nrows, v, part_acc, part_cnt, &nblocks, st, "q1");
-            else if (match_plan<PlanRev1>(R, F)) rc = launch_fused<PlanRev1>(F, A, nrows, v, part_acc, part_cnt, &nblocks, st, "rev1");
-            else if (match_plan<PlanMul1>(R, F)) rc = launch_fused<PlanMul1>(F, A, nrows, v, part_acc, part_cnt, &nblocks, st, "mul1");
-            else break;
+        if (variant != 7) {
+            if (match_plan<PlanQ1>(R, F)) rc = launch_fused<PlanQ1>(F, A, nrows, part_acc, part_cnt, &nblocks, st, "q1");
+            else if (match_plan<PlanRev1>(R, F)) rc = launch_fused<PlanRev1>(F, A, nrows, part_acc, part_cnt, &nblocks, st, "rev1");
+            else if (match_plan<PlanMul1>(R, F)) rc = launch_fused<PlanMul1>(F, A, nrows, part_acc, part_cnt, &nblocks, st, "mul1");
+        }
+        if (rc == 1) {
+            // no typed plan: the runtime-described plan over the same TMA tile ring (any aggregate of the grammar above)
+            static thread_local DyArgs D;
+            if (match_dyn(R, D, A)) rc = launch_dyn(D, A, nrows, part_acc, part_cnt, &nblocks, st);
         }
         if (rc < 0) return rc;
         done = rc == 0;
-        if (!done && (variant == 0 || variant == 3 || variant == 7)) {
-            // no typed plan: the runtime-described plan over the same TMA tile ring (any aggregate of the grammar above)
-            static thread_local DyArgs D;
-            if (match_dyn(R, D, A)) {
-                rc = launch_dyn(D, A, nrows, part_acc, part_cnt, &nblocks, st);
-                if (rc < 0) return rc;
-                done = rc == 0;
-            }
-        }
         if (!done && variant != 0) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: no fused plan matches this request (variant %d forced)", who, variant);
     }
     if (!done) {

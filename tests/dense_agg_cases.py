@@ -69,7 +69,7 @@ class Term:
 
 
 def irange(c, cmp, k) -> Term:
-    """integer column <cmp> integer constant (any int64 constant: range_of clamps it to the column's width)"""
+    """integer column <cmp> integer constant (any int64 constant: int_range clamps it to the column's width)"""
     return Term(f"{c} {cmp} {fmt(int(k))}", (c,), lambda d: _NP_CMP[cmp](d[c].astype(np.int64), np.int64(k)), "irange")
 
 

@@ -57,6 +57,19 @@ def test_argument_errors_are_reported_without_a_gpu():
     assert b"dtype" in lib.qk_last_error()
 
 
+@pytest.mark.parametrize("variant", [2, 4, 5, 6, 8, -1])
+def test_dense_agg_rejects_unknown_variants_first(variant):
+    """qk_scan_filter_agg_dense takes variants 0, 1, 3 and 7; any other is refused before the other arguments are looked
+    at (here ngroup_cols = -1 and null columns would be errors too)."""
+    from quokka_b200 import _lib as L
+    lib = L.lib()
+    args = (None, 0, 0, None, None, None, -1, None, None, 0, None, None, None, 0)
+    assert lib.qk_scan_filter_agg_dense(*args, variant, None) == -1
+    assert b"variant" in lib.qk_last_error()
+    assert lib.qk_scan_filter_agg_dense(*args, 0, None) == -1                # a known variant: the next check fails
+    assert b"variant" not in lib.qk_last_error()
+
+
 def test_no_cpu_fallback_in_ops():
     import torch
     from quokka_b200 import _lib as L, ops

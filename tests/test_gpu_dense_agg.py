@@ -1,6 +1,6 @@
 """Every device path of qk_scan_filter_agg_dense (csrc/scan.cu) against the exact reference of tests/dense_agg_cases.py:
-the typed plans q1 / rev1 / mul1 (LDG kernel, variant 2; TMA kernel, variants 3-6), the runtime-described plan (variant 7)
-in each of its six (threads x rows) shapes with its typed tile walk (config ends in "t") and its generic per-row walk, and
+the typed plans q1 / rev1 / mul1 (TMA kernel, variant 3, in each shape of its fallback chain), the runtime-described plan
+(variant 7) in each of its six (threads x rows) shapes with its typed tile walk (config ends in "t") and its generic per-row walk, and
 the postfix interpreter (variant 1).  After every call the test asserts which kernel, shape and walk ran.
 
 On dyadic data every path matches the reference bit for bit, SUMs included; on TPC-H data SUMs are within
@@ -139,11 +139,11 @@ def typed_plan(name, mode, pred_hi=500):
     return D.Plan(pred, [("k8a", 3)], [D.Agg("sum", [D.f_col("fa"), D.f_col("fb")])])
 
 
-TYPED_CFG = {0: "nt256v4s3", 2: "nt256v4", 3: "nt256v4s3", 4: "nt512v2s2", 5: "nt512v1s4", 6: "nt256v2s6"}
+TYPED_CFG = {0: "nt256v4s3", 3: "nt256v4s3"}
 
 
 @pytest.mark.parametrize("mode", ["dyadic", "tpch"])
-@pytest.mark.parametrize("variant", [0, 2, 3, 4, 5, 6])
+@pytest.mark.parametrize("variant", [0, 3])
 @pytest.mark.parametrize("name", ["q1", "rev1", "mul1"])
 def test_typed_plans(qk, name, variant, mode):
     plan = typed_plan(name, mode)
@@ -153,21 +153,52 @@ def test_typed_plans(qk, name, variant, mode):
         d, dd = data(n, n + 3, mode)
         v, cfg = run_and_check(qk, plan, d, dd, variant, mode == "dyadic", name)
         if n:
-            assert (v, cfg) == (("fused_ldg:" if variant == 2 else "fused_tma:") + name, TYPED_CFG[variant])
+            assert (v, cfg) == ("fused_tma:" + name, TYPED_CFG[variant])
 
 
-def test_typed_plan_int32_bound_beyond_int32(qk):
-    """`i32a < 2^32 + 5` holds for every int32: the typed plans and the typed tile walk compare in 32 bits, so range_of must
-    clamp the bound to INT32_MAX, not truncate it."""
+def test_int32_bound_beyond_int32_is_clamped(qk):
+    """`i32a < 2^32 + 5` holds for every int32: the typed plans and the typed tile walk compare in 32 bits, so int_range
+    (csrc/common.cuh) must clamp the bound to INT32_MAX, not truncate it."""
     d, dd = data(50_003, 9)
     for k in ((1 << 32) + 5, -(1 << 32) + 5, D.I32_MAX + 1, D.I32_MIN):
         for cmp in D.CMPS:
             plan = typed_plan("mul1", "dyadic")
             plan.terms = [D.irange("i32a", cmp, k)]
-            for variant in (2, 3, 1):
+            for variant in (3, 1):
                 run_and_check(qk, plan, d, dd, variant, True, f"i32a {cmp} {k}")
             plan.aggs.append(D.Agg("min", [D.f_kplus(20.0, "fa")]))           # not a typed plan: the dyn plan, typed walk
             assert_dyn(*run_and_check(qk, plan, d, dd, 7, True, f"i32a {cmp} {k}"), fast=True)
+
+
+# 256 threads x V rows x 3 stages of Q1's 38 B rows plus 256 lane-private copies of 5 SUMs and a count per group must fit
+# 227 KB (csrc/scan.cu launch_tma)
+Q1_ROW_BYTES, Q1_GROUP_BYTES = 38, 5 * 8 + 4
+
+
+def typed_q1_max_groups(v):
+    return (D.SMEM_CAP - 3 * Q1_ROW_BYTES * 256 * v) // (Q1_GROUP_BYTES * 256)
+
+
+@pytest.mark.parametrize("v", [4, 2, 1])
+def test_typed_q1_largest_grouping_per_shape(qk, v):
+    """The typed Q1 plan at the largest group count each shape of its fallback chain (256 threads x 4, 2, 1 rows) holds
+    runs in that shape; one group more takes the next shape, and after the last one the runtime-described plan."""
+    ng = typed_q1_max_groups(v)
+    assert ng == {4: 10, 2: 15, 1: 18}[v]
+    n = 60_011
+    rng = np.random.default_rng(100 + v)
+    for groups, want in ((ng, ("fused_tma:q1", f"nt256v{v}s3")),
+                         (ng + 1, ("fused_tma:q1", f"nt256v{v // 2}s3") if v > 1 else ("fused_tma:dyn", None))):
+        cards = next(((groups // p, p) for p in (3, 2) if groups % p == 0), (groups, 1))
+        d = {"i32a": rng.integers(-1000, 1000, n).astype(np.int32),
+             "q0": rng.integers(0, cards[0], n).astype(np.uint8), "q1": rng.integers(0, cards[1], n).astype(np.uint8)}
+        for c in ("fa", "fb", "fc", "fd"):
+            d[c] = D.dyadic(rng, n)
+        dd = {k: torch.from_numpy(x).cuda() for k, x in d.items()}
+        plan = typed_plan("q1", "dyadic")
+        plan.keys = [("q0", cards[0]), ("q1", cards[1])]
+        v_, cfg = run_and_check(qk, plan, d, dd, 0, True, f"ng {groups}")
+        assert v_ == want[0] and (want[1] is None or cfg == want[1]), (groups, v_, cfg)
 
 
 # ------------------------------------------------------------------ targeted edges of the grammar, both walks

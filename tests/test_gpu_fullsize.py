@@ -20,7 +20,7 @@ def qb():
     return type("QB", (), dict(L=_lib, E=expr, ops=ops, synth=synth))
 
 
-def test_q1_sf10_against_independent_fp64(qb):
+def test_q1_sf10_typed_dyn_and_interpreter_against_independent_fp64(qb):
     sf, names = 10, ["l_shipdate", "l_returnflag", "l_linestatus", "l_quantity", "l_extendedprice", "l_discount", "l_tax"]
     cols = {c: qb.synth.column(c, sf) for c in names}
     n = cols["l_shipdate"].numel()
@@ -30,7 +30,7 @@ def test_q1_sf10_against_independent_fp64(qb):
     aggs = [qb.E.compile_expr(qb.E.parse(a), sch) for a in
             ("l_quantity", "l_extendedprice", "l_extendedprice * (1 - l_discount)",
              "l_extendedprice * (1 - l_discount) * (1 + l_tax)", "l_discount")]
-    for variant in (0, 2, 1):
+    for variant in (0, 7, 1):
         st = qb.ops.DenseAggState([3, 2], [qb.L.AGG_SUM] * 5, "cuda")
         st.update(list(cols.values()), pred, [1, 2], aggs, variant=variant)
         m = cols["l_shipdate"] <= G.DAY_1998_09_02

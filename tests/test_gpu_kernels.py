@@ -187,8 +187,7 @@ def check_q1(st, li):
     np.testing.assert_allclose(acc[gid, 0] / cnt[gid], exp["avg_qty"], rtol=RTOL, atol=0)
 
 
-@pytest.mark.parametrize("variant,name", [(1, "generic"), (2, "fused_ldg:q1"), (3, "fused_tma:q1"), (4, "fused_tma:q1"),
-                                          (5, "fused_tma:q1"), (6, "fused_tma:q1"), (0, "fused_tma:q1")])
+@pytest.mark.parametrize("variant,name", [(1, "generic"), (3, "fused_tma:q1"), (7, "fused_tma:dyn"), (0, "fused_tma:q1")])
 @pytest.mark.parametrize("n", [1, 1023, 1024, 1025, 4099, 300_007])
 def test_q1_dense_agg_variants(qb, variant, name, n):
     li = G.gen_lineitem(1, 5_000_000, 5_000_000 + n, Q1_COLS)
@@ -198,12 +197,12 @@ def test_q1_dense_agg_variants(qb, variant, name, n):
     check_q1(st, li)
 
 
-def test_q1_dense_agg_accumulates_over_batches_and_is_deterministic(qb):
+def test_q1_typed_plan_accumulates_over_batches_and_is_deterministic(qb):
     n = 500_000
     li = G.gen_lineitem(1, 0, n, Q1_COLS)
     d = {k: dev(li[k]) for k in Q1_COLS}
-    whole = run_q1_dense(qb, d, 2)
-    again = run_q1_dense(qb, d, 2)
+    whole = run_q1_dense(qb, d, 3)
+    again = run_q1_dense(qb, d, 3)
     assert torch.equal(whole.acc, again.acc) and torch.equal(whole.cnt, again.cnt)     # fixed reduction order
     sch = _schema(qb, d)
     pred = qb.E.compile_expr(qb.E.parse("l_shipdate <= date '1998-09-02'"), sch)
@@ -216,7 +215,7 @@ def test_q1_dense_agg_accumulates_over_batches_and_is_deterministic(qb):
     np.testing.assert_allclose(host(st.acc), host(whole.acc), rtol=1e-12)
 
 
-def test_dense_agg_min_max_and_other_plans(qb):
+def test_dense_agg_min_max_and_rev1_typed_and_dyn(qb):
     n = 200_000
     li = G.gen_lineitem(1, 0, n, Q1_COLS)
     d = {k: dev(li[k]) for k in Q1_COLS}
@@ -231,9 +230,9 @@ def test_dense_agg_min_max_and_other_plans(qb):
     acc = host(st.acc)
     assert np.array_equal(acc[gid, 0], exp["mn"]) and np.array_equal(acc[gid, 1], exp["mx"])
     np.testing.assert_allclose(acc[gid, 2], exp["s"], rtol=RTOL)
-    # revenue-by-one-key plan (fused "rev1"), both staging variants
+    # revenue-by-one-key plan: the typed "rev1" plan and the runtime-described plan
     sch = _schema(qb, d)
-    for variant, name in ((2, "fused_ldg:rev1"), (3, "fused_tma:rev1")):
+    for variant, name in ((3, "fused_tma:rev1"), (7, "fused_tma:dyn")):
         st = qb.ops.DenseAggState([3], [qb.L.AGG_SUM], "cuda")
         st.update(list(d.values()), qb.E.compile_expr(qb.E.parse("l_shipdate > date '1995-03-15'"), sch), [sch["l_returnflag"].slot],
                   [qb.E.compile_expr(qb.E.parse("l_extendedprice * (1 - l_discount)"), sch)], variant=variant)
