@@ -273,14 +273,11 @@ extern "C" int qk_asof_backward(const qk_column* l_time, const qk_column* l_by, 
     int32_t* sorted_idx = (int32_t*)w; w += align_up((size_t)nr * 4, 256);
     if (int rc = qk_partition_plan(r_by, n_by, QK_PART_CODE, dest, seg, w, ws_bytes - asof_fixed_bytes(nr, n_by), stream)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const int cap = sm_count() * 16;
     if (nr > 0) {
-        int64_t nb = (nr + 255) / 256; if (nb > cap) nb = cap;
-        k_asof_prepare<<<(unsigned)nb, 256, 0, st>>>((const long long*)r_time->data, dest, nr, sorted_time, sorted_idx);
+        k_asof_prepare<<<grid_size(nr, 16), 256, 0, st>>>((const long long*)r_time->data, dest, nr, sorted_time, sorted_idx);
         QK_LAUNCH_CHECK("k_asof_prepare");
     }
-    int64_t nb = (nl + 255) / 256; if (nb > cap) nb = cap;
-    k_asof_search<<<(unsigned)nb, 256, 0, st>>>((const long long*)l_time->data, (const int32_t*)l_by->data, nl, n_by,
+    k_asof_search<<<grid_size(nl, 16), 256, 0, st>>>((const long long*)l_time->data, (const int32_t*)l_by->data, nl, n_by,
                                                 sorted_time, sorted_idx, seg, out_ridx);
     QK_LAUNCH_CHECK("k_asof_search");
     return QK_OK;

@@ -68,6 +68,18 @@ static inline int check_col(const qk_column* c, const char* what) {
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// grid of a grid-stride launch: one CTA per `per_cta` work items, at most `per_sm` CTAs per SM, at least one CTA
+static inline unsigned grid_size(int64_t n, int per_sm, int64_t per_cta = 256) {
+    const int64_t nb = (n + per_cta - 1) / per_cta, cap = (int64_t)sm_count() * per_sm;
+    return (unsigned)(nb < 1 ? 1 : (nb > cap ? cap : nb));
+}
+
+// counts -> exclusive offsets, one CTA per row of a row-major rows x n count matrix:
+// offsets[b * n + i] = counts[b * n] + ... + counts[b * n + i - 1] and totals[b] = the sum of row b.
+// With rows = 1 and totals = offsets + n, offsets[n] holds the total.  Instantiated for uint32_t and int64_t counts.
+template <typename T>
+int count_offsets(const T* counts, int64_t rows, int64_t n, int64_t* offsets, int64_t* totals, cudaStream_t st);
+
 // An integer-range predicate node (QK_OP_CMP_COL_IMM or QK_OP_RANGE_COL_IMM) as the branch-free test
 // ((lo <= x) & (x <= hi)) != neg, its bounds clamped to 32 bits when the column is QK_I32 (a kernel that compares in
 // 32 bits must not truncate a bound beyond int32) and to 64 bits otherwise.  An empty range is lo = 1, hi = 0.
@@ -140,18 +152,6 @@ __device__ __forceinline__ unsigned long long l2_policy_evict_first() {
 __device__ __forceinline__ unsigned long long l2_policy_evict_last() {
     unsigned long long p; asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p)); return p;
 }
-__device__ __forceinline__ unsigned ld_u32_hint(const void* p, unsigned long long pol) {
-    unsigned v; asm volatile("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol)); return v;
-}
-__device__ __forceinline__ unsigned ld_u8_stream(const void* p, unsigned long long pol) {
-    unsigned v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol)); return v;
-}
-__device__ __forceinline__ int ld_i32_stream(const void* p, unsigned long long pol) {
-    int v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.s32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol)); return v;
-}
-__device__ __forceinline__ long long ld_i64_stream(const void* p, unsigned long long pol) {
-    long long v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.s64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol)); return v;
-}
 
 // key mod nparts (non-negative result) without a 64-bit division: nparts is the number of ranks (1, 2, 4, 8 in practice).
 // A 64-bit `%` by a runtime divisor costs ~120 instructions per row and made the mask kernel instruction-bound.
@@ -171,6 +171,55 @@ __device__ __forceinline__ unsigned part_mod(long long key, unsigned nparts) {
 __device__ __forceinline__ unsigned lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ unsigned lanemask_lt() {
     unsigned m; asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m)); return m;
+}
+
+// inclusive prefix sum over the lanes of a warp (all 32 lanes active)
+template <typename T>
+__device__ __forceinline__ T warp_inclusive_scan(T x) {
+    for (int o = 1; o < 32; o <<= 1) {
+        const T y = __shfl_up_sync(0xffffffffu, x, o);
+        if ((int)lane_id() >= o) x += y;
+    }
+    return x;
+}
+
+// CTA-wide sums over NT threads.  Each takes a shared buffer of NT / 32 slots and holds the one __syncthreads between
+// writing it and reading it; a caller that uses the buffer again must pass a __syncthreads of its own first.
+
+// exclusive prefix sum of v in thread order; total = the CTA's sum
+template <int NT, typename T>
+__device__ __forceinline__ T cta_exclusive_scan(T v, T* wsum, T& total) {
+    const int warp = threadIdx.x >> 5;
+    const T x = warp_inclusive_scan(v);
+    if (lane_id() == 31) wsum[warp] = x;
+    __syncthreads();
+    T before = 0;
+    total = 0;
+    for (int w = 0; w < NT / 32; ++w) { if (w < warp) before += wsum[w]; total += wsum[w]; }
+    return before + x - v;
+}
+// the same over one flag per thread, given as its warp's ballot `bal`: the thread's rank among the CTA's set flags
+// (meaningful where the thread's own bit is set); total = the CTA's number of set flags
+template <int NT>
+__device__ __forceinline__ int cta_ballot_rank(unsigned bal, int* wsum, int& total) {
+    const int warp = threadIdx.x >> 5;
+    if (lane_id() == 0) wsum[warp] = __popc(bal);
+    __syncthreads();
+    int before = 0;
+    total = 0;
+    for (int w = 0; w < NT / 32; ++w) { if (w < warp) before += wsum[w]; total += wsum[w]; }
+    return before + __popc(bal & lanemask_lt());
+}
+// sum of v over the CTA, returned in thread 0 (0 elsewhere)
+template <int NT, typename T>
+__device__ __forceinline__ T cta_sum(T v, T* wsum) {
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane_id() == 0) wsum[threadIdx.x >> 5] = v;
+    __syncthreads();
+    T t = 0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < NT / 32; ++w) t += wsum[w];
+    return t;
 }
 
 }  // namespace qk

@@ -3,13 +3,14 @@
 //     projection = verbatim columns (keys, measures, dates, codes).
 // i.e. "filter by a range on one column and compact k columns" -- no expression evaluation at all.
 //
-// Two passes, no atomics, STABLE output (input row order is kept, so sorted streams stay sorted):
-//   pass 1  k_compact_count: every CTA counts the survivors of its contiguous chunk of rows (reads the
-//           predicate column only) -> k_compact_scan turns the counts into output offsets;
-//   pass 2  k_filter_compact_tma: column tiles of the chunk are staged into shared memory by the TMA
-//           engine (cp.async.bulk + mbarrier complete_tx, 3-stage ring, one elected producer thread); the
-//           CTA evaluates the predicate from shared memory, ranks the survivors of a tile with warp ballots
-//           + one small warp scan and writes them, column by column, at its running output offset.
+// Three passes, no atomics, STABLE output (input row order is kept, so sorted streams stay sorted):
+//   mask     k_compact_mask: every CTA evaluates the predicate (and the optional Bloom test) over its contiguous chunk
+//            of rows, writes one bit per row to a bitmap and the chunk's survivor count;
+//   scan     count_offsets (offsets.cu) turns the chunk counts into output offsets and the total into *out_rows;
+//   compact  k_filter_compact_tma: column tiles of the chunk are staged into shared memory by the TMA
+//            engine (cp.async.bulk + mbarrier complete_tx, 3-stage ring, one elected producer thread); the
+//            CTA ranks the survivors of a tile from the bitmap with one small warp scan and writes them, column by
+//            column, at its running output offset.  A chunk with few survivors skips the staging and gathers them.
 //
 // HBM-bound: reads (2 x pred + payload) bytes/row, writes payload bytes per surviving row.
 // Q3 lineitem scan at SF-100: 600 M x (28 + 4) B read + 324 M x 24 B written = 27.0 GB algorithmic.
@@ -41,7 +42,6 @@ struct CompactArgs {
     int32_t bloom_nparts, bloom_col;       // bloom_col = payload column holding the (int64 / int32) join key
 };
 
-// Blocked Bloom filter: one 32-byte block (a DRAM sector) per key, 3 bits inside it.
 // Blocked Bloom filter, one 64-bit word per key: the key picks a 32-byte block (a DRAM sector) of its partition's filter, one of
 // the block's four 64-bit words and three bits inside that word, so a test is ONE 8-byte load + one mask compare.  The hash is
 // two rounds of 32-bit multiply-xorshift (the mask kernel is instruction-bound: a 64-bit mix + three 4-byte probes cost
@@ -71,28 +71,6 @@ __device__ __forceinline__ void issue_tile(const CompactArgs& A, int64_t tile, u
     mbar_expect_tx(bar, (unsigned)A.stage_bytes);
     for (int c = 0; c < A.ncols; ++c)
         bulk_g2s(smem_u32(stage + A.off[c]), A.src[c] + base * A.width[c], (unsigned)(A.tile_rows * A.width[c]), bar);
-}
-
-__device__ __forceinline__ bool eval_pred(const CompactArgs& A, const unsigned char* p, int64_t i) {
-    if (!A.pred_col) return true;
-    long long x;
-    switch (A.pred_width) {
-        case 1: x = p[i]; break;
-        case 4: x = ((const int*)p)[i]; break;
-        default: x = ((const long long*)p)[i]; break;
-    }
-    return ((x >= A.pred_lo) & (x <= A.pred_hi)) != (A.pred_neg != 0);
-}
-// the same test on a column that is streamed once from global memory (pass 1): bypass L1, first to leave L2
-__device__ __forceinline__ bool eval_pred_stream(const CompactArgs& A, int64_t i, unsigned long long pol) {
-    if (!A.pred_col) return true;
-    long long x;
-    switch (A.pred_width) {
-        case 1: x = ld_u8_stream(A.pred_col + i, pol); break;
-        case 4: x = ld_i32_stream(A.pred_col + 4 * i, pol); break;
-        default: x = ld_i64_stream(A.pred_col + 8 * i, pol); break;
-    }
-    return ((x >= A.pred_lo) & (x <= A.pred_hi)) != (A.pred_neg != 0);
 }
 
 __device__ __forceinline__ void copy_row(const CompactArgs& A, const unsigned char* const* src, int64_t from, int64_t to) {
@@ -139,7 +117,7 @@ template <int W> __device__ __forceinline__ void load8(const unsigned char* col,
 }
 template <int PW, int KW>
 __global__ void __launch_bounds__(M_NT, 2) k_compact_mask(const __grid_constant__ CompactArgs A, int64_t nrows, int64_t chunk_rows,
-                                                          unsigned* bitmap, long long* counts) {
+                                                          unsigned* bitmap, int64_t* counts) {
     __shared__ int wsum[M_NT / 32];
     const int warp = threadIdx.x >> 5, lane = lane_id();
     const int64_t lo = blockIdx.x * chunk_rows;
@@ -194,40 +172,9 @@ __global__ void __launch_bounds__(M_NT, 2) k_compact_mask(const __grid_constant_
         v |= __shfl_xor_sync(0xffffffffu, v, 2);
         if ((lane & 3) == 0 && base + (int64_t)(lane >> 2) * 32 < hi) bitmap[(base >> 5) + (lane >> 2)] = v;
     }
-    for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    if (lane == 0) wsum[warp] = cnt;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        long long t = 0;
-        for (int w = 0; w < M_NT / 32; ++w) t += wsum[w];
-        counts[blockIdx.x] = t;
-    }
+    const int total = cta_sum<M_NT>(cnt, wsum);
+    if (threadIdx.x == 0) counts[blockIdx.x] = total;
 }
-// exclusive scan of up to 1024 chunk counts; offsets[n] = total, also stored to *out_rows
-__global__ void __launch_bounds__(1024) k_compact_scan(const long long* counts, int n, long long* offsets, long long* out_rows) {
-    __shared__ long long wtot[32];
-    const int i = threadIdx.x;
-    long long v = i < n ? counts[i] : 0, x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-        const long long y = __shfl_up_sync(0xffffffffu, x, o);
-        if ((int)lane_id() >= o) x += y;
-    }
-    if (lane_id() == 31) wtot[i >> 5] = x;
-    __syncthreads();
-    if (i < 32) {
-        long long w = wtot[i], t = w;
-        for (int o = 1; o < 32; o <<= 1) {
-            const long long y = __shfl_up_sync(0xffffffffu, t, o);
-            if ((int)lane_id() >= o) t += y;
-        }
-        wtot[i] = t - w;
-    }
-    __syncthreads();
-    const long long excl = wtot[i >> 5] + x - v;
-    if (i < n) offsets[i] = excl;
-    if (i == n - 1) { offsets[n] = excl + v; *out_rows = excl + v; }
-}
-
 template <typename T>
 __device__ __forceinline__ void copy_col(const unsigned char* src, unsigned char* dst, int slabs, unsigned my, const int* wcount,
                                          long long base, int warp, int lane) {
@@ -243,7 +190,8 @@ __device__ __forceinline__ void copy_col(const unsigned char* src, unsigned char
 
 // pass 2
 __global__ void __launch_bounds__(C_NT, 3) k_filter_compact_tma(const __grid_constant__ CompactArgs A, int64_t nrows, int64_t chunk_rows,
-                                                                const long long* offsets, const unsigned* __restrict__ bitmap) {
+                                                                const int64_t* counts, const int64_t* offsets,
+                                                                const unsigned* __restrict__ bitmap) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) unsigned long long bars[C_STAGES];
     __shared__ int wcount[C_MAXSLABS * (C_NT / 32) + 1];   // survivors per (slab, warp) -> exclusive prefix; [n] = tile total
@@ -257,7 +205,7 @@ __global__ void __launch_bounds__(C_NT, 3) k_filter_compact_tma(const __grid_con
     // Sparse chunk (fewer than 1 row in 8 survives, e.g. after the Bloom filter): do not stage whole tiles;
     // walk the bitmap and fetch only the surviving rows from global memory (one 32-byte sector per row
     // and column instead of the full column width for all rows).  Same output order.
-    if (hi > lo && (offsets[blockIdx.x + 1] - offsets[blockIdx.x]) * 8 < (hi - lo)) {
+    if (hi > lo && counts[blockIdx.x] * 8 < (hi - lo)) {
         __shared__ int wtot[C_NT / 32];
         long long run = offsets[blockIdx.x];
         const int64_t w_lo = lo >> 5, w_hi = (hi + 31) >> 5;
@@ -266,19 +214,11 @@ __global__ void __launch_bounds__(C_NT, 3) k_filter_compact_tma(const __grid_con
         for (int64_t wb = w_lo; wb < w_hi; wb += C_NT) {        // 256 bitmap words = 8192 rows per step
             const int64_t wi = wb + threadIdx.x;
             unsigned m = wi < w_hi ? __ldg(&bitmap[wi]) : 0u;
-            // exclusive scan of popc over the 256 threads
-            int v = __popc(m), x = v;
-            for (int o = 1; o < 32; o <<= 1) {
-                const int y = __shfl_up_sync(0xffffffffu, x, o);
-                if (lane >= o) x += y;
-            }
-            if (lane == 31) wtot[warp] = x;
-            __syncthreads();
-            int before = 0, total = 0;
-            for (int w = 0; w < C_NT / 32; ++w) { if (w < warp) before += wtot[w]; total += wtot[w]; }
+            int total;
+            const int first = cta_exclusive_scan<C_NT>(__popc(m), wtot, total);       // the thread's first survivor
             if (listed) {
                 // 1. every thread lists its survivors' row numbers (relative to the step) in output order
-                int slot = before + x - v;
+                int slot = first;
                 while (m) {
                     const int j = __ffs(m) - 1;
                     list[slot++] = (int)(threadIdx.x * 32 + j);
@@ -314,7 +254,7 @@ __global__ void __launch_bounds__(C_NT, 3) k_filter_compact_tma(const __grid_con
                     }
                 }
             } else {
-                long long pos = run + before + x - v;
+                long long pos = run + first;
                 while (m) {
                     const int j = __ffs(m) - 1;
                     copy_row(A, A.src, (wi << 5) + j, pos++);
@@ -354,11 +294,7 @@ __global__ void __launch_bounds__(C_NT, 3) k_filter_compact_tma(const __grid_con
             int carry = 0;
             for (int b = 0; b < nw; b += 32) {
                 const int i = b + lane;
-                int v = i < nw ? wcount[i] : 0, x = v;
-                for (int o = 1; o < 32; o <<= 1) {
-                    const int y = __shfl_up_sync(0xffffffffu, x, o);
-                    if (lane >= o) x += y;
-                }
+                const int v = i < nw ? wcount[i] : 0, x = warp_inclusive_scan(v);
                 if (i < nw) wcount[i] = carry + x - v;
                 carry += __shfl_sync(0xffffffffu, x, 31);
             }
@@ -387,12 +323,9 @@ __global__ void __launch_bounds__(C_NT, 3) k_filter_compact_tma(const __grid_con
         for (int64_t k0 = t0; k0 < hi; k0 += C_NT) {
             const int64_t row = k0 + threadIdx.x;
             const unsigned bal = k0 + warp * 32 < hi ? __ldg(&bitmap[(k0 >> 5) + warp]) : 0u;     // bits past `hi` are 0
-            const bool pass = (bal >> lane) & 1u;
-            if (lane == 0) tsum[warp] = __popc(bal);
-            __syncthreads();
-            int before = 0, total = 0;
-            for (int w = 0; w < C_NT / 32; ++w) { if (w < warp) before += tsum[w]; total += tsum[w]; }
-            if (pass) copy_row(A, A.src, row, running + before + __popc(bal & lanemask_lt()));
+            int total;
+            const int rank = cta_ballot_rank<C_NT>(bal, tsum, total);
+            if ((bal >> lane) & 1u) copy_row(A, A.src, row, running + rank);
             running += total;
             __syncthreads();
         }
@@ -451,14 +384,14 @@ int try_filter_compact_tma(const qk_column* cols, int ncols, int64_t nrows, cons
     // contiguous chunks of whole tiles, one per CTA
     const int64_t ntiles = (nrows + tile - 1) / tile;
     int64_t want = (int64_t)sms * ctas_per_sm;
-    if (want > 1024) want = 1024;
+    if (want > 1024) want = 1024;                        // the workspace below holds 1024 chunk counts and offsets
     const int64_t tiles_per_chunk = (ntiles + want - 1) / want;
     const int64_t chunk_rows = tiles_per_chunk * tile;
     const int nb = (int)((nrows + chunk_rows - 1) / chunk_rows);
     const size_t bitmap_bytes = align_up((size_t)((nrows + 31) / 32 + 8) * 4, 256);
     if (ws_bytes < (size_t)(2 * 1024 + 8) * 8 + bitmap_bytes || !workspace) return 1;
-    long long* counts = (long long*)workspace;
-    long long* offsets = counts + 1024;
+    int64_t* counts = (int64_t*)workspace;
+    int64_t* offsets = counts + 1024;
     unsigned* bitmap = (unsigned*)((char*)workspace + (size_t)(2 * 1024 + 8) * 8);
     if (A.bloom) {
         const int kd = cols[proj[A.bloom_col].nodes[0].a0].dtype;
@@ -473,18 +406,15 @@ int try_filter_compact_tma(const qk_column* cols, int ncols, int64_t nrows, cons
 #undef QK_MASK
     }
     QK_LAUNCH_CHECK("k_compact_mask");
-    k_compact_scan<<<1, 1024, 0, st>>>(counts, nb, offsets, (long long*)out_rows);
-    QK_LAUNCH_CHECK("k_compact_scan");
-    k_filter_compact_tma<<<nb, C_NT, smem, st>>>(A, nrows, chunk_rows, offsets, bitmap);
+    if (int rc = count_offsets(counts, 1, nb, offsets, out_rows, st)) return rc;
+    k_filter_compact_tma<<<nb, C_NT, smem, st>>>(A, nrows, chunk_rows, counts, offsets, bitmap);
     QK_LAUNCH_CHECK("k_filter_compact_tma");
     return 0;
 }
 
 int bloom_build(const qk_column* key, unsigned* bits, long long words_per_part, int nparts, cudaStream_t st) {
     if (key->length == 0) return QK_OK;
-    int64_t nb = (key->length + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_bloom_build<<<(unsigned)nb, 256, 0, st>>>(key->data, key->dtype, key->length, bits, words_per_part, nparts);
+    k_bloom_build<<<grid_size(key->length, 16), 256, 0, st>>>(key->data, key->dtype, key->length, bits, words_per_part, nparts);
     QK_LAUNCH_CHECK("k_bloom_build");
     return QK_OK;
 }

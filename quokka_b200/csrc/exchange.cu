@@ -355,10 +355,7 @@ extern "C" int qk_xchg_push(const qk_xchg* x, uint64_t epoch, const qk_column* c
         tiles += (hi - lo + X_TILE - 1) / X_TILE;
     }
     A.tile_base[x->world] = tiles;
-    long long nb = tiles < 1 ? 1 : tiles;
-    const long long cap = (long long)sm_count() * 4;
-    if (nb > cap) nb = cap;
-    k_xchg_push_contig<<<(unsigned)nb, X_NT, 0, (cudaStream_t)stream>>>(C, A);
+    k_xchg_push_contig<<<grid_size(tiles, 4, 1), X_NT, 0, (cudaStream_t)stream>>>(C, A);
     QK_LAUNCH_CHECK("k_xchg_push_contig");
     return QK_OK;
 }
@@ -372,10 +369,6 @@ extern "C" int qk_xchg_push_scatter(const qk_xchg* x, uint64_t epoch, const qk_c
     int64_t n = 0;
     if (int rc = fill_push(A, x, cols, ncols, dst_byte_off, &n, false, who)) return rc;
     if (n > 0 && (!dest || !part_offsets)) QK_FAIL(QK_ERR_INVALID, "%s: null partition plan", who);
-    long long nb = (n + X_TILE - 1) / X_TILE;
-    if (nb < 1) nb = 1;
-    const long long cap = (long long)sm_count() * 4;
-    if (nb > cap) nb = cap;
     if (n == 0) {
         for (int p = 0; p <= x->world; ++p) A.tile_base[p] = 0;
         for (int p = 0; p < x->world; ++p) A.send_lo[p] = A.send_hi[p] = 0;
@@ -383,7 +376,7 @@ extern "C" int qk_xchg_push_scatter(const qk_xchg* x, uint64_t epoch, const qk_c
         QK_LAUNCH_CHECK("k_xchg_push_contig");
         return QK_OK;
     }
-    k_xchg_push_scatter<<<(unsigned)nb, X_NT, 0, (cudaStream_t)stream>>>(C, A, dest, part_offsets, n);
+    k_xchg_push_scatter<<<grid_size(n, 4, X_TILE), X_NT, 0, (cudaStream_t)stream>>>(C, A, dest, part_offsets, n);
     QK_LAUNCH_CHECK("k_xchg_push_scatter");
     return QK_OK;
 }

@@ -186,9 +186,7 @@ extern "C" int qk_hashagg_init(const qk_hashagg_desc* desc, void* state, void* s
     if (int rc = make_layout(desc, &L, "qk_hashagg_init")) return rc;
     if (!state || ((uintptr_t)state & 15)) QK_FAIL(QK_ERR_INVALID, "qk_hashagg_init: state must be a 16-byte aligned device buffer");
     State S; carve(desc, state, &S);
-    int64_t nb = (desc->capacity + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_ha_init<<<(unsigned)nb, 256, 0, (cudaStream_t)stream>>>(S, desc->capacity, desc->nagg, *desc);
+    k_ha_init<<<grid_size(desc->capacity, 16), 256, 0, (cudaStream_t)stream>>>(S, desc->capacity, desc->nagg, *desc);
     QK_LAUNCH_CHECK("k_ha_init");
     return QK_OK;
 }
@@ -214,9 +212,7 @@ extern "C" int qk_hashagg_update(const qk_hashagg_desc* desc, void* state, const
     U.nagg = desc->nagg;
     if (nrows == 0) return QK_OK;
     State S; carve(desc, state, &S);
-    int64_t nb = (nrows + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_ha_update<<<(unsigned)nb, 256, 0, (cudaStream_t)stream>>>(S, (uint64_t)desc->capacity - 1, L, U, nrows, overflow);
+    k_ha_update<<<grid_size(nrows, 16), 256, 0, (cudaStream_t)stream>>>(S, (uint64_t)desc->capacity - 1, L, U, nrows, overflow);
     QK_LAUNCH_CHECK("k_ha_update");
     return QK_OK;
 }
@@ -242,9 +238,7 @@ extern "C" int qk_hashagg_finalize(const qk_hashagg_desc* desc, const void* stat
     cudaStream_t st = (cudaStream_t)stream;
     QK_CUDA(cudaMemsetAsync(out_groups, 0, sizeof(int64_t), st));
     State S; carve(desc, (void*)state, &S);
-    int64_t nb = (desc->capacity + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_ha_finalize<<<(unsigned)nb, 256, 0, st>>>(S, desc->capacity, L, F, (long long*)out_cnt, out_capacity, (unsigned long long*)out_groups);
+    k_ha_finalize<<<grid_size(desc->capacity, 16), 256, 0, st>>>(S, desc->capacity, L, F, (long long*)out_cnt, out_capacity, (unsigned long long*)out_groups);
     QK_LAUNCH_CHECK("k_ha_finalize");
     return QK_OK;
 }

@@ -72,12 +72,7 @@ __global__ void __launch_bounds__(256) k_join_probe(const Slot* slots, uint64_t 
             case QK_JOIN_SEMI: emit = matches > 0 ? 1 : 0; break;
             default: emit = (valid && matches == 0) ? 1 : 0; break;
         }
-        // warp inclusive scan of emit
-        int x = emit;
-        for (int o = 1; o < 32; o <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, x, o);
-            if ((int)lane_id() >= o) x += y;
-        }
+        const int x = warp_inclusive_scan(emit);
         const int total = __shfl_sync(0xffffffffu, x, 31);
         if (total == 0) continue;
         unsigned long long base = 0;
@@ -114,9 +109,7 @@ extern "C" size_t qk_join_table_bytes(int64_t capacity) { return capacity > 0 ? 
 extern "C" int qk_join_init(void* table, int64_t capacity, void* stream) {
     if (!table || !pow2(capacity)) QK_FAIL(QK_ERR_INVALID, "qk_join_init: table null or capacity %lld not a power of two", (long long)capacity);
     if (((uintptr_t)table & 15) != 0) QK_FAIL(QK_ERR_INVALID, "qk_join_init: table must be 16-byte aligned");
-    int64_t nb = (capacity + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_join_init<<<(unsigned)nb, 256, 0, (cudaStream_t)stream>>>((Slot*)table, capacity);
+    k_join_init<<<grid_size(capacity, 16), 256, 0, (cudaStream_t)stream>>>((Slot*)table, capacity);
     QK_LAUNCH_CHECK("k_join_init");
     return QK_OK;
 }
@@ -128,9 +121,7 @@ extern "C" int qk_join_build(void* table, int64_t capacity, const qk_column* key
     if (!dtype_is_int(key->dtype)) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: join keys must be integer columns", who);
     if (row_base < 0 || (int64_t)row_base + key->length > 0x7fffffffLL) QK_FAIL(QK_ERR_INVALID, "%s: build row numbers exceed int32", who);
     if (key->length == 0) return QK_OK;
-    int64_t nb = (key->length + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_join_build<<<(unsigned)nb, 256, 0, (cudaStream_t)stream>>>((Slot*)table, (uint64_t)capacity - 1, key->data, key->dtype, key->length, row_base, flags);
+    k_join_build<<<grid_size(key->length, 16), 256, 0, (cudaStream_t)stream>>>((Slot*)table, (uint64_t)capacity - 1, key->data, key->dtype, key->length, row_base, flags);
     QK_LAUNCH_CHECK("k_join_build");
     return QK_OK;
 }
@@ -147,9 +138,7 @@ extern "C" int qk_join_probe(const void* table, int64_t capacity, const qk_colum
     cudaStream_t st = (cudaStream_t)stream;
     QK_CUDA(cudaMemsetAsync(out_count, 0, sizeof(int64_t), st));
     if (key->length == 0) return QK_OK;
-    int64_t nb = (key->length + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_join_probe<<<(unsigned)nb, 256, 0, st>>>((const Slot*)table, (uint64_t)capacity - 1, key->data, key->dtype, key->length, how,
+    k_join_probe<<<grid_size(key->length, 16), 256, 0, st>>>((const Slot*)table, (uint64_t)capacity - 1, key->data, key->dtype, key->length, how,
                                                out_probe_idx, out_build_idx, out_capacity, (unsigned long long*)out_count);
     QK_LAUNCH_CHECK("k_join_probe");
     return QK_OK;

@@ -50,64 +50,6 @@ __global__ void __launch_bounds__(P_NT) k_part_hist(const void* key, int dt, int
     }
 }
 
-// pass 2a: one CTA per partition scans that partition's per-chunk counts (a contiguous row of the partition-major
-// histogram) -> offsets RELATIVE to the partition's start, and the partition's row total.
-__global__ void __launch_bounds__(P_NT) k_part_scan_rows(const unsigned* hist, int64_t nchunks, int64_t* offsets, int64_t* totals) {
-    __shared__ int64_t wtot[P_NT / 32];
-    const int64_t row = (int64_t)blockIdx.x * nchunks;
-    const int warp = threadIdx.x >> 5;
-    int64_t carry = 0;
-    for (int64_t base = 0; base < nchunks; base += P_NT) {
-        const int64_t i = base + threadIdx.x;
-        const int64_t v = i < nchunks ? hist[row + i] : 0;
-        int64_t x = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            const int64_t y = __shfl_up_sync(0xffffffffu, x, o);
-            if ((int)lane_id() >= o) x += y;
-        }
-        if (lane_id() == 31) wtot[warp] = x;
-        __syncthreads();
-        int64_t before = 0, total = 0;
-        for (int w = 0; w < P_NT / 32; ++w) { if (w < warp) before += wtot[w]; total += wtot[w]; }
-        if (i < nchunks) offsets[row + i] = carry + before + x - v;
-        carry += total;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) totals[blockIdx.x] = carry;
-}
-// pass 2b: exclusive scan of the nparts totals (single CTA; nparts <= 16384) -> part_offsets[nparts + 1]
-__global__ void __launch_bounds__(1024) k_part_scan_totals(const int64_t* totals, int nparts, int64_t* part_offsets) {
-    __shared__ int64_t wtot[32];
-    __shared__ int64_t carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (int base = 0; base < nparts; base += 1024) {
-        const int i = base + threadIdx.x;
-        int64_t v = i < nparts ? totals[i] : 0, x = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            int64_t y = __shfl_up_sync(0xffffffffu, x, o);
-            if ((int)lane_id() >= o) x += y;
-        }
-        if (lane_id() == 31) wtot[threadIdx.x >> 5] = x;
-        __syncthreads();
-        if (threadIdx.x < 32) {
-            int64_t w = wtot[threadIdx.x], t = w;
-            for (int o = 1; o < 32; o <<= 1) {
-                int64_t y = __shfl_up_sync(0xffffffffu, t, o);
-                if ((int)lane_id() >= o) t += y;
-            }
-            wtot[threadIdx.x] = t - w;
-        }
-        __syncthreads();
-        const int64_t excl = carry + wtot[threadIdx.x >> 5] + x - v;
-        if (i < nparts) part_offsets[i] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = excl + v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) part_offsets[nparts] = carry;
-}
-
 // pass 3: stable rank of every row inside its chunk -> dest.  Rows are visited in order, one 256-row
 // slab at a time.  Inside a warp the rank among equal partitions comes from match_any + popc (peer
 // ballot); across warps from a per-warp count table in shared memory, so all 8 warps work in parallel
@@ -288,26 +230,20 @@ static int smem_plan(const qk_column* key, int32_t nparts, int32_t mode, int32_t
     unsigned* hist = (unsigned*)workspace;
     int64_t* offsets = (int64_t*)((char*)workspace + align_up((size_t)(nchunks + 1) * nparts * 4, 256));
     int64_t* totals = (int64_t*)((char*)offsets + align_up((size_t)(nchunks + 1) * nparts * 8, 256));
-    const int sms = sm_count();
-    const int64_t nb = nchunks < (int64_t)sms * 8 ? nchunks : (int64_t)sms * 8;
+    const unsigned nb = grid_size(nchunks, 8, 1);                      // grid-stride over the chunks
     const size_t smem = (size_t)nparts * 4;
     QK_CUDA(cudaFuncSetAttribute(k_part_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_part_hist<<<(unsigned)nb, P_NT, smem, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, hist);
+    k_part_hist<<<nb, P_NT, smem, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, hist);
     QK_LAUNCH_CHECK("k_part_hist");
-    k_part_scan_rows<<<(unsigned)nparts, P_NT, 0, st>>>(hist, nchunks, offsets, totals);
-    QK_LAUNCH_CHECK("k_part_scan_rows");
-    k_part_scan_totals<<<1, 1024, 0, st>>>(totals, nparts, part_offsets);
-    QK_LAUNCH_CHECK("k_part_scan_totals");
+    // pass 2: every partition's per-chunk counts (a row of the partition-major histogram) -> offsets relative to the
+    // partition's start and the partition's total; then the totals -> part_offsets[nparts + 1]
+    if (int rc = count_offsets(hist, nparts, nchunks, offsets, totals, st)) return rc;
+    if (int rc = count_offsets(totals, 1, nparts, part_offsets, part_offsets + nparts, st)) return rc;
     const size_t smem_dest = (size_t)nparts * 12;
     QK_CUDA(cudaFuncSetAttribute(k_part_dest, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_dest));
-    k_part_dest<<<(unsigned)nb, P_NT, smem_dest, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, offsets, part_offsets, dest);
+    k_part_dest<<<nb, P_NT, smem_dest, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, offsets, part_offsets, dest);
     QK_LAUNCH_CHECK("k_part_dest");
     return QK_OK;
-}
-
-static unsigned grid_of(int64_t n) {            // grid-stride kernels: 256 threads per block, at most 16 blocks per SM
-    const int64_t nb = (n + 255) / 256, cap = (int64_t)sm_count() * 16;
-    return (unsigned)(nb < 1 ? 1 : (nb > cap ? cap : nb));
 }
 
 // CODE partition with more than P_SMEM_PARTS parts: one stable shared-memory pass per 14-bit digit of the clamped code,
@@ -320,7 +256,7 @@ static int radix_plan(const qk_column* key, int32_t nparts, int32_t* dest, int64
     int32_t* pass_dest = (int32_t*)w; w += col_bytes;
     int32_t* codes[2] = {(int32_t*)w, (int32_t*)(w + col_bytes)}; w += 2 * col_bytes;
     int64_t* pass_offsets = (int64_t*)w; w += align_up((size_t)(P_SMEM_PARTS + 1) * 8, 256);
-    const unsigned grid = grid_of(n);
+    const unsigned grid = grid_size(n, 16);
     const void* src = key->data;
     int src_dt = key->dtype;
     const int passes = radix_passes(nparts);
@@ -336,7 +272,7 @@ static int radix_plan(const qk_column* key, int32_t nparts, int32_t* dest, int64
         QK_LAUNCH_CHECK("k_radix_move");
         src = codes[d & 1]; src_dt = QK_I32;
     }
-    k_radix_offsets<<<grid_of((int64_t)nparts + 1), 256, 0, st>>>((const int32_t*)src, n, nparts, part_offsets);
+    k_radix_offsets<<<grid_size((int64_t)nparts + 1, 16), 256, 0, st>>>((const int32_t*)src, n, nparts, part_offsets);
     QK_LAUNCH_CHECK("k_radix_offsets");
     return QK_OK;
 }
@@ -369,9 +305,7 @@ extern "C" int qk_scatter(const qk_column* cols, int32_t ncols, const int32_t* d
     if (int rc = fill_move(M, cols, ncols, out, n, n, "qk_scatter")) return rc;
     if (n == 0) return QK_OK;
     if (!dest) QK_FAIL(QK_ERR_INVALID, "qk_scatter: null dest");
-    int64_t nb = (n + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_scatter<<<(unsigned)nb, 256, 0, (cudaStream_t)stream>>>(M, dest, n);
+    k_scatter<<<grid_size(n, 16), 256, 0, (cudaStream_t)stream>>>(M, dest, n);
     QK_LAUNCH_CHECK("k_scatter");
     return QK_OK;
 }
@@ -407,21 +341,18 @@ extern "C" int qk_gather(const qk_column* cols, int32_t ncols, const int32_t* id
             continue;
         }
         const int L = row_lanes(&cols[c]);
-        int64_t nb = (n_idx * L + 255) / 256;
-        if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
+        const unsigned nb = grid_size(n_idx * L, 16);
         switch (dtype_size(cols[c].dtype)) {
-            case 1: k_gather_rows<uint8_t><<<(unsigned)nb, 256, 0, st>>>((const uint8_t*)cols[c].data, (uint8_t*)out[c].data, idx, n_idx, L); break;
-            case 2: k_gather_rows<uint16_t><<<(unsigned)nb, 256, 0, st>>>((const uint16_t*)cols[c].data, (uint16_t*)out[c].data, idx, n_idx, L); break;
-            case 4: k_gather_rows<uint32_t><<<(unsigned)nb, 256, 0, st>>>((const uint32_t*)cols[c].data, (uint32_t*)out[c].data, idx, n_idx, L); break;
-            default: k_gather_rows<uint64_t><<<(unsigned)nb, 256, 0, st>>>((const uint64_t*)cols[c].data, (uint64_t*)out[c].data, idx, n_idx, L); break;
+            case 1: k_gather_rows<uint8_t><<<nb, 256, 0, st>>>((const uint8_t*)cols[c].data, (uint8_t*)out[c].data, idx, n_idx, L); break;
+            case 2: k_gather_rows<uint16_t><<<nb, 256, 0, st>>>((const uint16_t*)cols[c].data, (uint16_t*)out[c].data, idx, n_idx, L); break;
+            case 4: k_gather_rows<uint32_t><<<nb, 256, 0, st>>>((const uint32_t*)cols[c].data, (uint32_t*)out[c].data, idx, n_idx, L); break;
+            default: k_gather_rows<uint64_t><<<nb, 256, 0, st>>>((const uint64_t*)cols[c].data, (uint64_t*)out[c].data, idx, n_idx, L); break;
         }
         QK_LAUNCH_CHECK("k_gather_rows");
     }
     if (nscal == 0) return QK_OK;
     if (int rc = fill_move(M, scal_in, nscal, scal_out, -1, n_idx, who)) return rc;
-    int64_t nb = (n_idx + 255) / 256;
-    if (nb > (int64_t)sm_count() * 16) nb = (int64_t)sm_count() * 16;
-    k_gather<<<(unsigned)nb, 256, 0, st>>>(M, idx, n_idx);
+    k_gather<<<grid_size(n_idx, 16), 256, 0, st>>>(M, idx, n_idx);
     QK_LAUNCH_CHECK("k_gather");
     return QK_OK;
 }

@@ -227,57 +227,19 @@ __global__ void __launch_bounds__(256) k_filter_project_unordered(const __grid_c
 
 // stable compaction, pass 1: passing rows per CHUNK
 constexpr int STABLE_CHUNK = 2048;
-__global__ void __launch_bounds__(256) k_filter_count(const __grid_constant__ Programs P, int64_t nrows, int32_t* chunk_counts) {
-    __shared__ int wsum[8];
+__global__ void __launch_bounds__(256) k_filter_count(const __grid_constant__ Programs P, int64_t nrows, uint32_t* chunk_counts) {
+    __shared__ unsigned wsum[8];
     for (int64_t chunk = blockIdx.x; chunk * STABLE_CHUNK < nrows; chunk += gridDim.x) {
-        int cnt = 0;
+        unsigned cnt = 0;
         const int64_t base = chunk * STABLE_CHUNK;
         for (int t = threadIdx.x; t < STABLE_CHUNK; t += 256) {
             const int64_t row = base + t;
             cnt += (row < nrows && eval_pred(P, row)) ? 1 : 0;
         }
-        for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-        if (lane_id() == 0) wsum[threadIdx.x >> 5] = cnt;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            int s = 0;
-            for (int w = 0; w < 8; ++w) s += wsum[w];
-            chunk_counts[chunk] = s;
-        }
+        const unsigned total = cta_sum<256>(cnt, wsum);
+        if (threadIdx.x == 0) chunk_counts[chunk] = total;
         __syncthreads();
     }
-}
-// exclusive scan of chunk counts (single CTA, sequential over 1024-wide tiles), total -> out_rows
-__global__ void __launch_bounds__(1024) k_scan_counts(const int32_t* counts, int64_t n, int64_t* offsets, int64_t* out_rows) {
-    __shared__ int64_t wtot[32];
-    __shared__ int64_t carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (int64_t base = 0; base < n; base += 1024) {
-        const int64_t i = base + threadIdx.x;
-        int64_t v = i < n ? counts[i] : 0, x = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            int64_t y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane_id() >= o) x += y;
-        }
-        if (lane_id() == 31) wtot[threadIdx.x >> 5] = x;
-        __syncthreads();
-        if (threadIdx.x < 32) {
-            int64_t w = wtot[threadIdx.x], s = w;
-            for (int o = 1; o < 32; o <<= 1) {
-                int64_t y = __shfl_up_sync(0xffffffffu, s, o);
-                if (lane_id() >= o) s += y;
-            }
-            wtot[threadIdx.x] = s - w;     // exclusive warp offsets
-        }
-        __syncthreads();
-        const int64_t excl = carry + wtot[threadIdx.x >> 5] + x - v;
-        if (i < n) offsets[i] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = excl + v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *out_rows = carry;
 }
 // stable compaction, pass 2
 __global__ void __launch_bounds__(256) k_filter_project_stable(const __grid_constant__ Programs P, const __grid_constant__ ProjOut O,
@@ -289,16 +251,9 @@ __global__ void __launch_bounds__(256) k_filter_project_stable(const __grid_cons
         for (int t0 = 0; t0 < STABLE_CHUNK; t0 += 256) {
             const int64_t row = base + t0 + threadIdx.x;
             const bool pass = row < nrows && eval_pred(P, row);
-            const unsigned m = __ballot_sync(0xffffffffu, pass);
-            if (lane_id() == 0) wcnt[threadIdx.x >> 5] = __popc(m);
-            __syncthreads();
-            int before = 0, total = 0;
-            for (int w = 0; w < 8; ++w) {
-                const int c = wcnt[w];
-                if (w < (int)(threadIdx.x >> 5)) before += c;
-                total += c;
-            }
-            if (pass) write_proj(P, O, nproj, row, running + before + __popc(m & lanemask_lt()));
+            int total;
+            const int rank = cta_ballot_rank<256>(__ballot_sync(0xffffffffu, pass), wcnt, total);
+            if (pass) write_proj(P, O, nproj, row, running + rank);
             running += total;
             __syncthreads();
         }
@@ -1310,7 +1265,6 @@ static int scan_filter_project_impl(const qk_column* cols, int32_t ncols, int64_
     cudaStream_t st = (cudaStream_t)stream;
     QK_CUDA(cudaMemsetAsync(out_rows, 0, sizeof(int64_t), st));
     if (nrows == 0) return QK_OK;
-    const int sms = sm_count();
     {
         // fast path (stable by construction): integer-range predicate + verbatim columns
         const int rc = try_filter_compact_tma(cols, ncols, nrows, pred, proj, nproj, out, out_rows, workspace, ws_bytes, bloom, st);
@@ -1320,22 +1274,19 @@ static int scan_filter_project_impl(const qk_column* cols, int32_t ncols, int64_
         g_variant = "filter_interpreter"; g_variant_cfg = "nt256";
     }
     if (!stable) {
-        int64_t nb = (nrows + 255) / 256;
-        if (nb > (int64_t)sms * 8) nb = (int64_t)sms * 8;
-        k_filter_project_unordered<<<(unsigned)nb, 256, 0, st>>>(P, O, nproj, nrows, (unsigned long long*)out_rows);
+        k_filter_project_unordered<<<grid_size(nrows, 8), 256, 0, st>>>(P, O, nproj, nrows, (unsigned long long*)out_rows);
         QK_LAUNCH_CHECK("k_filter_project_unordered");
         return QK_OK;
     }
     const int64_t nchunks = (nrows + STABLE_CHUNK - 1) / STABLE_CHUNK;
     if (ws_bytes < qk_scan_workspace_bytes(nrows) || !workspace) QK_FAIL(QK_ERR_CAPACITY, "qk_scan_filter_project: workspace too small (%zu < %zu)", ws_bytes, qk_scan_workspace_bytes(nrows));
-    int32_t* counts = (int32_t*)workspace;
+    uint32_t* counts = (uint32_t*)workspace;
     int64_t* offsets = (int64_t*)((char*)workspace + align_up((size_t)(nchunks + 1) * 4, 256));
-    int64_t nb = nchunks < (int64_t)sms * 8 ? nchunks : (int64_t)sms * 8;
-    k_filter_count<<<(unsigned)nb, 256, 0, st>>>(P, nrows, counts);
+    const unsigned nb = grid_size(nchunks, 8, 1);                      // grid-stride over the chunks
+    k_filter_count<<<nb, 256, 0, st>>>(P, nrows, counts);
     QK_LAUNCH_CHECK("k_filter_count");
-    k_scan_counts<<<1, 1024, 0, st>>>(counts, nchunks, offsets, out_rows);
-    QK_LAUNCH_CHECK("k_scan_counts");
-    k_filter_project_stable<<<(unsigned)nb, 256, 0, st>>>(P, O, nproj, nrows, offsets);
+    if (int rc = count_offsets(counts, 1, nchunks, offsets, out_rows, st)) return rc;
+    k_filter_project_stable<<<nb, 256, 0, st>>>(P, O, nproj, nrows, offsets);
     QK_LAUNCH_CHECK("k_filter_project_stable");
     return QK_OK;
 }
@@ -1403,13 +1354,10 @@ extern "C" int qk_scan_filter_agg_dense(const qk_column* cols, int32_t ncols, in
         const size_t smem = (size_t)ng * (nagg * 8 + 4) * GEN_NT;
         if (smem > 200 * 1024) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: %lld groups x %d aggregates exceed the shared-memory dense path; use the hash aggregate", who, (long long)ng, nagg);
         QK_CUDA(cudaFuncSetAttribute(k_dense_agg_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const int sms = sm_count();
         int per_sm = (int)((220 * 1024) / (smem + 1024));
         if (per_sm < 1) per_sm = 1;
         if (per_sm > 4) per_sm = 4;
-        int64_t nb = (nrows + GEN_NT - 1) / GEN_NT;
-        if (nb > (int64_t)sms * per_sm) nb = (int64_t)sms * per_sm;
-        nblocks = (int)nb;
+        nblocks = (int)grid_size(nrows, per_sm, GEN_NT);
         k_dense_agg_generic<<<nblocks, GEN_NT, smem, st>>>(P, A, nrows, part_acc, part_cnt);
         QK_LAUNCH_CHECK("k_dense_agg_generic");
         g_variant = "generic"; g_variant_cfg = "nt256";

@@ -152,10 +152,7 @@ extern "C" int qk_synth_column(int32_t table, int32_t column, const int64_t* siz
     Sizes sz{sizes[0], sizes[1], sizes[2], sizes[3], sizes[4], sizes[5]};
     if (sz.n_orders <= 0 || sz.n_customer <= 0 || sz.n_supplier <= 0 || sz.n_part <= 0)
         QK_FAIL(QK_ERR_INVALID, "qk_synth_column: sizes must be positive");
-    int64_t blocks = (nrows + 255) / 256;
-    int64_t cap = (int64_t)sm_count() * 32;
-    if (blocks > cap) blocks = cap;
-    k_synth<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(table, column, sz, row_lo, nrows, out);
+    k_synth<<<grid_size(nrows, 32), 256, 0, (cudaStream_t)stream>>>(table, column, sz, row_lo, nrows, out);
     QK_LAUNCH_CHECK("k_synth");
     return QK_OK;
 }

@@ -111,22 +111,21 @@ extern "C" int qk_topk_candidates(const qk_column* key, int32_t k, int32_t desce
     if (!workspace || ws_bytes < qk_topk_workspace_bytes(n)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
     unsigned long long* img = (unsigned long long*)workspace;
     SelState* S = (SelState*)((char*)workspace + align_up((size_t)n * 8, 256));
-    int64_t nb = (n + 255) / 256;
-    if (nb > (int64_t)sm_count() * 8) nb = (int64_t)sm_count() * 8;
-    k_topk_image<<<(unsigned)nb, 256, 0, st>>>(key->data, key->dtype, n, descending, img);
+    const unsigned nb = grid_size(n, 8);
+    k_topk_image<<<nb, 256, 0, st>>>(key->data, key->dtype, n, descending, img);
     QK_LAUNCH_CHECK("k_topk_image");
     const int take_all = n <= k;
     if (!take_all) {
         k_topk_reset<<<1, 256, 0, st>>>(S, k);
         QK_LAUNCH_CHECK("k_topk_reset");
         for (int pass = 0; pass < 8; ++pass) {
-            k_topk_hist<<<(unsigned)nb, 256, 0, st>>>(img, n, pass, S);
+            k_topk_hist<<<nb, 256, 0, st>>>(img, n, pass, S);
             QK_LAUNCH_CHECK("k_topk_hist");
             k_topk_pick<<<1, 256, 0, st>>>(S);
             QK_LAUNCH_CHECK("k_topk_pick");
         }
     }
-    k_topk_emit<<<(unsigned)nb, 256, 0, st>>>(img, n, S, take_all, out_idx, (unsigned long long*)out_n);
+    k_topk_emit<<<nb, 256, 0, st>>>(img, n, S, take_all, out_idx, (unsigned long long*)out_n);
     QK_LAUNCH_CHECK("k_topk_emit");
     return QK_OK;
 }

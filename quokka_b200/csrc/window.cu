@@ -86,55 +86,26 @@ __global__ void __launch_bounds__(256) k_win_session_flag(const long long* time,
         flag[i] = (i == 0 || by[i] != by[i - 1] || time[i] - time[i - 1] > timeout) ? 1 : 0;
 }
 
-// inclusive prefix sum int32 -> int64: per-block sums, one block scans them, every block adds its offset
+// inclusive prefix sum int32 -> int64: per-block sums, count_offsets turns them into block offsets, every block adds its offset
 constexpr int S_NT = 256, S_PER = 8, S_TILE = S_NT * S_PER;
-__global__ void __launch_bounds__(S_NT) k_scan_block_sums(const int32_t* in, int64_t n, long long* sums) {
-    __shared__ long long w[S_NT / 32];
+__global__ void __launch_bounds__(S_NT) k_scan_block_sums(const int32_t* in, int64_t n, int64_t* sums) {
+    __shared__ int64_t w[S_NT / 32];
     const int64_t base = (int64_t)blockIdx.x * S_TILE;
-    long long s = 0;
+    int64_t s = 0;
     for (int j = 0; j < S_PER; ++j) { const int64_t i = base + j * S_NT + threadIdx.x; s += i < n ? in[i] : 0; }
-    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane_id() == 0) w[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) { long long t = 0; for (int k = 0; k < S_NT / 32; ++k) t += w[k]; sums[blockIdx.x] = t; }
+    const int64_t total = cta_sum<S_NT>(s, w);
+    if (threadIdx.x == 0) sums[blockIdx.x] = total;
 }
-__global__ void __launch_bounds__(1024) k_scan_sums(long long* sums, int64_t nb) {      // exclusive, in place, single CTA
-    __shared__ long long wtot[32];
-    __shared__ long long carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (int64_t base = 0; base < nb; base += 1024) {
-        const int64_t i = base + threadIdx.x;
-        long long v = i < nb ? sums[i] : 0, x = v;
-        for (int o = 1; o < 32; o <<= 1) { const long long y = __shfl_up_sync(0xffffffffu, x, o); if ((int)lane_id() >= o) x += y; }
-        if (lane_id() == 31) wtot[threadIdx.x >> 5] = x;
-        __syncthreads();
-        if (threadIdx.x < 32) {
-            long long ww = wtot[threadIdx.x], t = ww;
-            for (int o = 1; o < 32; o <<= 1) { const long long y = __shfl_up_sync(0xffffffffu, t, o); if ((int)lane_id() >= o) t += y; }
-            wtot[threadIdx.x] = t - ww;
-        }
-        __syncthreads();
-        const long long excl = carry + wtot[threadIdx.x >> 5] + x - v;
-        if (i < nb) sums[i] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = excl + v;
-        __syncthreads();
-    }
-}
-__global__ void __launch_bounds__(S_NT) k_scan_apply(const int32_t* in, int64_t n, const long long* sums, long long* out) {
-    __shared__ long long wtot[S_NT / 32];
+__global__ void __launch_bounds__(S_NT) k_scan_apply(const int32_t* in, int64_t n, const int64_t* offsets, long long* out) {
+    __shared__ int64_t wtot[S_NT / 32];
     const int64_t base = (int64_t)blockIdx.x * S_TILE;
-    long long run = sums[blockIdx.x];
+    int64_t run = offsets[blockIdx.x];
     for (int j = 0; j < S_PER; ++j) {
         const int64_t i = base + j * S_NT + threadIdx.x;
-        long long v = i < n ? in[i] : 0, x = v;
-        for (int o = 1; o < 32; o <<= 1) { const long long y = __shfl_up_sync(0xffffffffu, x, o); if ((int)lane_id() >= o) x += y; }
-        if (lane_id() == 31) wtot[threadIdx.x >> 5] = x;
-        __syncthreads();
-        long long before = 0, total = 0;
-        for (int k = 0; k < S_NT / 32; ++k) { if (k < (int)(threadIdx.x >> 5)) before += wtot[k]; total += wtot[k]; }
-        if (i < n) out[i] = run + before + x;
+        const int64_t v = i < n ? in[i] : 0;
+        int64_t total;
+        const int64_t before = cta_exclusive_scan<S_NT>(v, wtot, total);
+        if (i < n) out[i] = run + before + v;
         run += total;
         __syncthreads();
     }
@@ -144,12 +115,6 @@ __global__ void __launch_bounds__(S_NT) k_scan_apply(const int32_t* in, int64_t 
 }  // namespace qk
 
 using namespace qk;
-
-static int grid_for(int64_t n) {
-    int64_t nb = (n + 255) / 256;
-    const int64_t cap = (int64_t)sm_count() * 16;
-    return (int)(nb < 1 ? 1 : (nb > cap ? cap : nb));
-}
 
 static int check_ts(const qk_column* time, const qk_column* by, const char* who) {
     if (int rc = check_col(time, who)) return rc;
@@ -182,7 +147,7 @@ extern "C" int qk_window_sliding(const qk_column* time, const qk_column* by, con
     }
     W.nout = nout;
     if (n == 0) return QK_OK;
-    k_win_sliding<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>((const long long*)time->data, (const int32_t*)by->data, seg, n_by, n, size, W);
+    k_win_sliding<<<grid_size(n, 16), 256, 0, (cudaStream_t)stream>>>((const long long*)time->data, (const int32_t*)by->data, seg, n_by, n, size, W);
     QK_LAUNCH_CHECK("k_win_sliding");
     return QK_OK;
 }
@@ -196,7 +161,7 @@ extern "C" int qk_window_hop_expand(const qk_column* time, const qk_column* by, 
     if (n * slots > 0x7fffffffLL) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: %lld rows x %d windows exceed int32 row numbers; feed smaller batches", who, (long long)n, slots);
     if (n == 0) return QK_OK;
     if (!wstart || !key || !src) QK_FAIL(QK_ERR_INVALID, "%s: null outputs", who);
-    k_win_hop_expand<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>((const long long*)time->data, (const int32_t*)by->data, seg, n_by, n, size, hop,
+    k_win_hop_expand<<<grid_size(n, 16), 256, 0, (cudaStream_t)stream>>>((const long long*)time->data, (const int32_t*)by->data, seg, n_by, n, size, hop,
                                                                      slots, (long long*)wstart, key, src);
     QK_LAUNCH_CHECK("k_win_hop_expand");
     return QK_OK;
@@ -216,15 +181,14 @@ extern "C" int qk_window_session_ids(const qk_column* time, const qk_column* by,
     if (n == 0) return QK_OK;
     if (!ids || !workspace || ws_bytes < qk_window_session_workspace_bytes(n)) QK_FAIL(QK_ERR_CAPACITY, "%s: null output / workspace too small", who);
     int32_t* flag = (int32_t*)workspace;
-    long long* sums = (long long*)((char*)workspace + align_up((size_t)n * 4, 256));
+    int64_t* sums = (int64_t*)((char*)workspace + align_up((size_t)n * 4, 256));    // nb + 1: offsets, then the total
     cudaStream_t st = (cudaStream_t)stream;
-    k_win_session_flag<<<grid_for(n), 256, 0, st>>>((const long long*)time->data, (const int32_t*)by->data, n, timeout, flag);
+    k_win_session_flag<<<grid_size(n, 16), 256, 0, st>>>((const long long*)time->data, (const int32_t*)by->data, n, timeout, flag);
     QK_LAUNCH_CHECK("k_win_session_flag");
     const int64_t nb = (n + S_TILE - 1) / S_TILE;
     k_scan_block_sums<<<(unsigned)nb, S_NT, 0, st>>>(flag, n, sums);
     QK_LAUNCH_CHECK("k_scan_block_sums");
-    k_scan_sums<<<1, 1024, 0, st>>>(sums, nb);
-    QK_LAUNCH_CHECK("k_scan_sums");
+    if (int rc = count_offsets(sums, 1, nb, sums, sums + nb, st)) return rc;      // in place
     k_scan_apply<<<(unsigned)nb, S_NT, 0, st>>>(flag, n, sums, (long long*)ids);
     QK_LAUNCH_CHECK("k_scan_apply");
     return QK_OK;

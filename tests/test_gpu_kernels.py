@@ -346,7 +346,8 @@ def test_hash_aggregate(qb, n, card):
 
 
 # ------------------------------------------------------------------ K3 partition + scatter
-@pytest.mark.parametrize("n,nparts", [(0, 8), (1, 8), (4097, 2), (100_000, 8), (100_000, 7), (50_000, 1000)])
+@pytest.mark.parametrize("n,nparts", [(0, 8), (1, 8), (4097, 2), (100_000, 8), (100_000, 7), (50_000, 1000),
+                                      (1024 * 4096 + 1, 3)])          # 1025 chunks of 4096 rows: one carry of the count scan
 def test_partition_matches_key_mod_n_and_is_stable(qb, n, nparts):
     rng = np.random.default_rng(1)
     key = rng.integers(0, 10_000_000, n).astype(np.int64)

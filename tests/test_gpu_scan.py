@@ -1,12 +1,12 @@
 """Every device path of qk_scan_filter_project against the exact reference of tests/scan_cases.py:
-- the stable interpreter (k_filter_count -> k_scan_counts -> k_filter_project_stable): bit-exact, in input order;
+- the stable interpreter (k_filter_count -> k_count_offsets -> k_filter_project_stable): bit-exact, in input order;
 - the unordered interpreter (k_filter_project_unordered): the same multiset of rows;
 - the TMA compaction (csrc/compact.cu, "compact_tma"), reached by an integer compare / range (or no predicate) and 1-8
   verbatim 16-byte aligned columns: bit-exact, in input order;
 - its fall-backs to the interpreter: a misaligned view (t[1:]), more than 8 columns, an expression projection;
 - the Bloom-reduced compaction (qk_scan_filter_project_sj, "compact_tma+bloom"): no false negatives, survivors in order.
 After every call with rows the test asserts which kernel ran.  Sizes cover the warp, CTA, chunk (2048 rows) and TMA tile
-edges, two carries of k_scan_counts' 1024-chunk tiles (4 300 000 rows), and 2^31 - 1 rows of uint8 (the largest call)."""
+edges, two carries of k_count_offsets' 1024-chunk tiles (4 300 000 rows), and 2^31 - 1 rows of uint8 (the largest call)."""
 import functools
 
 import numpy as np
