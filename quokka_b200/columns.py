@@ -16,6 +16,7 @@ import numpy as np
 import pyarrow as pa
 import pyarrow.compute as pc
 import torch
+import torch.distributed as dist
 
 from . import _lib as L
 from . import ops
@@ -30,6 +31,15 @@ def _default_device():
 
 def default_device():
     return _default_device()
+
+
+def world_size() -> int:
+    """How many ranks (one process per GPU) there are: the one definition, here because every module imports this one."""
+    return dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+
+
+def rank() -> int:
+    return dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
 
 
 @dataclass

@@ -16,7 +16,7 @@ from . import expr as E
 from . import ops
 # host arithmetic, the same whichever kernel backend `ops` names: imported by name, not looked up through `ops`
 from .ops import dense_agg_fits
-from .columns import DeviceColumn, DeviceTable
+from .columns import DeviceColumn, DeviceTable, world_size
 from .target_info import (BroadcastPartitioner, FunctionPartitioner, HashPartitioner, PassThroughPartitioner,
                           RangePartitioner)
 
@@ -237,11 +237,6 @@ def drop_null_predicate_rows(t: DeviceTable, pred) -> DeviceTable:
 _AGG_OPS = {"sum": L.AGG_SUM, "min": L.AGG_MIN, "max": L.AGG_MAX}
 
 
-def _single_process() -> bool:
-    import torch.distributed as dist
-    return not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1)
-
-
 def to_f64(t: torch.Tensor) -> torch.Tensor:
     """An integer / float32 column as fp64 (one pass of the scan kernel: column + 0.0)."""
     if t.dtype == torch.float64:
@@ -267,6 +262,16 @@ def restore_type(v: torch.Tensor, rt) -> DeviceColumn:
     if rt is None or v.dtype != torch.float64:
         return DeviceColumn(v)
     return DeviceColumn(torch.round(v).to(rt[0]), None, rt[1])
+
+
+def keyless_aggregate(state, vals: list, agg_ops: list, n: int, device, variant: int = 0):
+    """Folds the fp64 columns `vals` (one per aggregate of `agg_ops`, sum|min|max) of `n` rows into the empty-grouping dense
+    state `state` (None: a new one) and returns it.  Without a value (count(*) only) a zero column carries the row count."""
+    if state is None:
+        state = ops.DenseAggState([], [_AGG_OPS[op] for op in agg_ops], device)
+    cols_in = vals or [torch.zeros(n, dtype=torch.uint8, device=device)]
+    state.update(cols_in, None, [], [[(L.OP_COL, i, 0, 0.0, 0)] for i in range(len(vals))], variant=variant)
+    return state
 
 
 class PartialAgg:
@@ -307,7 +312,7 @@ class PartialAgg:
         value_aggs = [(op, e, name) for op, e, name in vals if op != "count"]
         if dense and dense_agg_fits(n_groups, len(value_aggs)):
             return self._dense(t, edge, key_exprs, vals, value_aggs, n_groups)
-        if key_exprs and _single_process():
+        if key_exprs and world_size() == 1:
             return self._rows(t, edge, key_exprs, vals, value_aggs)
         return self._hashed(t, edge, key_exprs, vals, value_aggs)
 
@@ -434,9 +439,7 @@ class PartialAgg:
                 raise L.QkError(f"group key {k!r} must be an integer / date / dictionary column (got {kc.data.dtype})")
         self.last_path = "hash"
         if not keys:
-            st = ops.DenseAggState([], [_AGG_OPS[op] for op, _, _ in value_aggs], t.device)
-            cols_in = fvals or [torch.zeros(len(s), dtype=torch.uint8, device=s.device)]
-            st.update(cols_in, None, [], [[(L.OP_COL, i, 0, 0.0, 0)] for i in range(len(value_aggs))])
+            st = keyless_aggregate(None, fvals, [op for op, _, _ in value_aggs], len(s), s.device)
             out, j = {}, 0
             for op, e, name in vals:
                 if op == "count":

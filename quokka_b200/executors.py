@@ -20,8 +20,8 @@ import torch
 from . import _lib as L
 from . import expr as E
 from . import ops
-from .columns import DeviceColumn, DeviceTable, as_device_table, concat_tables, default_device, unify_dictionaries
-from .edge import EdgeOps, agg_result_type, restore_type, to_f64
+from .columns import DeviceColumn, DeviceTable, as_device_table, concat_tables, default_device, unify_dictionaries, world_size
+from .edge import EdgeOps, agg_result_type, keyless_aggregate, restore_type, to_f64
 
 
 class Executor:
@@ -35,14 +35,6 @@ class Executor:
 
     def done(self, executor_id):
         raise NotImplementedError
-
-
-def _retire(state):
-    """A state buffer replaced while chunks are in flight on several lanes: it may have been allocated on another lane's
-    stream, so the allocator must not hand it out again before the kernels queued on THIS stream have read it."""
-    for t in (getattr(state, "state", None), getattr(state, "overflow", None)):
-        if isinstance(t, torch.Tensor) and t.is_cuda:
-            t.record_stream(torch.cuda.current_stream())
 
 
 def _clean(batches, dictionaries=None):
@@ -110,7 +102,6 @@ class OutputExecutor(Executor):
         self.num = 0
 
     def execute(self, batches, stream_id, executor_id):
-        import os
         batches = _clean(batches)
         if not batches:
             return
@@ -180,17 +171,10 @@ class HostTransformExecutor(Executor):
 _HOW = {"inner": L.JOIN_INNER, "left": L.JOIN_LEFT, "semi": L.JOIN_SEMI, "anti": L.JOIN_ANTI}
 
 
-def _join_output(probe: DeviceTable, build: DeviceTable | None, pi, bi, left_on, right_on, how, suffix):
-    out = probe.gather(pi)
-    if how in ("semi", "anti") or build is None:
-        return out
-    right = build.drop([right_on]).gather(bi)
-    valid = None
-    if how == "left":
-        valid = (bi >= 0).to(torch.uint8)
-        right = right.with_validity(valid)
-    cols = dict(out.columns)
-    for n, c in right.columns.items():
+def _append_right(left: DeviceTable, right: dict, suffix: str) -> DeviceTable:
+    """The left side's columns followed by the right side's; a right column whose name is already taken gets `suffix`."""
+    cols = dict(left.columns)
+    for n, c in right.items():
         cols[n + suffix if n in cols else n] = c
     return DeviceTable(cols)
 
@@ -220,23 +204,38 @@ def _float_key(t: torch.Tensor) -> torch.Tensor:
     return (t + 0.0).view(torch.int64) if t.dtype == torch.float64 else t
 
 
-def _world() -> int:
-    import torch.distributed as dist
-    return dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+class _HashedBuild:
+    """The build side of a hash join, hashed once on its key column `on`, and the probe against it: what the shuffled and
+    the broadcast join share."""
 
+    def __init__(self, table: DeviceTable, on: str):
+        key = table[on]
+        if key.data.dtype not in (torch.uint8, torch.int32, torch.int64, torch.float64):
+            raise L.QkError(f"join key {on!r} must be an integer / date / fp64 column (got {key.data.dtype})")
+        self.table, self.on = table, on
+        self.hashed = ops.JoinTable(len(table), key.data.device)
+        self.hashed.build(key.data.to(torch.int32) if key.dictionary is not None else _float_key(key.data))
+        self.hashed.check_flags()
 
-def _build_key(build_col: DeviceColumn) -> torch.Tensor:
-    return build_col.data.to(torch.int32) if build_col.dictionary is not None else _float_key(build_col.data)
+    def probe(self, batch: DeviceTable, probe_on: str, how: str, suffix: str) -> DeviceTable:
+        key = _probe_key(batch[probe_on], self.table[self.on], f"join {probe_on} = {self.on}")
+        pi, bi = self.hashed.probe(key, _HOW[how])
+        out = batch.gather(pi)
+        if how in ("semi", "anti"):
+            return out
+        right = self.table.drop([self.on]).gather(bi)
+        if how == "left":
+            right = right.with_validity((bi >= 0).to(torch.uint8))
+        return _append_right(out, right.columns, suffix)
 
 
 class BuildProbeJoinExecutor(Executor):
-    silent_streams = (1,)        # build batches never produce output: nothing to push downstream after them
-
     """sql_executors.py:325-377.  stream 1 = build (right), stream 0 = probe (left); every build batch
     must arrive before the first probe batch (assert, :357); how in inner/left/semi/anti; the result
     keeps the left key (renamed to the right key when key_to_keep == "right", :372-373); an anti join
     against an empty build side passes the probe through, the others emit nothing (:362-366)."""
 
+    silent_streams = (1,)        # build batches never produce output: nothing to push downstream after them
     emits_on_done = False        # done() returns nothing: the runtime skips the (empty) exchange after it
 
     def __init__(self, on=None, left_on=None, right_on=None, how="inner", key_to_keep="left"):
@@ -255,7 +254,7 @@ class BuildProbeJoinExecutor(Executor):
         self.key_to_keep = key_to_keep
         self.things_seen = []
         self._pending = []          # build batches, hashed once at the first probe
-        self._table = None
+        self._build = None
 
     def build_rows(self) -> int:
         return sum(len(b) for b in self._pending) + (len(self.state) if self.state is not None else 0)
@@ -273,16 +272,11 @@ class BuildProbeJoinExecutor(Executor):
         return all(c.dictionary is None and c.data.dtype != torch.float64 for c in cols)
 
     def _freeze_build(self):
-        if self._table is not None:
+        if self._build is not None:
             return
         self.state = concat_tables(self._pending)
         self._pending = []
-        key = self.state[self.right_on].data
-        if key.dtype not in (torch.uint8, torch.int32, torch.int64, torch.float64):
-            raise L.QkError(f"join key {self.right_on!r} must be an integer / date / fp64 column (got {key.dtype})")
-        self._table = ops.JoinTable(len(self.state), key.device)
-        self._table.build(_build_key(self.state[self.right_on]))
-        self._table.check_flags()
+        self._build = _HashedBuild(self.state, self.right_on)
 
     def execute(self, batches, stream_id, executor_id):
         batches = _clean(batches)
@@ -301,9 +295,7 @@ class BuildProbeJoinExecutor(Executor):
             if self.phase == "build":
                 self._freeze_build()
             self.phase = "probe"
-            key = _probe_key(batch[self.left_on], self.state[self.right_on], f"join {self.left_on} = {self.right_on}")
-            pi, bi = self._table.probe(key, _HOW[self.how])
-            result = _join_output(batch, self.state, pi, bi, self.left_on, self.right_on, self.how, "_right")
+            result = self._build.probe(batch, self.left_on, self.how, "_right")
             if self.key_to_keep == "right":
                 result = result.rename({self.left_on: self.right_on})
             return result
@@ -333,21 +325,17 @@ class BroadcastJoinExecutor(Executor):
             self.big_on = big_on
         names = small_table.column_names if hasattr(small_table, "column_names") else list(small_table.columns)
         assert self.small_on in names
-        self._table = None
+        self._build = None
 
     def execute(self, batches, stream_id, executor_id):
         batches = _clean(batches)
         if len(batches) == 0:
             return
         batch = concat_tables(batches)
-        if self._table is None:                         # opened lazily on first execute (tutorial.md:56)
+        if self._build is None:                         # opened lazily on first execute (tutorial.md:56)
             self.state = as_device_table(self._small_src)
-            self._table = ops.JoinTable(len(self.state), batch.device)
-            self._table.build(_build_key(self.state[self.small_on]))
-            self._table.check_flags()
-        key = _probe_key(batch[self.big_on], self.state[self.small_on], f"join {self.big_on} = {self.small_on}")
-        pi, bi = self._table.probe(key, _HOW[self.how])
-        return _join_output(batch, self.state, pi, bi, self.big_on, self.small_on, self.how, self.suffix)
+            self._build = _HashedBuild(self.state, self.small_on)
+        return self._build.probe(batch, self.big_on, self.how, self.suffix)
 
     def done(self, executor_id):
         return
@@ -357,8 +345,34 @@ class BroadcastJoinExecutor(Executor):
 _AGG_OPS = {"sum": L.AGG_SUM, "min": L.AGG_MIN, "max": L.AGG_MAX}
 
 
-def _to_f64(col: DeviceColumn) -> torch.Tensor:
-    return to_f64(col.data)
+class _GrowingHashAgg:
+    """The hash-aggregate state of a streaming executor.  `state` is created on the first batch with
+    max(1 << 16, first_factor * rows) slots; when a batch would push the load past 1/2, the groups are re-inserted into a
+    larger table first (SUM / MIN / MAX are all re-foldable)."""
+
+    def __init__(self, agg_ops: list, first_factor: int):
+        self.agg_ops, self.first_factor, self.state = agg_ops, first_factor, None
+
+    def update(self, keys: list, vals: list):
+        n = keys[0].numel()
+        if self.state is None:
+            self.state = ops.HashAggState([k.dtype for k in keys], self.agg_ops, max(1 << 16, self.first_factor * n), keys[0].device)
+        elif self.state.rows_seen + n > self.state.capacity // 2:
+            self._grow(n)
+        self.state.update(keys, vals)
+
+    def _grow(self, incoming: int):
+        old = self.state
+        ok, ov, _ = old.finalize()
+        self.state = ops.HashAggState(old.key_dtypes, self.agg_ops, max(4 * (len(ok[0]) + incoming), 2 * old.capacity), old.device)
+        if len(ok[0]):
+            self.state.update(ok, ov)
+        self.state.rows_seen = len(ok[0])
+        # the replaced buffers may have been allocated on another lane's stream while chunks are in flight on several: the
+        # allocator must not hand them out again before the kernels queued on THIS stream have read them
+        for t in (getattr(old, "state", None), getattr(old, "overflow", None)):
+            if isinstance(t, torch.Tensor) and t.is_cuda:
+                t.record_stream(torch.cuda.current_stream())
 
 
 class SQLAggExecutor(Executor):
@@ -395,7 +409,7 @@ class SQLAggExecutor(Executor):
         for e, alias in self.final:
             collect(e)
         self.state = None
-        self._ha = None
+        self._ha = _GrowingHashAgg([_AGG_OPS[f] for f, _ in self.calls], first_factor=2)
         self._dense = None
         self._key_meta = None
         self._types = None          # per call: (torch dtype, arrow type) of an integer / date result, None = fp64
@@ -408,12 +422,9 @@ class SQLAggExecutor(Executor):
         if self._types is None:
             # integer partials (COUNT, integer SUM / MIN / MAX, dates) give integer results, like the reference's engines
             self._types = [agg_result_type(f, batch[c]) for f, c in self.calls]
-        vals = [_to_f64(batch[c]) for _, c in self.calls]
+        vals = [to_f64(batch[c].data) for _, c in self.calls]
         if not self.groupby_keys:
-            if self._dense is None:
-                self._dense = ops.DenseAggState([], [_AGG_OPS[f] for f, _ in self.calls], batch.device)
-            cols_in = vals or [torch.zeros(len(batch), dtype=torch.uint8, device=batch.device)]
-            self._dense.update(cols_in, None, [], [[(L.OP_COL, i, 0, 0.0, 0)] for i in range(len(vals))], variant=1)
+            self._dense = keyless_aggregate(self._dense, vals, [f for f, _ in self.calls], len(batch), batch.device, variant=1)
             return
         keys = [batch[k] for k in self.groupby_keys]
         if self._key_meta is not None:
@@ -429,26 +440,10 @@ class SQLAggExecutor(Executor):
             keys = fixed
         else:
             self._key_meta = [(k.dictionary, k.arrow_type) for k in keys]
-        if self._ha is None:
-            self._ha = ops.HashAggState([k.data.dtype for k in keys], [_AGG_OPS[f] for f, _ in self.calls],
-                                        max(1 << 16, 2 * len(batch)), batch.device)
-        elif self._ha.rows_seen + len(batch) > self._ha.capacity // 2:
-            self._grow(len(batch))
         self._ha.update([k.data for k in keys], vals)
 
-    def _grow(self, incoming):
-        """Re-insert the current groups into a table twice as large (SUM/MIN/MAX are all re-foldable)."""
-        ok, ov, oc = self._ha.finalize()
-        new = ops.HashAggState(self._ha.key_dtypes, [_AGG_OPS[f] for f, _ in self.calls],
-                               max(4 * (len(ok[0]) + incoming), 2 * self._ha.capacity), self._ha.device)
-        if len(ok[0]):
-            new.update(ok, ov)
-        new.rows_seen = len(ok[0])
-        _retire(self._ha)
-        self._ha = new
-
     def done(self, executor_id):
-        if self._ha is None and self._dense is None:
+        if self._ha.state is None and self._dense is None:
             return None
         if self._dense is not None:
             acc = self._dense.acc
@@ -456,7 +451,7 @@ class SQLAggExecutor(Executor):
             if not cols:
                 cols = {"__n": DeviceColumn(self._dense.cnt.to(torch.float64))}
         else:
-            ok, ov, _ = self._ha.finalize()
+            ok, ov, _ = self._ha.state.finalize()
             cols = {k: DeviceColumn(o, m[0], m[1]) for k, o, m in zip(self.groupby_keys, ok, self._key_meta)}
             cols.update({f"__a{i}": restore_type(v, self._types[i]) for i, v in enumerate(ov)})
         t = DeviceTable(cols)
@@ -584,7 +579,7 @@ class DistinctExecutor(Executor):
     def __init__(self, keys) -> None:
         self.keys = keys
         self.state = None
-        self._ha = None
+        self._ha = _GrowingHashAgg([], first_factor=4)
         self._meta = None
 
     def execute(self, batches, stream_id, executor_id):
@@ -593,23 +588,14 @@ class DistinctExecutor(Executor):
             return
         batch = concat_tables(batches)
         keys = [batch[k] for k in self.keys]
-        if self._ha is None:
+        if self._meta is None:
             self._meta = [(k.dictionary, k.arrow_type) for k in keys]
-            self._ha = ops.HashAggState([k.data.dtype for k in keys], [], max(1 << 16, 4 * len(batch)), batch.device)
-        elif self._ha.rows_seen + len(batch) > self._ha.capacity // 2:
-            ok, _, _ = self._ha.finalize()
-            new = ops.HashAggState(self._ha.key_dtypes, [], max(4 * (len(ok[0]) + len(batch)), 2 * self._ha.capacity), batch.device)
-            if len(ok[0]):
-                new.update(ok, [])
-            new.rows_seen = len(ok[0])
-            _retire(self._ha)
-            self._ha = new
         self._ha.update([k.data for k in keys], [])
 
     def done(self, executor_id):
-        if self._ha is None:
+        if self._ha.state is None:
             return
-        ok, _, _ = self._ha.finalize()
+        ok, _, _ = self._ha.state.finalize()
         self.state = DeviceTable({k: DeviceColumn(o, m[0], m[1]) for k, o, m in zip(self.keys, ok, self._meta)})
         return self.state
 
@@ -889,6 +875,88 @@ class KnnFinalExecutor(Executor):
         return self.state
 
 
+# ---------------------------------------------------------------------------------------------- ordered streams
+class KeyCodes:
+    """An append-only code space for the `by` column of ordered streams: codes that mean the same key in every batch of
+    every stream that goes through one KeyCodes (batch dictionaries are re-sorted unions and differ from batch to batch).
+    Strings are numbered in order of first appearance, integer codes are used as is."""
+
+    def __init__(self) -> None:
+        self.values, self.index, self.luts = None, None, {}        # strings: values by code, code by value, table per dictionary
+        self.n_by = 0                                              # codes handed out so far are below this
+
+    def codes(self, col: DeviceColumn) -> torch.Tensor:
+        if col.dictionary is not None:
+            if self.values is None:
+                if self.n_by:
+                    raise L.QkError("as-of `by` columns must both be strings or both be integer codes")
+                self.values, self.index = [], {}
+            key = (id(col.dictionary), len(col.dictionary))
+            lut = self.luts.get(key)
+            if lut is None:
+                codes = []
+                for v in col.dictionary:
+                    i = self.index.get(v)
+                    if i is None:
+                        i = self.index[v] = len(self.values)
+                        self.values.append(v)
+                    codes.append(i)
+                lut = (col.dictionary, torch.tensor(codes or [0], dtype=torch.int32, device=col.data.device))
+                self.luts[key] = lut                                # keeps the dictionary alive, so its id stays unique
+            self.n_by = max(self.n_by, len(self.values))
+            return lut[1][col.data.long()]
+        if self.values is not None:
+            raise L.QkError("as-of `by` columns must both be strings or both be integer codes")
+        codes = col.data.to(torch.int32)
+        if len(codes):
+            lo, hi = (int(v) for v in torch.stack(torch.aminmax(codes)).tolist())       # one pass, one read-back
+            if lo < 0:
+                raise L.QkError("as-of `by` codes must be non-negative")
+            self.n_by = max(self.n_by, hi + 1)
+        return codes
+
+    def column(self, codes: torch.Tensor, bycol: DeviceColumn) -> DeviceColumn:
+        """`codes` as a column of the type `bycol` came in."""
+        if self.values is not None:
+            return DeviceColumn(codes, list(self.values), None)
+        return DeviceColumn(codes.to(bycol.data.dtype), None, bycol.arrow_type)
+
+
+class _SourceRanks:
+    """A sorted stream whose batches come from several producer ranks, each holding a contiguous TIME RANGE of it
+    (range-partitioned sorted readers, dataset/ordered_readers.py:84-100).  All ranks ship their batches at once, so arrival
+    order is not time order across ranks; rank r's rows all precede rank r + 1's, so the batches are kept per source rank in
+    arrival order and the stream is put back together when it is complete."""
+
+    def __init__(self) -> None:
+        self.parts = {}              # source rank -> batches in arrival order
+
+    def add(self, batches: list):
+        for b in batches:
+            self.parts.setdefault(getattr(b, "src_rank", 0) or 0, []).append(b)
+
+    def take(self) -> DeviceTable | None:
+        """The whole stream as one table (None when nothing arrived); its time column still has to pass _require_sorted."""
+        parts = [b for r in sorted(self.parts) for b in self.parts[r]]
+        self.parts = {}
+        return concat_tables(parts) if parts else None
+
+
+def _require_sorted(time: torch.Tensor, message: str):
+    if len(time) > 1 and not bool((time[1:] >= time[:-1]).all().item()):
+        raise L.QkError(message)
+
+
+def _require_int64_time(*times: torch.Tensor):
+    if any(t.dtype != torch.int64 for t in times):
+        raise L.QkError("as-of time columns must be int64 / timestamp")
+
+
+def _time_unit(tcol: DeviceColumn) -> str | None:
+    """The unit of a timestamp column, None for a plain integer (or date) time column."""
+    return str(tcol.arrow_type.unit) if tcol.arrow_type is not None and pa.types.is_timestamp(tcol.arrow_type) else None
+
+
 # ---------------------------------------------------------------------------------------------- as-of
 class SortedAsofExecutor(Executor):
     """ts_executors.py:324-383: streaming backward as-of join of two time-sorted streams per symbol.
@@ -906,7 +974,10 @@ class SortedAsofExecutor(Executor):
 
     @property
     def silent_streams(self):      # across ranks over time ranges everything is held until done(); streaming otherwise
-        return "all" if (self.time_ranges and _world() > 1) else ()
+        return "all" if self._over_time_ranges() else ()
+
+    def _over_time_ranges(self) -> bool:
+        return bool(self.time_ranges) and world_size() > 1
 
     def __init__(self, time_col_trades="time", time_col_quotes="time", symbol_col_trades="symbol",
                  symbol_col_quotes="symbol", suffix="_right", time_ranges=False) -> None:
@@ -919,46 +990,13 @@ class SortedAsofExecutor(Executor):
         self.symbol_col_trades = symbol_col_trades
         self.symbol_col_quotes = symbol_col_quotes
         self.suffix = suffix
-        self._values, self._index, self._luts = None, None, {}     # the executor's own, append-only symbol codes
-        self._n_by = 0
+        self._codes = KeyCodes()     # the executor's own symbol codes, shared by both streams
         self._carry = None           # int32[n_by]: row of quote_state holding the newest swept quote of each symbol, -1 = none
         self._swept = 0              # rows of quote_state already folded into _carry
         self._whole_state = False    # too many symbols for the merge kernel: keep every quote, search the whole state
-        self._by_source = None       # several producer ranks: {stream: {source rank: [batches in arrival order]}}, joined at done()
+        self._by_source = None       # several producer ranks: {stream: _SourceRanks}, joined at done()
 
     BY = "__by"                      # hidden column: the symbol in the executor's code space
-
-    def _stable_codes(self, col: DeviceColumn) -> torch.Tensor:
-        """Codes that mean the same symbol in every batch of both streams (batch dictionaries are re-sorted unions and
-        differ from batch to batch): strings are numbered in order of first appearance, integer codes are used as is."""
-        if col.dictionary is not None:
-            if self._values is None:
-                if self._n_by:
-                    raise L.QkError("as-of `by` columns must both be strings or both be integer codes")
-                self._values, self._index = [], {}
-            key = (id(col.dictionary), len(col.dictionary))
-            lut = self._luts.get(key)
-            if lut is None:
-                codes = []
-                for v in col.dictionary:
-                    i = self._index.get(v)
-                    if i is None:
-                        i = self._index[v] = len(self._values)
-                        self._values.append(v)
-                    codes.append(i)
-                lut = (col.dictionary, torch.tensor(codes or [0], dtype=torch.int32, device=col.data.device))
-                self._luts[key] = lut                               # keeps the dictionary alive, so its id stays unique
-            self._n_by = max(self._n_by, len(self._values))
-            return lut[1][col.data.long()]
-        if self._values is not None:
-            raise L.QkError("as-of `by` columns must both be strings or both be integer codes")
-        codes = col.data.to(torch.int32)
-        if len(codes):
-            lo, hi = (int(v) for v in torch.stack(torch.aminmax(codes)).tolist())       # one pass, one read-back
-            if lo < 0:
-                raise L.QkError("as-of `by` codes must be non-negative")
-            self._n_by = max(self._n_by, hi + 1)
-        return codes
 
     def _append(self, state, batch, tcol):
         if state is None or len(state) == 0:
@@ -968,7 +1006,7 @@ class SortedAsofExecutor(Executor):
         return concat_tables([state, batch])
 
     def _carry_table(self, device) -> torch.Tensor:
-        n = max(1, self._n_by)
+        n = max(1, self._codes.n_by)
         if self._carry is None:
             self._carry = torch.full((n,), -1, dtype=torch.int32, device=device)
         elif self._carry.numel() < n:                              # new symbols appeared
@@ -981,10 +1019,9 @@ class SortedAsofExecutor(Executor):
         quotes = self.quote_state
         upto = len(quotes) if upto is None else upto
         lt, rt = trades[self.time_col_trades].data, quotes[self.time_col_quotes].data
-        if lt.dtype != torch.int64 or rt.dtype != torch.int64:
-            raise L.QkError("as-of time columns must be int64 / timestamp")
+        _require_int64_time(lt, rt)
         lby, rby = trades[self.BY].data, quotes[self.BY].data
-        n_by = max(1, self._n_by)
+        n_by = max(1, self._codes.n_by)
         ridx = None
         if not self._whole_state:
             carry = self._carry_table(lt.device)
@@ -999,15 +1036,13 @@ class SortedAsofExecutor(Executor):
             ridx = ops.asof_backward(lt, lby, rt, rby, n_by)
         right = quotes.drop([self.time_col_quotes, self.symbol_col_quotes, self.BY]).gather(ridx)
         right = right.with_validity((ridx >= 0).to(torch.uint8))
-        cols = dict(trades.drop([self.BY]).columns)
-        for n, c in right.columns.items():
-            cols[n + self.suffix if n in cols else n] = c
+        out = _append_right(trades.drop([self.BY]), right.columns, self.suffix)
         self._trim()
-        return DeviceTable(cols)
+        return out
 
     def _trim(self):
         """Swept quotes only matter as "newest of their symbol": keep those rows (<= n_symbols), drop the rest."""
-        if self._whole_state or self._swept < max(self.TRIM_ROWS, 4 * self._n_by):
+        if self._whole_state or self._swept < max(self.TRIM_ROWS, 4 * self._codes.n_by):
             return
         carry = self._carry
         live = carry >= 0
@@ -1023,24 +1058,21 @@ class SortedAsofExecutor(Executor):
         batches = _clean(batches)
         if not batches:
             return
-        if self.time_ranges and _world() > 1:
+        if self._over_time_ranges():
             if self._held is None:
                 self._held = {0: [], 1: []}
             self._held[stream_id].extend(batches)
             return
         if self._by_source is not None or any(getattr(b, "src_rank", None) is not None for b in batches):
-            # The batches come from several producer ranks, each holding a contiguous TIME RANGE of the sorted stream
-            # (range-partitioned sorted readers, dataset/ordered_readers.py:84-100), and all ranks ship their batches at
-            # once: arrival order is not time order across ranks.  Rank r's rows all precede rank r + 1's, so the
-            # stream is put back together per source rank, in arrival order, and joined when it is complete.
+            # the batches come from several producer ranks: once one has said so, both streams are put back together
+            # per source rank (_SourceRanks) and joined when they are complete
             if self._by_source is None:
-                self._by_source = {0: {}, 1: {}}
-            for b in batches:
-                self._by_source[stream_id].setdefault(getattr(b, "src_rank", 0) or 0, []).append(b)
+                self._by_source = {0: _SourceRanks(), 1: _SourceRanks()}
+            self._by_source[stream_id].add(batches)
             return
         batch = concat_tables(batches)
         by = self.symbol_col_trades if stream_id == 0 else self.symbol_col_quotes
-        batch = batch.with_column(self.BY, DeviceColumn(self._stable_codes(batch[by])))
+        batch = batch.with_column(self.BY, DeviceColumn(self._codes.codes(batch[by])))
         if stream_id == 0:
             self.trade_state = self._append(self.trade_state, batch, self.time_col_trades)
         else:
@@ -1088,9 +1120,7 @@ class SortedAsofExecutor(Executor):
         def shape(batches, t, col):                                 # rows, first time, last time, batches in time order?
             if t is None or len(t) == 0:
                 return [0, 0, 0, 1]
-            d = t[col].data
-            if d.dtype != torch.int64:
-                raise L.QkError("as-of time columns must be int64 / timestamp")
+            _require_int64_time(t[col].data)
             # the streams are declared sorted (OrderedStream); what is verified is how the pieces fit: batch against batch
             # here, rank against rank below -- not every row (two extra passes over both streams)
             ends = torch.stack([x for b in batches if len(b) for x in (b[col].data[0], b[col].data[-1])]).tolist()
@@ -1108,8 +1138,8 @@ class SortedAsofExecutor(Executor):
         # ---- newest quote per symbol of every rank, to everybody
         newest = None
         if quotes is not None and len(quotes) > 0:
-            codes = self._stable_codes(quotes[self.symbol_col_quotes])
-            n_by = max(1, self._n_by)
+            codes = self._codes.codes(quotes[self.symbol_col_quotes])
+            n_by = max(1, self._codes.n_by)
             empty_t, empty_b = torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int32, device=dev)
             _, table = ops.asof_merge(empty_t, empty_b, quotes[qt].data, codes, n_by, want_carry=True)
             if table is None:                                       # symbol set too large for the table: the last row of each code
@@ -1152,8 +1182,8 @@ class SortedAsofExecutor(Executor):
         if out is not None:
             return out
         q = concat_tables(all_q)
-        self.quote_state = q.with_column(self.BY, DeviceColumn(self._stable_codes(q[self.symbol_col_quotes])))
-        t = t.with_column(self.BY, DeviceColumn(self._stable_codes(t[self.symbol_col_trades])))
+        self.quote_state = q.with_column(self.BY, DeviceColumn(self._codes.codes(q[self.symbol_col_quotes])))
+        t = t.with_column(self.BY, DeviceColumn(self._codes.codes(t[self.symbol_col_trades])))
         return self._join(t, None)
 
     def _join_carried(self, trades, earlier, quotes):
@@ -1168,15 +1198,14 @@ class SortedAsofExecutor(Executor):
         sq, st_ = quotes[self.symbol_col_quotes], trades[self.symbol_col_trades]
         if sq.dictionary is not None or st_.dictionary is not None or E[self.symbol_col_quotes].dictionary is not None:
             both = concat_tables([E.select([self.symbol_col_quotes]), quotes.select([self.symbol_col_quotes])])     # one dictionary for both
-            codes = self._stable_codes(both[self.symbol_col_quotes])
+            codes = self._codes.codes(both[self.symbol_col_quotes])
             e_codes, q_codes = codes[:len(E)], codes[len(E):]
         else:
-            e_codes, q_codes = self._stable_codes(E[self.symbol_col_quotes]), self._stable_codes(sq)
-        t_codes = self._stable_codes(st_)
-        n_by, dev = max(1, self._n_by), trades.device
+            e_codes, q_codes = self._codes.codes(E[self.symbol_col_quotes]), self._codes.codes(sq)
+        t_codes = self._codes.codes(st_)
+        n_by, dev = max(1, self._codes.n_by), trades.device
         lt, rt = trades[self.time_col_trades].data, quotes[self.time_col_quotes].data
-        if lt.dtype != torch.int64 or rt.dtype != torch.int64:
-            raise L.QkError("as-of time columns must be int64 / timestamp")
+        _require_int64_time(lt, rt)
         none_t, none_b = torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int32, device=dev)
         _, carried = ops.asof_merge(none_t, none_b, E[self.time_col_quotes].data, e_codes, n_by, want_carry=True)
         if carried is None:
@@ -1190,25 +1219,20 @@ class SortedAsofExecutor(Executor):
         valid = (ridx >= 0).to(torch.uint8)
         if os.environ.get("QK_DEBUG_ASOF"):
             print(f"[asof] carried join: {len(E)} carried rows, {int((~in_shard & (ridx >= 0)).sum())} answers from them", flush=True)
-        cols = dict(trades.columns)
-        for n in payload:
-            a, b_ = from_shard[n], from_carry[n]
-            cols[n + self.suffix if n in cols else n] = DeviceColumn(torch.where(in_shard, a.data, b_.data), a.dictionary, a.arrow_type, valid)
-        return DeviceTable(cols)
+        right = {n: DeviceColumn(torch.where(in_shard, from_shard[n].data, from_carry[n].data), from_shard[n].dictionary,
+                                 from_shard[n].arrow_type, valid) for n in payload}
+        return _append_right(trades, right, self.suffix)
 
     def done(self, executor_id):
-        if self.time_ranges and _world() > 1:
+        if self._over_time_ranges():
             return self._join_time_ranges()
         if self._by_source is not None:
             for sid, tcol, by in ((0, self.time_col_trades, self.symbol_col_trades), (1, self.time_col_quotes, self.symbol_col_quotes)):
-                parts = [b for r in sorted(self._by_source[sid]) for b in self._by_source[sid][r]]
-                if not parts:
+                t = self._by_source[sid].take()
+                if t is None:
                     continue
-                t = concat_tables(parts)
-                tt = t[tcol].data
-                if len(tt) > 1 and not bool((tt[1:] >= tt[:-1]).all().item()):
-                    raise L.QkError("as-of join: the producer ranks do not hold consecutive time ranges of a sorted stream")
-                t = t.with_column(self.BY, DeviceColumn(self._stable_codes(t[by])))
+                _require_sorted(t[tcol].data, "as-of join: the producer ranks do not hold consecutive time ranges of a sorted stream")
+                t = t.with_column(self.BY, DeviceColumn(self._codes.codes(t[by])))
                 if sid == 0:
                     self.trade_state = t
                 else:
@@ -1228,40 +1252,31 @@ class _KeySegmented(Executor):
     """Input handling shared by the done-time operators over an OrderedStream hash-partitioned by a key (the windows, the
     pattern search): batches are kept per source rank in arrival order (ranks hold consecutive time ranges), put back together
     and checked to be time-sorted, and the rows are segmented by key with the stable partition kernel, so time order survives
-    inside a key."""
+    inside a key.  The pieces are _SourceRanks, _require_sorted and KeyCodes."""
 
     silent_streams = "all"       # the answer is computed when the channel's input is complete
 
     def _init_segments(self):
-        self._parts = {}             # source rank -> batches in arrival order
-        self._codes = SortedAsofExecutor()      # only for its append-only symbol codes
+        self._input = _SourceRanks()
+        self._codes = KeyCodes()
 
     def execute(self, batches, stream_id, executor_id):
-        for b in _clean(batches):
-            self._parts.setdefault(getattr(b, "src_rank", 0) or 0, []).append(b)
+        self._input.add(_clean(batches))
 
     def _sorted_input(self, time_col: str, who: str):
         """(the whole input as one table, its time column as int64), or None when nothing arrived."""
-        parts = [b for r in sorted(self._parts) for b in self._parts[r]]
-        self._parts = {}
-        if not parts:
+        t = self._input.take()
+        if t is None:
             return None
-        t = concat_tables(parts)
         time = t[time_col].data.to(torch.int64)
-        if len(time) > 1 and not bool((time[1:] >= time[:-1]).all().item()):
-            raise L.QkError(f"{who}: the stream is not sorted by " + time_col)
+        _require_sorted(time, f"{who}: the stream is not sorted by " + time_col)
         return t, time
 
     def _segment(self, codes: torch.Tensor, columns: list):
         """(columns moved into key-segmented order, segment starts int64[n_by + 1], n_by)."""
-        n_by = max(1, self._codes._n_by)
+        n_by = max(1, self._codes.n_by)
         dest, seg = ops.partition_plan(codes, n_by, L.PART_CODE)
         return ops.scatter(columns, dest), seg, n_by
-
-    def _by_column(self, codes: torch.Tensor, bycol: DeviceColumn) -> DeviceColumn:
-        if self._codes._values is not None:
-            return DeviceColumn(codes, list(self._codes._values), None)
-        return DeviceColumn(codes.to(bycol.data.dtype), None, bycol.arrow_type)
 
     def _time_column(self, time: torch.Tensor, tcol: DeviceColumn) -> DeviceColumn:
         return DeviceColumn(time.to(tcol.data.dtype), None, tcol.arrow_type)
@@ -1290,7 +1305,7 @@ class _WindowExecutor(_KeySegmented):
         t, time = got
         tcol = t[self.time_col]
         bycol = t[self.by_col]
-        codes = self._codes._stable_codes(bycol)
+        codes = self._codes.codes(bycol)
         aggs = self.window.parsed()
         exprs, vals = [], []
         for _, op, arg in aggs:                                   # one fp64 column per distinct argument expression
@@ -1300,13 +1315,7 @@ class _WindowExecutor(_KeySegmented):
                 vals.append(to_f64(e["__v"].data))
         moved, seg, n_by = self._segment(codes, [time, codes] + vals)
         spec = [(name, op, exprs.index(arg.sql()) if arg is not None else -1) for name, op, arg in aggs]
-        unit = str(tcol.arrow_type.unit) if tcol.arrow_type is not None and pa_is_timestamp(tcol.arrow_type) else None
-        return moved[0], moved[1], seg, n_by, moved[2:], spec, (bycol, tcol, unit)
-
-
-def pa_is_timestamp(t) -> bool:
-    import pyarrow as pa
-    return pa.types.is_timestamp(t)
+        return moved[0], moved[1], seg, n_by, moved[2:], spec, (bycol, tcol, _time_unit(tcol))
 
 
 _WIN = {"sum": L.WIN_SUM, "min": L.WIN_MIN, "max": L.WIN_MAX, "count": L.WIN_COUNT, "avg": L.WIN_AVG}
@@ -1327,7 +1336,7 @@ class SlidingWindowExecutor(_WindowExecutor):
         time, codes, seg, n_by, vals, spec, (bycol, tcol, unit) = seg_in
         size = self.window.ticks(self.window.size_before, unit)
         outs = ops.window_sliding(time, codes, seg, n_by, size, vals, [(_WIN[op], max(src, 0)) for _, op, src in spec])
-        cols = {self.time_col: self._time_column(time, tcol), self.by_col: self._by_column(codes, bycol)}
+        cols = {self.time_col: self._time_column(time, tcol), self.by_col: self._codes.column(codes, bycol)}
         for (name, op, _), o in zip(spec, outs):
             cols[name] = _int_result(op, o)
         return DeviceTable(cols)
@@ -1381,7 +1390,7 @@ class HoppingWindowExecutor(_HashedWindow):
             return None
         gathered = ops.gather(vals, src) if vals else []
         ok, out = self._aggregate([key, wstart], gathered, spec)
-        cols = {self.time_col: self._time_column(ok[1], tcol), self.by_col: self._by_column(ok[0], bycol)}
+        cols = {self.time_col: self._time_column(ok[1], tcol), self.by_col: self._codes.column(ok[0], bycol)}
         cols.update(out)
         return DeviceTable(cols)
 
@@ -1405,7 +1414,7 @@ class SessionWindowExecutor(_HashedWindow):
         # the first row of session s (ids are 1-based and increase along the segmented order)
         starts = torch.nonzero(torch.diff(ids, prepend=ids[:1] - 1)).flatten()
         at = starts[ok[0] - 1]
-        cols = {self.by_col: self._by_column(codes[at], bycol), self.time_col: self._time_column(time[at], tcol)}
+        cols = {self.by_col: self._codes.column(codes[at], bycol), self.time_col: self._time_column(time[at], tcol)}
         cols.update(out)
         return DeviceTable(cols)
 
@@ -1450,19 +1459,18 @@ class CEPExecutor(_KeySegmented):
             if not float(days).is_integer():
                 raise E.ExprError("maxspan over a date column must be a whole number of days")
             return int(days)
-        unit = str(tcol.arrow_type.unit) if tcol.arrow_type is not None and pa_is_timestamp(tcol.arrow_type) else None
-        return Window.ticks(self.max_span, unit)
+        return Window.ticks(self.max_span, _time_unit(tcol))
 
     def _empty(self, tcol: DeviceColumn, bycol: DeviceColumn, dev) -> DeviceTable:
         none = torch.empty(0, dtype=torch.int64, device=dev)
-        return DeviceTable({self.by_col: self._by_column(none.to(torch.int32), bycol)} |
+        return DeviceTable({self.by_col: self._codes.column(none.to(torch.int32), bycol)} |
                            {n: self._time_column(none, tcol) for n in self.names})
 
     def search_inputs(self, t: DeviceTable, time: torch.Tensor) -> dict:
         """The arguments of ops.pattern_search for the rows of `t` (time = its time column as int64): the rows segmented by key,
         the candidate mask from the row-local conjuncts, the start rows and the link programs.  None when no row starts a match."""
         tcol, bycol = t[self.time_col], t[self.by_col]
-        codes = self._codes._stable_codes(bycol)
+        codes = self._codes.codes(bycol)
         read = sorted(self.preds.columns, key=t.column_names.index)
         plain, mask_of = t.select(read).split_validity()
         hidden = sorted(set(mask_of.values()))
@@ -1520,14 +1528,14 @@ class CEPExecutor(_KeySegmented):
         except ops.PatternBudgetError as err:
             r = int(starts[err.index].item())
             code = int(scodes[r].item())
-            key = self._codes._values[code] if self._codes._values is not None else code
+            key = self._codes.values[code] if self._codes.values is not None else code
             raise L.QkError(f"pattern_recognize: the search from the row of key {key!r} at time {int(stime[r].item())} tested more "
                             f"than {self.BUDGET} rows; narrow the pattern (maxspan, more selective predicates)") from err
         keep = torch.nonzero(bound[:, 0] >= 0).flatten()
         bound = bound[keep]
         if bound.shape[0] == 0:
             return self._empty(tcol, bycol, time.device)
-        out = {self.by_col: self._by_column(ops.gather([scodes], bound[:, 0].contiguous())[0], bycol)}
+        out = {self.by_col: self._codes.column(ops.gather([scodes], bound[:, 0].contiguous())[0], bycol)}
         for e, name in enumerate(self.names):
             out[name] = self._time_column(ops.gather([stime], bound[:, e].contiguous())[0], tcol)
         return DeviceTable(out)

@@ -27,7 +27,7 @@ import torch.distributed as dist
 
 from . import _lib as L
 from . import ops
-from .columns import DeviceColumn, DeviceTable, as_device_table, concat_tables, unify_dictionaries
+from .columns import DeviceColumn, DeviceTable, as_device_table, concat_tables, rank, unify_dictionaries, world_size
 from .edge import Parts, partition_fn
 from .placement_strategy import CustomChannelsStrategy, SingleChannelStrategy
 from .target_info import BroadcastPartitioner, PassThroughPartitioner, TargetInfo
@@ -36,14 +36,6 @@ from .target_info import BroadcastPartitioner, PassThroughPartitioner, TargetInf
 def _default_device():
     from . import columns
     return columns.default_device()
-
-
-def world_size() -> int:
-    return dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-
-
-def rank() -> int:
-    return dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
 
 
 # ------------------------------------------------------------------ the shuffle

@@ -772,6 +772,20 @@ def case_executor_protocol(qc, golden_dir):
         raise RuntimeError("expected an assertion")
     except AssertionError:
         pass
+    # the broadcast join is the same build and probe over a table the executor holds, refusals included
+    from quokka_b200 import _lib as L
+    from quokka_b200.executors import BroadcastJoinExecutor
+    big = DeviceTable.from_arrow(ta)
+    shuffled = BuildProbeJoinExecutor(left_on="key_a", right_on="key_b", how="left")
+    shuffled.execute([DeviceTable.from_arrow(tb)], 1, 0)
+    got = BroadcastJoinExecutor(tb, small_on="key_b", big_on="key_a", suffix="_right", how="left").execute([big], 0, 0)
+    by = [(c, "ascending") for c in ("key_a", "val1_a", "val1_b")]            # the probe emits its rows in no fixed order
+    assert got.to_arrow().sort_by(by).equals(shuffled.execute([big], 0, 0).to_arrow().sort_by(by))
+    try:
+        BroadcastJoinExecutor(pa.table({"k": np.zeros(4, np.float32)}), on="k").execute([t], 0, 0)
+        raise RuntimeError("expected a refusal of the float32 key")
+    except L.QkError as err:
+        assert "join key 'k' must be" in str(err)
 
 
 def case_scalar_aggs(qc):

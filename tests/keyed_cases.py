@@ -1,6 +1,7 @@
 """Exact references and seeded generators for the keyed kernels: the hash aggregate (csrc/hashagg.cu), the hash join
 (csrc/join.cu) and the top-k select (csrc/topk.cu) with the host ordering after it (executors.sort_table / top_k_table).
-numpy only: no torch, no quokka_b200 import, so the CPU suite can check these references against brute-force loops.
+numpy only: no torch, no quokka_b200 import, so the CPU suite can check these references against brute-force loops.  The two
+executor cases at the end take the executors module from their caller, which runs them on the device or on the CPU shim.
 
 Ordering (DESIGN.md section 2, DuckDB's ORDER BY):
   numbers compare by value and -0.0 = +0.0; every NaN, whichever sign, is greater than +inf (last ASC, first DESC);
@@ -254,3 +255,56 @@ def order_column(rng, dt, n: int, card: int, specials: bool = True) -> np.ndarra
         v = pool[rng.integers(0, len(pool), n)]
         return v.astype(dt) if dt == np.float32 else v
     return int_keys(rng, dt, n, card, edges=specials)
+
+
+# ------------------------------------------------------------------ the executors that grow the hash aggregate
+# (the executors module comes from the caller: on the device, or on the CPU shim)
+def count_grows(X, monkeypatch) -> list:
+    """Records the incoming row count of every re-insertion into a larger table, whichever executor asks for it."""
+    grows = []
+    real = X._GrowingHashAgg._grow
+    monkeypatch.setattr(X._GrowingHashAgg, "_grow", lambda self, inc: (grows.append(inc), real(self, inc))[1])
+    return grows
+
+
+def case_sql_agg_executor_grow(X, monkeypatch):
+    """SQLAggExecutor re-inserts its groups into a larger table when a batch would push the load past 1/2; batches of rising
+    cardinality grow it several times.  SUM / MIN / MAX of the re-inserted partials equal one aggregate over all rows."""
+    import pyarrow as pa
+    rng = np.random.default_rng(5)
+    grows = count_grows(X, monkeypatch)
+    ex = X.SQLAggExecutor(["k"], None, "SUM(v) AS s, MIN(v) AS mn, MAX(v) AS mx")
+    parts = []
+    for n, card in zip([1000, 40_000, 100_000, 400_000, 20_000], [300, 20_000, 80_000, 400_000, 500_000]):
+        parts.append((rng.integers(-card, card, n).astype(np.int64) * 31, float_values(rng, n, "dyadic", specials=True)))
+    for k, v in parts:
+        ex.execute([pa.table({"k": k, "v": v})], 0, 0)
+    out = ex.done(0).to_numpy()
+    assert len(grows) >= 2, grows
+    k = np.concatenate([p[0] for p in parts])
+    v = np.concatenate([p[1] for p in parts])
+    ref = ref_groupby([k], [v] * 3, ["sum", "min", "max"])
+    o = np.argsort(out["k"])
+    assert np.array_equal(out["k"][o], ref["keys"][0])
+    for name, r in zip(("s", "mn", "mx"), ref["vals"]):
+        assert np.array_equal(out[name][o], r, equal_nan=True), name
+
+
+def case_distinct_executor_grow(X, monkeypatch):
+    import pyarrow as pa
+    rng = np.random.default_rng(6)
+    grows = count_grows(X, monkeypatch)
+    ex = X.DistinctExecutor(["a", "b"])
+    seen = []
+    for n, card in zip([2000, 60_000, 200_000, 300_000], [100, 30_000, 150_000, 600_000]):
+        a = rng.integers(-card, card, n).astype(np.int64)
+        b = rng.integers(-3, 3, n).astype(np.int32)
+        seen.append((a, b))
+        ex.execute([pa.table({"a": a, "b": b})], 0, 0)
+    assert ex._ha.state.capacity > (1 << 16) and len(grows) >= 2, grows      # the table grew
+    out = ex.done(0).to_numpy()
+    a = np.concatenate([s[0] for s in seen])
+    b = np.concatenate([s[1] for s in seen])
+    ref = ref_groupby([a, b], [], [])
+    o = np.lexsort((out["b"], out["a"]))
+    assert np.array_equal(out["a"][o], ref["keys"][0]) and np.array_equal(out["b"][o], ref["keys"][1])

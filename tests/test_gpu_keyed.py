@@ -5,7 +5,6 @@ use the kernels' bounded probes and the flags they return."""
 import zlib
 
 import numpy as np
-import pyarrow as pa
 import pytest
 import torch
 
@@ -163,53 +162,10 @@ def test_hash_aggregate_empty_and_single_row(qb):
     _check_agg(qb, [np.array([K.I64_MIN])], np.array([K.NAN_NEG]), 16)
 
 
-def _arrow_batches(rng, sizes, cards, nan=True):
-    out = []
-    for n, card in zip(sizes, cards):
-        k = rng.integers(-card, card, n).astype(np.int64) * 31
-        v = K.float_values(rng, n, "dyadic", specials=nan)
-        out.append((k, v))
-    return out
+def test_sql_agg_executor_grow(qb, monkeypatch): K.case_sql_agg_executor_grow(qb.X, monkeypatch)
 
 
-def test_sql_agg_executor_grow(qb, monkeypatch):
-    """SQLAggExecutor re-inserts its groups into a larger table when a batch would push the load past 1/2; batches of rising
-    cardinality grow it several times.  SUM / MIN / MAX of the re-inserted partials equal one aggregate over all rows."""
-    rng = np.random.default_rng(5)
-    grows = []
-    real = qb.X.SQLAggExecutor._grow
-    monkeypatch.setattr(qb.X.SQLAggExecutor, "_grow", lambda self, inc: (grows.append(inc), real(self, inc))[1])
-    ex = qb.X.SQLAggExecutor(["k"], None, "SUM(v) AS s, MIN(v) AS mn, MAX(v) AS mx")
-    parts = _arrow_batches(rng, [1000, 40_000, 100_000, 400_000, 20_000], [300, 20_000, 80_000, 400_000, 500_000])
-    for k, v in parts:
-        ex.execute([pa.table({"k": k, "v": v})], 0, 0)
-    out = ex.done(0).to_numpy()
-    assert len(grows) >= 2, grows
-    k = np.concatenate([p[0] for p in parts])
-    v = np.concatenate([p[1] for p in parts])
-    ref = K.ref_groupby([k], [v] * 3, OPS)
-    o = np.argsort(out["k"])
-    assert np.array_equal(out["k"][o], ref["keys"][0])
-    for name, r in zip(("s", "mn", "mx"), ref["vals"]):
-        assert np.array_equal(out[name][o], r, equal_nan=True), name
-
-
-def test_distinct_executor_grow(qb):
-    rng = np.random.default_rng(6)
-    ex = qb.X.DistinctExecutor(["a", "b"])
-    seen = []
-    for n, card in zip([2000, 60_000, 200_000, 300_000], [100, 30_000, 150_000, 600_000]):
-        a = rng.integers(-card, card, n).astype(np.int64)
-        b = rng.integers(-3, 3, n).astype(np.int32)
-        seen.append((a, b))
-        ex.execute([pa.table({"a": a, "b": b})], 0, 0)
-    assert ex._ha.capacity > (1 << 16)                                   # the table grew
-    out = ex.done(0).to_numpy()
-    a = np.concatenate([s[0] for s in seen])
-    b = np.concatenate([s[1] for s in seen])
-    ref = K.ref_groupby([a, b], [], [])
-    o = np.lexsort((out["b"], out["a"]))
-    assert np.array_equal(out["a"][o], ref["keys"][0]) and np.array_equal(out["b"][o], ref["keys"][1])
+def test_distinct_executor_grow(qb, monkeypatch): K.case_distinct_executor_grow(qb.X, monkeypatch)
 
 
 def test_dense_and_hash_paths_agree(qb, monkeypatch):
@@ -227,7 +183,7 @@ def test_dense_and_hash_paths_agree(qb, monkeypatch):
     for force_hash in (False, True):
         if force_hash:
             monkeypatch.setattr(qb.edge, "dense_agg_fits", lambda *a: False)
-            monkeypatch.setattr(qb.edge, "_single_process", lambda: False)
+            monkeypatch.setattr(qb.edge, "world_size", lambda: 2)
         out = agg(t).to_numpy()
         runs.append((agg.last_path, out))
     assert runs[0][0] != "hash" and runs[1][0] == "hash", [r[0] for r in runs]

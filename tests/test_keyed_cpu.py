@@ -249,6 +249,12 @@ def test_top_k_same_answer_on_both_sides_of_the_switch(shim):
         assert np.array_equal(keys[small], keys[big])
 
 
+def test_sql_agg_executor_grow(shim, monkeypatch): K.case_sql_agg_executor_grow(shim, monkeypatch)
+
+
+def test_distinct_executor_grow(shim, monkeypatch): K.case_distinct_executor_grow(shim, monkeypatch)
+
+
 # ------------------------------------------------------------------ the DataStream API on the shim
 @pytest.fixture
 def qc(monkeypatch):
