@@ -492,6 +492,29 @@ QK_API int qk_pattern_search(const qk_column* time, const qk_column* by, const i
                              int32_t nlink, const qk_expr* links, int64_t budget, int32_t* out_bound, uint64_t* status,
                              uint64_t* rows_tested, void* stream);
 
+/* ---- K13: stable radix sort to a permutation ---------------------------------------------------------------------
+ * Replaces the per-batch polars sort, the spill files and the final merge of SuperFastSortExecutor
+ * (pyquokka/executors/sql_executors.py:128,153,185) behind DataStream.sort.  key = one scalar column (QK_U8 / QK_I32 / QK_I64 /
+ * QK_F32 / QK_F64) of nrows rows.  perm_out (device int32[nrows]) receives the row numbers of `key` in ascending order of the
+ * 64-bit order image: integers exact over their whole range, -0.0 = +0.0, every NaN after +inf; descending != 0 sorts by the
+ * complemented image (NaN first).  valid (device uint8 per row of `key`, or NULL): rows with valid == 0 come after every valid
+ * row in both directions and tie with each other (NULLS LAST).
+ * STABLE: rows with equal images keep the order they have in perm_in (device int32[nrows], a permutation of the row numbers;
+ * NULL = identity), so a multi-column sort is a chain of calls, last column first, each reading key[perm_in[i]].
+ * image_out (device uint64[nrows] or NULL) receives the sorted images as the sort compared them (already complemented when
+ * descending; the image of a NULL row is 0, ~0 when descending).
+ * An LSD radix sort of (image, row number) pairs by 8-bit digits; a digit in which all valid rows agree costs no pass, which the
+ * device decides from the histograms of the first pass (no host round trip).  Deterministic: positions are sums of counts.
+ * Workspace: qk_sort_workspace_bytes(nrows) (two pair buffers: 24 B/row, plus 3 MB).  nrows == 0 is a no-op.
+ * Errors: nrows > 2^31 - 1: QK_ERR_UNSUPPORTED; key->length != nrows, a bad dtype, null perm_out: QK_ERR_INVALID; a vector
+ * column: QK_ERR_UNSUPPORTED; workspace too small: QK_ERR_CAPACITY.
+ * qk_sort_last_plan: the passes the last qk_sort_perm of this thread ran, e.g. "d8 passes=2/8 nulls=0" (8-bit digits, live
+ * image passes of 8, whether the NULL pass ran).  It waits for the device and reads the plan back: for tests and benchmarks. */
+QK_API size_t qk_sort_workspace_bytes(int64_t nrows);
+QK_API int qk_sort_perm(const qk_column* key, const uint8_t* valid, int32_t descending, const int32_t* perm_in, int32_t* perm_out,
+                        uint64_t* image_out, int64_t nrows, void* workspace, size_t workspace_bytes, void* stream);
+QK_API const char* qk_sort_last_plan(void);
+
 /* ---- synthetic TPC-H-shaped / SIP-shaped columns, generated in HBM --------------------------
  * Bit-identical to oracle/tpch_gen.py (counter-based hash of (table, column, row)); lets bench.py hold
  * SF-100 (600 037 902 lineitem rows) resident without a 23 GB host copy.  `column` ids: see

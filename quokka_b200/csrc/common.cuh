@@ -133,6 +133,27 @@ __device__ __forceinline__ int64_t load_i64(const void* p, int dt, int64_t i) {
         default: return ((const int64_t*)p)[i];
     }
 }
+// The ascending order image of element i (DESIGN.md section 2 "Ordering rules"): unsigned comparison of images is DuckDB's
+// ORDER BY.  Integers are exact over their whole range, -0.0 is folded onto +0.0 and every NaN, whatever its sign and
+// payload, takes the greatest image (after +inf).  32-bit and 8-bit types sit in the top bytes.  Descending = ~image.
+__device__ __forceinline__ unsigned long long order_image(const void* p, int dt, int64_t i) {
+    switch (dt) {
+        case QK_F64: {
+            unsigned long long b = ((const unsigned long long*)p)[i];
+            if (b == 0x8000000000000000ULL) b = 0;
+            return (b << 1) > 0xffe0000000000000ULL ? ~0ULL : (b >> 63) ? ~b : (b | 0x8000000000000000ULL);
+        }
+        case QK_F32: {
+            unsigned b = ((const unsigned*)p)[i];
+            if (b == 0x80000000u) b = 0;
+            const unsigned v = (b << 1) > 0xff000000u ? ~0u : (b >> 31) ? ~b : (b | 0x80000000u);
+            return (unsigned long long)v << 32;
+        }
+        case QK_I64: return ((const unsigned long long*)p)[i] ^ 0x8000000000000000ULL;
+        case QK_I32: return (unsigned long long)(((const unsigned*)p)[i] ^ 0x80000000u) << 32;
+        default: return (unsigned long long)((const uint8_t*)p)[i] << 56;
+    }
+}
 __device__ __forceinline__ bool cmp_i64(int64_t a, int cmp, int64_t b) {
     switch (cmp) {
         case QK_CMP_LT: return a < b;

@@ -12,26 +12,9 @@ namespace {
 
 struct SelState { unsigned long long prefix; long long k_rem; unsigned hist[256]; };
 
-// The order is DuckDB's ORDER BY (DESIGN.md section 2): -0.0 = +0.0, and every NaN, whatever its sign and payload, is
-// greater than +inf -- so -0.0 is folded onto +0.0 and a NaN takes the greatest image before the ascending flip.
+// The select keeps the largest images, so the order image (common.cuh order_image) is flipped for ascending order.
 __device__ __forceinline__ unsigned long long image_of(const void* p, int dt, int64_t i, int descending) {
-    unsigned long long u;
-    switch (dt) {
-        case QK_F64: {
-            unsigned long long b = ((const unsigned long long*)p)[i];
-            if (b == 0x8000000000000000ULL) b = 0;
-            u = (b << 1) > 0xffe0000000000000ULL ? ~0ULL : (b >> 63) ? ~b : (b | 0x8000000000000000ULL);
-        } break;
-        case QK_F32: {
-            unsigned b = ((const unsigned*)p)[i];
-            if (b == 0x80000000u) b = 0;
-            const unsigned v = (b << 1) > 0xff000000u ? ~0u : (b >> 31) ? ~b : (b | 0x80000000u);
-            u = (unsigned long long)v << 32;
-        } break;
-        case QK_I64: u = ((const unsigned long long*)p)[i] ^ 0x8000000000000000ULL; break;
-        case QK_I32: u = (unsigned long long)(((const unsigned*)p)[i] ^ 0x80000000u) << 32; break;
-        default: u = (unsigned long long)((const uint8_t*)p)[i] << 56; break;
-    }
+    const unsigned long long u = order_image(p, dt, i);
     return descending ? u : ~u;
 }
 

@@ -17,7 +17,7 @@ from . import _lib as L
 from . import expr as E
 from .edge import EdgeOps, PartialAgg
 from .executors import (BuildProbeJoinExecutor, ConcatThenSQLExecutor, DistinctExecutor, OutputExecutor,
-                        SortedAsofExecutor, SQLAggExecutor, top_k_table)
+                        SortedAsofExecutor, SortExecutor, SQLAggExecutor, top_k_table)
 from .placement_strategy import CustomChannelsStrategy, SingleChannelStrategy
 from .target_info import BroadcastPartitioner, HashPartitioner, PassThroughPartitioner, TargetInfo
 
@@ -178,6 +178,22 @@ class TopKNode(Node):
 
     def est_rows(self):
         return self.k
+
+
+class SortNode(Node):
+    kind = "sort"
+
+    def __init__(self, parent, by, desc):
+        _reject_vectors(parent.vectors, by, "sort key")
+        super().__init__(parent.schema, [parent])
+        self.by, self.desc = by, desc
+
+
+def ends_in_sort(node: Node) -> bool:
+    """True when the rows of `node` are a sort's output seen through row-wise operators (filter / select / rename / map)."""
+    while node.kind in ("filter", "select", "rename", "map"):
+        node = node.parents[0]
+    return node.kind == "sort"
 
 
 class DistinctNode(Node):
@@ -366,6 +382,8 @@ class Lowering:
             return self._agg(node, stage)
         if k == "topk":
             return self._topk(node, need, stage)
+        if k == "sort":
+            return self._sort(node, need, stage)
         if k == "distinct":
             aid, ops, raw = self.lower(node.parents[0], set(node.keys), stage)
             ops.select(node.keys, raw)
@@ -472,6 +490,13 @@ class Lowering:
         sql = "select * from batch_arrow order by " + ",".join(c + (" desc" if d else " asc") for c, d in zip(by, desc)) + " limit " + str(k)
         ti = TargetInfo(BroadcastPartitioner(), None, None, [lambda t: top_k_table(t, by, desc, k)], edge_ops=ops)
         out = self.g.new_non_blocking_node({0: aid}, ConcatThenSQLExecutor(sql), stage, SingleChannelStrategy(), {0: ti})
+        return out, EdgeOps(), ops.visible(raw)
+
+    def _sort(self, node: SortNode, need, stage):
+        # every rank sorts what it holds and the ranks trade ranges inside the executor (SortExecutor.done): the edge moves nothing
+        aid, ops, raw = self.lower(node.parents[0], None if need is None else set(need) | set(node.by), stage)
+        ti = TargetInfo(PassThroughPartitioner(), None, None, [], edge_ops=ops, stable=True)
+        out = self.g.new_non_blocking_node({0: aid}, SortExecutor(node.by, node.desc), stage, CustomChannelsStrategy(1), {0: ti})
         return out, EdgeOps(), ops.visible(raw)
 
     def _asof(self, node: AsofNode, need, stage):
@@ -686,6 +711,27 @@ class DataStream:
         assert type(k) == int and k > 0
         assert all(c in self.schema for c in columns)
         return DataStream(self.quokka_context, TopKNode(self.node, columns, k, descending))
+
+    def sort(self, columns, descending=None):
+        """ORDER BY over the whole stream (the reference's SuperFastSortExecutor, sql_executors.py:88-187): `columns` a name or a
+        list, `descending` a bool or one per column (default ascending); NULLs last in both directions, rows that tie on every
+        column keep their order of arrival.  Returns an OrderedStream: collect() gives the rows in order, and when the first
+        column is ascending the stream is sorted by it for join_asof / windowed_transform / pattern_recognize.  On several
+        ranks, rank r holds the r-th range of the first column and all rows of one of its values are on one rank.  A later
+        select / rename / filter keeps the order; an operator that hash-partitions does not.  The stream must fit in device
+        memory."""
+        if isinstance(columns, str):
+            columns = [str(columns)]
+        assert type(columns) == list and len(columns) > 0
+        if descending is not None:
+            if type(descending) == bool:
+                descending = [descending]
+            assert type(descending) == list and len(descending) == len(columns)
+            assert all([type(i) == bool for i in descending])
+        else:
+            descending = [False] * len(columns)
+        assert all(c in self.schema for c in columns)
+        return OrderedStream(self.quokka_context, SortNode(self.node, columns, descending), None if descending[0] else columns[0])
 
     def distinct(self, keys):
         if isinstance(keys, str):
@@ -923,7 +969,7 @@ class DataStream:
     # ---- actions
     def collect(self):
         """Run the plan; returns a pyarrow.Table (the reference returns a Polars frame; Polars is not
-        installable here -- SURVEY.md Appendix A-14).  Rows are unordered unless the plan ends in top_k /
+        installable here -- SURVEY.md Appendix A-14).  Rows are unordered unless the plan ends in top_k, sort /
         an ordered aggregate."""
         return self.quokka_context.execute_node(self.node)
 
@@ -938,6 +984,7 @@ class DataStream:
         def walk(n, d=0):
             extra = {"filter": lambda: n.pred.sql(), "join": lambda: f"{n.how} {n.left_on}={n.right_on}",
                      "agg": lambda: f"keys={n.keys}", "topk": lambda: f"{n.by} k={n.k}",
+                     "sort": lambda: ", ".join(c + (" desc" if d else "") for c, d in zip(n.by, n.desc)),
                      "stateful": lambda: getattr(n.executor, "explain", lambda: "")()}.get(n.kind, lambda: "")()
             print("  " * d + f"{n.kind} {extra} -> {n.schema}")
             for p in n.parents:

@@ -14,7 +14,7 @@ def _default_device():
     return _columns.default_device()
 
 from .dataset import InputArrowDataset, InputDeviceDataset, InputDiskCSVDataset, InputParquetDataset, InputPinnedDataset, InputSortedParquetDataset
-from .datastream import DataStream, Lowering, OrderedStream, SourceNode, push_filters
+from .datastream import DataStream, Lowering, OrderedStream, SourceNode, ends_in_sort, push_filters
 from .executors import StorageExecutor
 from .placement_strategy import CustomChannelsStrategy
 from .runtime import TaskGraph, gather_to_all, world_size
@@ -152,7 +152,8 @@ class QuokkaContext:
         node = push_filters(node, [])
         g = TaskGraph(self)
         aid, ops, raw = Lowering(g).lower(node, None, 0)
-        ti = TargetInfo(PassThroughPartitioner(), None, None, [], edge_ops=ops)
+        # a plan that ends in a sort (under row-wise operators only) is collected in order: its filters must not reorder rows
+        ti = TargetInfo(PassThroughPartitioner(), None, None, [], edge_ops=ops, stable=ends_in_sort(node))
         sink = g.new_blocking_node({0: aid}, StorageExecutor(), 0, CustomChannelsStrategy(1), {0: ti})
         g.create()
         g.run()

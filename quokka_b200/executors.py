@@ -471,6 +471,7 @@ class SQLAggExecutor(Executor):
 
 
 _SIGN = np.uint64(1 << 63)
+_SIGN_I64 = -(1 << 63)          # the same bit in an int64 tensor: image ^ _SIGN_I64 orders as int64 the way the image orders
 
 
 def order_image(v: np.ndarray, descending: bool) -> np.ndarray:
@@ -568,6 +569,118 @@ class ConcatThenSQLExecutor(Executor):
         if not self._batches:
             return None
         self.state = top_k_table(concat_tables(self._batches), self.by, self.desc, self.k)
+        return self.state
+
+
+def _sort_key(col: DeviceColumn, name: str) -> torch.Tensor:
+    """The values a column sorts by: a string column by its value (the rank of every dictionary entry), not by its code."""
+    if col.is_vector:
+        raise L.QkError(f"sort: column {name!r} is a vector column")
+    if col.dictionary is None:
+        return col.data
+    rank = np.argsort(np.argsort(np.array(col.dictionary, dtype=object), kind="stable"), kind="stable")
+    lut = torch.from_numpy(rank.astype(np.int32) if len(rank) else np.zeros(1, np.int32)).to(col.data.device)
+    return lut[col.data.long()]
+
+
+def sort_perm_table(t: DeviceTable, by: list, descending: list, want_image: bool = False):
+    """The permutation that puts `t` in ORDER BY by[0] [DESC], by[1] [DESC], ... order, NULLS LAST, rows that tie on every
+    column in their order in `t`: a chain of stable device sorts (qk_sort_perm), last column first.  want_image: also the
+    sorted order images of by[0] (int64 holding the uint64 bits) -> (perm, image)."""
+    perm, image = None, None
+    for i in range(len(by) - 1, -1, -1):
+        col = t[by[i]]
+        got = ops.sort_perm(_sort_key(col, by[i]), col.valid, bool(descending[i]), perm, want_image and i == 0)
+        perm, image = got if want_image and i == 0 else (got, None)
+    return (perm, image) if want_image else perm
+
+
+class SortExecutor(Executor):
+    """sql_executors.py:88-187 (SuperFastSortExecutor): ORDER BY over the whole stream, answered in done().  The reference
+    sorts every batch with Polars, spills the runs to disk and merges them on one channel; here the rows stay in HBM, every
+    rank sorts what it holds with the device radix sort and, across ranks, a sample sort leaves rank r with the r-th RANGE
+    of the first sort column -- the layout of a range-partitioned sorted reader, which the ordered operators (as-of join
+    over time ranges, windows, pattern search) consume as it is:
+      * every rank takes SAMPLES_PER_RANK * world regularly spaced (image, NULL) samples of its sorted run; all ranks sort
+        the same samples and cut them at the same world - 1 splitters;
+      * a row goes to rank #{splitters <= its first-column image}, so all rows of one first-column value land on one rank
+        (one value that holds most of the rows makes that rank hold most of the rows); the run is sorted, so every
+        destination is one contiguous slice;
+      * the received runs, in source-rank order, are sorted once more (stable: ties keep source rank, then arrival order).
+    Multi-column, per-column direction, stable, NULLS LAST.  Everything must fit in device memory: nothing is spilled."""
+
+    silent_streams = "all"
+    ordered_output = True            # rank r's rows precede rank r + 1's on the first sort column
+    SAMPLES_PER_RANK = 64
+
+    def __init__(self, columns, descending) -> None:
+        self.columns, self.descending = list(columns), [bool(d) for d in descending]
+        self._batches = []
+        self.state = None
+
+    def explain(self) -> str:
+        return "sort " + ", ".join(c + (" desc" if d else "") for c, d in zip(self.columns, self.descending))
+
+    def execute(self, batches, stream_id, executor_id):
+        self._batches.extend(_clean(batches))
+
+    def _sorted(self, t: DeviceTable):
+        perm, image = sort_perm_table(t, self.columns, self.descending, want_image=True)
+        return t.gather(perm), image
+
+    def done(self, executor_id):
+        from . import runtime as RT
+        t, self._batches = (concat_tables(self._batches) if self._batches else None), []
+        w = RT.world_size()
+        if w == 1:
+            self.state = self._sorted(t)[0] if t is not None else None
+            return self.state
+        me, dev, first = RT.rank(), default_device(), self.columns[0]
+        ex = RT.Exchange(dev)
+        if t is not None and t[first].dictionary is not None:
+            # string first column: the ranks compare images, so they need one dictionary -- every rank's entries to everybody
+            d = t[first].dictionary
+            entries = DeviceTable({first: DeviceColumn(torch.arange(len(d), device=dev).to(t[first].data.dtype), d)})
+        else:
+            entries = None
+        has_dict = max(r[0] for r in ex.allgather_words([int(entries is not None)]))
+        if has_dict:
+            got = ex({r: entries for r in range(w)} if entries is not None else {}, w, edge_key=("sort-dictionary", id(self)))
+            if entries is not None:
+                union = DeviceColumn(torch.empty(0, dtype=t[first].data.dtype, device=dev), got[0][first].dictionary)
+                t = t.with_column(first, unify_dictionaries([t[first], union])[1][0])
+        run, image = self._sorted(t) if t is not None else (None, None)
+        # ---- the same samples on every rank: signed images (image ^ sign bit, so int64 order is image order) + NULL flags
+        samples = None
+        if run is not None:
+            n, s = len(run), self.SAMPLES_PER_RANK * w
+            at = (torch.arange(s, device=dev, dtype=torch.int64) * n + n // 2) // s if n > s else torch.arange(n, device=dev)
+            fv = run[first].valid
+            null = (fv[at] == 0).to(torch.uint8) if fv is not None else torch.zeros(len(at), dtype=torch.uint8, device=dev)
+            samples = DeviceTable({"image": DeviceColumn(image[at] ^ _SIGN_I64), "null": DeviceColumn(null)})
+        got = ex({r: samples for r in range(w)} if samples is not None else {}, w, edge_key=("sort-samples", id(self)))
+        if not got:
+            return None
+        allsamp = concat_tables(sorted(got, key=lambda g: g.src_rank))
+        order = ops.sort_perm(allsamp["image"].data.contiguous(), (1 - allsamp["null"].data).contiguous(), False)
+        cut = order[(torch.arange(1, w, device=dev) * len(order)) // w].long()
+        split_img, split_null = allsamp["image"].data[cut], allsamp["null"].data[cut].tolist()
+        # ---- my run's slice for every rank: rows whose image is below splitter r stay left of it; NULLs are past every value
+        parts, own = {}, None
+        if run is not None:
+            fv = run[first].valid
+            nvalid = len(run) if fv is None else int(fv.sum().item())      # NULLS LAST: the run's valid rows come first
+            pos = torch.searchsorted(image[:nvalid] ^ _SIGN_I64, split_img).tolist()
+            bounds = [0] + [nvalid if isnull else p for p, isnull in zip(pos, split_null)] + [len(run)]
+            parts = {r: run.slice(bounds[r], bounds[r + 1]) for r in range(w) if r != me and bounds[r + 1] > bounds[r]}
+            own = run.slice(bounds[me], bounds[me + 1])
+        mine = list(ex(parts, w, edge_key=("sort-rows", id(self))))
+        if own is not None and len(own) > 0:
+            own.src_rank = me
+            mine.append(own)
+        if not mine:
+            return None
+        self.state = self._sorted(concat_tables(sorted(mine, key=lambda g: g.src_rank)))[0]
         return self.state
 
 

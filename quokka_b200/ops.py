@@ -503,6 +503,35 @@ def topk_candidates(key: torch.Tensor, k: int, descending: bool):
     return idx[:int(cnt.item())]
 
 
+# ------------------------------------------------------------------ K13 sort
+def sort_perm(key: torch.Tensor, valid: torch.Tensor | None, descending: bool, perm_in: torch.Tensor | None = None,
+              want_image: bool = False):
+    """Stable sort of one key column to a permutation (qk_sort_perm): perm[i] = the row of `key` at sorted position i, int32.
+    valid (uint8 per row, or None): rows with 0 come last in both directions.  perm_in (int32 permutation, or None =
+    identity): the order equal keys keep, so a multi-column sort chains calls from the last column to the first.
+    want_image: also the sorted order images as int64 tensors holding the uint64 bits -> (perm, image)."""
+    n = key.numel()
+    if n > 0x7fffffff:
+        raise L.QkError("sort_perm: more than 2^31 - 1 rows")
+    kc = col(key, "sort key")
+    for t, what, dt in ((valid, "sort validity mask", torch.uint8), (perm_in, "sort input permutation", torch.int32)):
+        if t is not None:
+            _require_cuda(t, what)
+            if t.dtype != dt or t.numel() != n:
+                raise L.QkError(f"sort_perm: the {what} must be {dt} with one entry per row")
+    perm = torch.empty(n, dtype=torch.int32, device=key.device)
+    image = torch.empty(n, dtype=torch.int64, device=key.device) if want_image else None
+    ws = _ws(L.lib().qk_sort_workspace_bytes(n), key.device)
+    L.check(L.lib().qk_sort_perm(C.byref(kc), valid.data_ptr() if valid is not None else None, 1 if descending else 0,
+                                 perm_in.data_ptr() if perm_in is not None else None, perm.data_ptr(),
+                                 image.data_ptr() if want_image else None, n, ws.data_ptr(), ws.numel(), _stream()), "qk_sort_perm")
+    return (perm, image) if want_image else perm
+
+
+def sort_last_plan() -> str:
+    return L.lib().qk_sort_last_plan().decode()
+
+
 # ------------------------------------------------------------------ K9 Gram matrix
 class GramState:
     """Running Gram matrix of a stream of k-column batches (qk_gram): gram = sum (X - c)^T (X - c) (fp64 [k, k]),

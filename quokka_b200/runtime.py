@@ -575,6 +575,7 @@ class TaskGraph:
         single = isinstance(placement_strategy, SingleChannelStrategy)
         a = _Actor(self.current_actor, "exec", functionObject, stage, single)
         a.blocking = blocking
+        a.ordered = bool(getattr(functionObject, "ordered_output", False))     # a sort: rank r's output precedes rank r + 1's
         for stream_id, src in streams.items():
             ti = source_target_info.get(stream_id) if source_target_info else None
             if ti is None:
@@ -796,6 +797,7 @@ class TaskGraph:
         lines = []
         for a in sorted(self.actors.values(), key=lambda a: (a.stage if a.kind == "input" else 1 << 30, a.id)):
             what = type(a.obj).__name__ + (" [single channel]" if a.single else "") + (" [sink]" if a.blocking else "")
+            what += " [ordered]" if a.kind == "exec" and a.ordered else ""
             lines.append(f"actor {a.id}: {what}" + (f"  stage {a.stage}" if a.kind == "input" else ""))
             for tgt, sid, ti in a.targets:
                 e = ti.edge_ops
