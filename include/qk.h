@@ -515,6 +515,37 @@ QK_API int qk_sort_perm(const qk_column* key, const uint8_t* valid, int32_t desc
                         uint64_t* image_out, int64_t nrows, void* workspace, size_t workspace_bytes, void* stream);
 QK_API const char* qk_sort_last_plan(void);
 
+/* ---- K14: lag / lead per key over a stream in order -----------------------------------------------------------------
+ * Stands in for OrderedStream.shift(n, by, fill_value) (pyquokka/orderedstream.py:13-35), whose ShiftOperator the reference
+ * imports and never defines; the semantics are Polars' pl.all().shift(n, fill_value).over(by).
+ * qk_shift_plan: rows 0 .. nrows-1 in stream order.  by = device int32 codes in [0, n_by), with dest / seg the output of
+ * qk_partition_plan(by, n_by, QK_PART_CODE) (stable); or all three NULL: one key.  For each row i in [lo, hi), src[i - lo]
+ * (device int32) receives the row n places EARLIER in i's key (n > 0, a lag) or |n| places LATER (n < 0, a lead), or -1 when
+ * there is none; n == 0 gives the row itself, |n| >= 2^31 no row.  Source rows are numbered from lo: row r is reported as
+ * r - lo for r >= lo and r - lo + nrows below lo, so a caller that puts other ranks' rows in front of its own ([B | A], lo =
+ * rows of B) gets A's rows as [0, n_a) and B's after them -- the numbering qk_shift_gather reads.
+ * edge (device uint8[nrows] or NULL): 1 for the rows among the last n (lag) / first |n| (lead) rows of their key: the rows a
+ * later (earlier) rank needs.  time (device int64[nrows] or NULL): *status (device uint64, zeroed by the call) receives the
+ * number of rows whose time is below that of the previous row of their key -- the order check, in the same pass.
+ * Workspace: qk_shift_workspace_bytes(nrows) (the inverse permutation; unused without by).  Two launches with by, one without.
+ * Errors: nrows > 2^31 - 1: QK_ERR_UNSUPPORTED; by / dest / seg not all given or all NULL, [lo, hi) outside the rows, null src
+ * with hi > lo, time without status: QK_ERR_INVALID; workspace too small: QK_ERR_CAPACITY.
+ * qk_shift_gather: out[c][i] for i < nrows, all shifted columns in one launch: src[i] in [0, n_a) reads a_cols[c] (n_a =
+ * a_cols[0].length, the rank's own rows), src[i] in [n_a, n_a + n_b) reads b_cols[c] (the boundary rows of other ranks), -1
+ * writes the fill value: the low dtype_size bytes of fill[c] (HOST uint64 array).  Validity: a_valid / b_valid are NULL or HOST
+ * arrays of ncols device uint8 masks (an entry may be NULL = all valid); out_valid is NULL or a HOST array of ncols device
+ * uint8[nrows] outputs (an entry may be NULL: not written), receiving fill_valid[c] (HOST uint8 array) for -1 and the source
+ * row's validity otherwise.  Scalar QK_U8 / QK_I32 / QK_I64 / QK_F32 / QK_F64 columns, b_cols[c] of a_cols[c]'s dtype, at most
+ * QK_MAX_COLS columns.  Errors: a vector column: QK_ERR_UNSUPPORTED; mismatched dtypes or lengths: QK_ERR_INVALID; a short
+ * output: QK_ERR_CAPACITY. */
+QK_API size_t qk_shift_workspace_bytes(int64_t nrows);
+QK_API int qk_shift_plan(const int32_t* by, int32_t n_by, const int32_t* dest, const int64_t* seg, int64_t nrows, int64_t n,
+                         int64_t lo, int64_t hi, int32_t* src, uint8_t* edge, const int64_t* time, uint64_t* status,
+                         void* workspace, size_t ws_bytes, void* stream);
+QK_API int qk_shift_gather(const qk_column* a_cols, const qk_column* b_cols, int32_t ncols, const uint8_t* const* a_valid,
+                           const uint8_t* const* b_valid, const uint64_t* fill, const uint8_t* fill_valid, const int32_t* src,
+                           int64_t nrows, int64_t n_b, qk_column* out, uint8_t* const* out_valid, void* stream);
+
 /* ---- synthetic TPC-H-shaped / SIP-shaped columns, generated in HBM --------------------------
  * Bit-identical to oracle/tpch_gen.py (counter-based hash of (table, column, row)); lets bench.py hold
  * SF-100 (600 037 902 lineitem rows) resident without a 23 GB host copy.  `column` ids: see

@@ -155,6 +155,11 @@ _SIGNATURES = {
     "qk_sort_perm": (C.c_int, [_P(qk_column), C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                C.c_size_t, C.c_void_p]),
     "qk_sort_last_plan": (C.c_char_p, []),
+    "qk_shift_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "qk_shift_plan": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
+                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "qk_shift_gather": (C.c_int, [_P(qk_column), _P(qk_column), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_int64, C.c_int64, _P(qk_column), C.c_void_p, C.c_void_p]),
     "qk_synth_column": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_int64), C.c_int64, C.c_int64, C.c_void_p,
                                   C.c_int32, C.c_void_p]),
     "qk_parquet_walk_chunk": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

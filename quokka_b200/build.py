@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libqk.so")
-SOURCES = ["abi.cu", "offsets.cu", "synth.cu", "scan.cu", "compact.cu", "partition.cu", "exchange.cu", "join.cu", "hashagg.cu", "asof.cu", "window.cu", "topk.cu", "parquet.cu", "gram.cu", "quantile.cu", "knn.cu", "pattern.cu", "sort.cu"]
+SOURCES = ["abi.cu", "offsets.cu", "synth.cu", "scan.cu", "compact.cu", "partition.cu", "exchange.cu", "join.cu", "hashagg.cu", "asof.cu", "window.cu", "topk.cu", "parquet.cu", "gram.cu", "quantile.cu", "knn.cu", "pattern.cu", "sort.cu", "shift.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-std=c++17", *GENCODE, "-lineinfo", "-O3",
               # no FMA contraction: projected fp64 columns are bit-identical to the numpy oracle

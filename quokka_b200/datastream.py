@@ -190,10 +190,11 @@ class SortNode(Node):
 
 
 def ends_in_sort(node: Node) -> bool:
-    """True when the rows of `node` are a sort's output seen through row-wise operators (filter / select / rename / map)."""
+    """True when the rows of `node` are a sort's output seen through row-wise operators (filter / select / rename / map), or
+    the output of an executor that keeps its rows in stream order (`ordered_output`, e.g. shift)."""
     while node.kind in ("filter", "select", "rename", "map"):
         node = node.parents[0]
-    return node.kind == "sort"
+    return node.kind == "sort" or (node.kind == "stateful" and bool(getattr(node.executor, "ordered_output", False)))
 
 
 class DistinctNode(Node):
@@ -1042,6 +1043,53 @@ class OrderedStream(DataStream):
             raise Exception("unknown window type")
         node = StatefulNode({0: self.node}, operator, new_schema, {0: sorted(required)}, {0: HashPartitioner(by_col)}, CustomChannelsStrategy(1))
         return OrderedStream(self.quokka_context, node, time_col)
+
+    def shift(self, n, by=None, fill_value=None, columns=None, suffix=None):
+        """Lag / lead per key (pyquokka/orderedstream.py:13-35; the reference never implements its ShiftOperator, so this
+        follows Polars' pl.all().shift(n, fill_value).over(by)).  Stream order is the order collect() returns: rank order, then
+        arrival order within a rank -- the sort order after sort() and sorted readers.  For n > 0 every row receives the values
+        of the row n places earlier among the rows of its `by` key (n < 0: |n| places later); by=None makes the whole stream one
+        key; n = 0 leaves the values as they are.  Rows without such a row get `fill_value`: None gives NULL, a scalar fills
+        every shifted column, a {column: value} dict fills per column (columns it does not name get NULL).  The value is
+        converted to the column's type (int, float, bool, datetime.date, datetime.datetime or an int in the column's unit, str
+        for string columns, where it joins the dictionary); one the column cannot hold raises QkError.  NULL values move as
+        NULL.  `by` is a string column or non-negative integer codes.
+        Deviations from the reference's form shift(n, by, fill_value), which shifts every column in place:
+          * `columns`: the columns whose values move (default: every column but `by`, which cannot be listed; a vector column
+            raises NotImplementedError);
+          * `suffix`: None shifts in place (the schema is unchanged); a string appends the shifted copies as c + suffix after
+            the schema and keeps the originals, so shift(1, by="symbol", columns=["bid"], suffix="_prev") followed by
+            with_columns_sql("bid - bid_prev as d") computes a difference per key.
+        Every row stays where it was (same rank, same position).  The result is sorted by what this stream is sorted by, unless
+        that column is shifted in place.  When the sort column is an integer, date or timestamp column, a key whose rows are
+        not in order in it raises QkError.  The rank's input must fit in device memory."""
+        from .executors import ShiftExecutor
+        assert type(n) == int, "n must be an int"
+        assert by is None or by in self.schema, f"shift: by column {by!r} not in schema"
+        if columns is None:
+            columns = [c for c in self.schema if c != by]
+        else:
+            columns = [columns] if isinstance(columns, str) else list(columns)
+            assert all(c in self.schema for c in columns), "shift: columns must be in the schema"
+            assert len(set(columns)) == len(columns), "shift: columns must be distinct"
+            assert by is None or by not in columns, "shift: the by column cannot be shifted"
+        assert len(columns) > 0, "shift: no column to shift"
+        if by is not None:
+            _reject_vectors(self.node.vectors, [by], "shift key")
+        _reject_vectors(self.node.vectors, columns, "shift")
+        if isinstance(fill_value, dict):
+            assert all(c in columns for c in fill_value), "shift: fill_value names a column that is not shifted"
+        schema = list(self.schema)
+        if suffix is not None:
+            assert isinstance(suffix, str) and suffix, "shift: suffix must be a non-empty string"
+            for c in columns:
+                if c + suffix in schema:
+                    raise L.QkError(f"shift: column {c + suffix!r} would be duplicated; pick another suffix")
+                schema.append(c + suffix)
+        ex = ShiftExecutor(n, by, fill_value, columns, suffix, self.sorted_by)
+        node = StatefulNode({0: self.node}, ex, schema, {0: set(self.schema)}, {0: PassThroughPartitioner()}, CustomChannelsStrategy(1))
+        sorted_by = None if suffix is None and self.sorted_by in columns else self.sorted_by
+        return OrderedStream(self.quokka_context, node, sorted_by)
 
     def join_asof(self, right, on=None, left_on=None, right_on=None, by=None, left_by=None, right_by=None, suffix="_2"):
         """Backward as-of join by key (orderedstream.py:114-191); `by` is mandatory (:127-128); the right

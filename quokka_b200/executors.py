@@ -1652,3 +1652,235 @@ class CEPExecutor(_KeySegmented):
         for e, name in enumerate(self.names):
             out[name] = self._time_column(ops.gather([stime], bound[:, e].contiguous())[0], tcol)
         return DeviceTable(out)
+
+
+# ---------------------------------------------------------------------------------------------- shift (lag / lead)
+_INT_RANGE = {torch.uint8: (0, 255), torch.int32: (-(1 << 31), (1 << 31) - 1), torch.int64: (-(1 << 63), (1 << 63) - 1)}
+
+
+def shift_fill(col: DeviceColumn, name: str, value):
+    """`value` as column `name` stores it, for the rows of OrderedStream.shift without a source -> (the stored value, the
+    output dictionary).  None stays None (NULL); a string joins a copy of the column's dictionary when it is not in it yet.
+    A value the column cannot hold raises QkError."""
+    import datetime
+    import numbers
+    dictionary = col.dictionary
+    if value is None:
+        return None, dictionary
+    at, dt = col.arrow_type, col.data.dtype
+
+    def bad():
+        return L.QkError(f"shift: fill value {value!r} cannot be stored in column {name!r} ({at or dt})")
+    if dictionary is not None:
+        if not isinstance(value, str):
+            raise bad()
+        if value not in dictionary:
+            dictionary = list(dictionary) + [value]
+        return dictionary.index(value), dictionary
+    if at is not None and pa.types.is_boolean(at):
+        if not isinstance(value, bool):
+            raise bad()
+        return int(value), None
+    if isinstance(value, bool):
+        raise bad()
+    if at is not None and (pa.types.is_date(at) or pa.types.is_timestamp(at)):
+        if isinstance(value, numbers.Integral):                     # days / milliseconds / the timestamp's unit
+            v = int(value)
+        elif pa.types.is_timestamp(at) and isinstance(value, datetime.datetime):
+            try:
+                v = pa.scalar(value, type=at).value
+            except (pa.ArrowInvalid, pa.ArrowTypeError, OverflowError, ValueError):
+                raise bad() from None
+        elif pa.types.is_date(at) and isinstance(value, datetime.date) and not isinstance(value, datetime.datetime):
+            v = (value - datetime.date(1970, 1, 1)).days * (1 if pa.types.is_date32(at) else 86_400_000)
+        else:
+            raise bad()
+    elif dt in (torch.float32, torch.float64):
+        if not isinstance(value, numbers.Real):
+            raise bad()
+        return float(value), None
+    elif isinstance(value, numbers.Integral):
+        v = int(value)
+    else:
+        raise bad()
+    lo, hi = _INT_RANGE.get(dt, (1, 0))
+    if not lo <= v <= hi:
+        raise bad()
+    return v, None
+
+
+class ShiftExecutor(Executor):
+    """OrderedStream.shift (pyquokka/orderedstream.py:13-35; the reference never defines its ShiftOperator, so the semantics are
+    Polars' pl.all().shift(n, fill_value).over(by)): every row receives the values of `columns` from the row n places earlier
+    (n > 0) or |n| later (n < 0) among the rows of its `by` key in stream order -- rank order, then arrival order -- or the fill.
+    Rows stay where they are; answered in done().
+      * one rank: KeyCodes codes, the stable code partition, qk_shift_plan (source rows and the order check in one pass) and
+        qk_shift_gather (every shifted column in one launch).  Unshifted columns are passed on as they are.
+      * several ranks: each rank holds a contiguous piece of the stream (sort(), sorted readers, from_device(sorted_by=...), or a
+        hash edge on `by`), so nothing is shuffled.  A rank flags the last n rows of each of its keys (first |n| for a lead)
+        and sends them to every later (earlier) rank -- at most |n| x keys rows; it then plans over the key codes of
+        [earlier ranks' tails in rank order | own rows] (lead: [own rows | later ranks' heads]) and gathers the payload from
+        its shard and from that small boundary table.  A key with fewer than |n| rows on the neighbouring rank still finds its
+        rows, because the tails of ALL earlier ranks arrive.  String payload columns of the boundary table are re-coded onto
+        the shard's dictionary (new entries appended); the shard is not re-coded.
+    When `time_col` (the stream's sorted_by) is an integer, date or timestamp column, rows of a key whose time falls below the
+    previous row's raise QkError, across rank boundaries too (NULL times count as the largest, where sort() puts them)."""
+
+    silent_streams = "all"
+    ordered_output = True            # rows stay in place: rank r's rows precede rank r + 1's
+    HUGE = 1 << 31                   # |n| at or above this: no row has a source
+
+    def __init__(self, n, by, fill_value, columns, suffix=None, time_col=None) -> None:
+        self.n, self.by, self.fill_value, self.columns = int(n), by, fill_value, list(columns)
+        self.suffix, self.time_col = suffix, time_col
+        self._batches = []
+        self._codes = KeyCodes()
+        self.state = None
+
+    def explain(self) -> str:
+        return (f"shift n={self.n} by={self.by} columns={self.columns}" + (f" suffix={self.suffix}" if self.suffix else "")
+                + (f" checked on {self.time_col}" if self.time_col else ""))
+
+    def execute(self, batches, stream_id, executor_id):
+        self._batches.extend(_clean(batches))
+
+    def _fill_of(self, c):
+        return self.fill_value.get(c) if isinstance(self.fill_value, dict) else self.fill_value
+
+    def _time(self, t: DeviceTable):
+        """The column the order check reads as int64 (NULL = largest), or None when there is nothing to check."""
+        if self.time_col is None or self.time_col not in t:
+            return None
+        c = t[self.time_col]
+        if c.dictionary is not None or c.is_vector or c.data.dtype not in (torch.int32, torch.int64):
+            return None
+        time = c.data.to(torch.int64)
+        if c.valid is not None:
+            time = torch.where(c.valid.bool(), time, torch.full_like(time, (1 << 63) - 1))
+        return time
+
+    def _key_codes(self, t: DeviceTable) -> torch.Tensor:
+        col = t[self.by]
+        if col.dictionary is None and col.data.dtype not in (torch.uint8, torch.int32, torch.int64):
+            raise L.QkError(f"shift: `by` column {self.by!r} must be a string column or integer codes")
+        return self._codes.codes(col)
+
+    def _require_order(self, bad):
+        if bad:
+            raise L.QkError(f"shift: the stream is not sorted by {self.time_col}")
+
+    def _gather(self, t: DeviceTable, boundary: DeviceTable | None, src: torch.Tensor) -> DeviceTable:
+        a, b, av, bv, fills, dicts = [], [], [], [], [], []
+        for c in self.columns:
+            col = t[c]
+            if col.is_vector:
+                raise L.QkError(f"shift: column {c!r} is a vector column")
+            ad, bcol = col.data, boundary[c] if boundary is not None else None
+            bd, dic = (bcol.data if bcol is not None else None), col.dictionary
+            if dic is not None and bcol is not None and bcol.dictionary != dic:
+                dic = list(dic)                                       # the boundary's strings join the shard's dictionary
+                index = {v: i for i, v in enumerate(dic)}
+                lut = []
+                for v in bcol.dictionary:
+                    if v not in index:
+                        index[v] = len(dic)
+                        dic.append(v)
+                    lut.append(index[v])
+                bd = torch.tensor(lut or [0], dtype=torch.int64, device=ad.device)[bd.long()]
+            fill, dic = shift_fill(DeviceColumn(ad, dic, col.arrow_type), c, self._fill_of(c))
+            if dic is not None and len(dic) > 255 and ad.dtype == torch.uint8:
+                ad = ad.to(torch.int32)                               # codes past 255 need a wider column
+            if bd is not None and bd.dtype != ad.dtype:
+                bd = bd.to(ad.dtype)
+            a.append(ad)
+            b.append(bd)
+            av.append(col.valid)
+            bv.append(bcol.valid if bcol is not None else None)
+            fills.append(fill)
+            dicts.append(dic)
+        outs, valids = ops.shift_gather(a, b if boundary is not None else None, src, fills, av, bv)
+        cols = dict(t.columns)
+        for c, o, v, dic in zip(self.columns, outs, valids, dicts):
+            cols[c if self.suffix is None else c + self.suffix] = DeviceColumn(o, dic, t[c].arrow_type, v)
+        return DeviceTable(cols)
+
+    def done(self, executor_id):
+        t, self._batches = (concat_tables(self._batches) if self._batches else None), []
+        if world_size() > 1:
+            self.state = self._across_ranks(t)
+            return self.state
+        if t is None:
+            return None
+        if self.n == 0:
+            self.state = self._unchanged(t)
+            return self.state
+        nrows = len(t)
+        time = self._time(t)
+        if self.by is None:
+            src, _, bad = ops.shift_plan(self.n, nrows, time=time, device=t.device)
+        else:
+            codes = self._key_codes(t)
+            n_by = max(1, self._codes.n_by)
+            dest, seg = ops.partition_plan(codes, n_by, L.PART_CODE)
+            src, _, bad = ops.shift_plan(self.n, nrows, codes, n_by, dest, seg, time=time)
+        self._require_order(bad)
+        self.state = self._gather(t, None, src)
+        return self.state
+
+    def _unchanged(self, t: DeviceTable) -> DeviceTable:
+        if self.suffix is None:
+            return t
+        return DeviceTable(dict(t.columns) | {c + self.suffix: t[c] for c in self.columns})
+
+    def _across_ranks(self, t: DeviceTable | None):
+        from . import runtime as RT
+        w, me, dev = RT.world_size(), RT.rank(), default_device()
+        if self.n == 0:
+            return self._unchanged(t) if t is not None else None
+        ex = RT.Exchange(dev)
+        lag = self.n > 0
+        # a shift past 2^31 rows has no sources; the boundary then only serves the order check: one row per key
+        edge_n = self.n if abs(self.n) < self.HUGE else (1 if lag else -1)
+        na = len(t) if t is not None else 0
+        parts, codes, time = {}, None, None
+        if na:
+            time = self._time(t)
+            if self.by is not None:
+                codes = self._key_codes(t)
+                n_by = max(1, self._codes.n_by)
+                dest, seg = ops.partition_plan(codes, n_by, L.PART_CODE)
+                _, edge, _ = ops.shift_plan(edge_n, na, codes, n_by, dest, seg, lo=0, hi=0, want_edge=True)
+            else:
+                _, edge, _ = ops.shift_plan(edge_n, na, lo=0, hi=0, want_edge=True, device=t.device)
+            need = list(dict.fromkeys(self.columns + ([self.by] if self.by is not None else [])
+                                      + ([self.time_col] if time is not None else [])))
+            rows = torch.nonzero(edge).flatten().to(torch.int32)
+            if rows.numel():
+                boundary = t.select(need).gather(rows)
+                parts = {r: boundary for r in range(w) if (r > me if lag else r < me)}
+        got = sorted(ex(parts, w, edge_key=("shift-boundary", id(self))), key=lambda g: g.src_rank)
+        B = concat_tables(got) if got else None
+        nb = len(B) if B is not None else 0
+        bad = 0
+        if na:
+            lo = nb if lag else 0
+            allcodes = alltime = None
+            if nb and self.by is not None:
+                bcodes = self._key_codes(B)
+                allcodes = torch.cat([bcodes, codes] if lag else [codes, bcodes])
+            elif self.by is not None:
+                allcodes = codes
+            if time is not None:
+                btime = self._time(B) if nb else None
+                alltime = time if btime is None else torch.cat([btime, time] if lag else [time, btime])
+            if self.by is not None:
+                n_by = max(1, self._codes.n_by)
+                dest, seg = ops.partition_plan(allcodes, n_by, L.PART_CODE)
+                src, _, bad = ops.shift_plan(self.n, na + nb, allcodes, n_by, dest, seg, lo=lo, hi=lo + na, time=alltime)
+            else:
+                src, _, bad = ops.shift_plan(self.n, na + nb, lo=lo, hi=lo + na, time=alltime, device=t.device)
+        if any(r[0] for r in ex.allgather_words([int(bad or 0)])):          # every rank raises, or none does
+            self._require_order(1)
+        if not na:
+            return None
+        return self._gather(t, B if nb else None, src)

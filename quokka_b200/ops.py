@@ -532,6 +532,69 @@ def sort_last_plan() -> str:
     return L.lib().qk_sort_last_plan().decode()
 
 
+# ------------------------------------------------------------------ K14 shift
+def shift_plan(n: int, nrows: int, by: torch.Tensor | None = None, n_by: int = 0, dest: torch.Tensor | None = None,
+               seg: torch.Tensor | None = None, lo: int = 0, hi: int | None = None, want_edge: bool = False,
+               time: torch.Tensor | None = None, device=None):
+    """Source rows of a shift by `n` per key (qk_shift_plan) -> (src int32[hi - lo], edge uint8[nrows] or None, rows out of
+    order or None).  by: int32 codes with dest / seg of partition_plan(by, n_by, PART_CODE), or None for one key.  src numbers
+    the rows from lo (see include/qk.h).  time (int64 per row): count the rows below their key's previous row (one read-back)."""
+    hi = nrows if hi is None else hi
+    if nrows > 0x7fffffff:
+        raise L.QkError("shift_plan: more than 2^31 - 1 rows")
+    dev = by.device if by is not None else (time.device if time is not None else device)
+    for t, what, dt in ((by, "shift key codes", torch.int32), (dest, "shift partition", torch.int32), (time, "shift time", torch.int64)):
+        if t is not None:
+            _require_cuda(t, what)
+            if t.dtype != dt or t.numel() != nrows:
+                raise L.QkError(f"shift_plan: the {what} must be {dt} with one entry per row")
+    src = torch.empty(hi - lo, dtype=torch.int32, device=dev)
+    edge = torch.empty(nrows, dtype=torch.uint8, device=dev) if want_edge else None
+    if nrows == 0:
+        return src, edge, (0 if time is not None else None)
+    status = torch.zeros(1, dtype=torch.int64, device=dev) if time is not None else None
+    ws = _ws(L.lib().qk_shift_workspace_bytes(nrows) if by is not None else 0, dev)
+    p = lambda t: t.data_ptr() if t is not None and t.numel() else None
+    L.check(L.lib().qk_shift_plan(p(by), int(n_by), p(dest), p(seg), nrows, max(-(1 << 63), min(int(n), (1 << 63) - 1)), lo, hi,
+                                  p(src), p(edge), p(time), p(status), ws.data_ptr(), ws.numel(), _stream()), "qk_shift_plan")
+    return src, edge, (int(status.item()) if status is not None else None)
+
+
+def fill_bits(value, dtype: torch.dtype) -> int:
+    """The 8-byte word whose low bytes hold `value` stored as `dtype` (qk_shift_gather's fill)."""
+    raw = torch.tensor([value], dtype=dtype).numpy().tobytes()
+    return int.from_bytes(raw.ljust(8, b"\0"), "little")
+
+
+def shift_gather(a: Sequence[torch.Tensor], b: Sequence[torch.Tensor] | None, src: torch.Tensor, fills: Sequence,
+                 a_valid: Sequence[torch.Tensor | None] | None = None, b_valid: Sequence[torch.Tensor | None] | None = None):
+    """out[c][i] = a[c][src[i]] for src < len(a[c]), b[c][src[i] - len(a[c])] above, fills[c] for -1 (qk_shift_gather).  fills[c]
+    is a value of the column's dtype or None (NULL).  -> (outputs, validity masks: uint8 per row, or None where every output
+    row is valid)."""
+    nc, n = len(a), src.numel()
+    if nc == 0:
+        return [], []
+    dev = a[0].device
+    _require_cuda(src, "shift sources")
+    a_valid = list(a_valid) if a_valid is not None else [None] * nc
+    b_valid = list(b_valid) if b_valid is not None else [None] * nc
+    n_b = b[0].numel() if b else 0
+    outs = [torch.empty(n, dtype=t.dtype, device=dev) for t in a]
+    vouts = [torch.empty(n, dtype=torch.uint8, device=dev) if (fills[c] is None or a_valid[c] is not None or b_valid[c] is not None)
+             else None for c in range(nc)]
+    for lo in range(0, nc, L.MAX_COLS):
+        sl = slice(lo, min(nc, lo + L.MAX_COLS))
+        k = sl.stop - sl.start
+        ptrs = lambda ts: C.cast((C.c_void_p * k)(*[None if t is None else t.data_ptr() for t in ts[sl]]), C.c_void_p)
+        fill = (C.c_uint64 * k)(*[0 if f is None else fill_bits(f, t.dtype) for f, t in zip(fills[sl], a[sl])])
+        fvalid = (C.c_uint8 * k)(*[0 if f is None else 1 for f in fills[sl]])
+        L.check(L.lib().qk_shift_gather(cols(a[sl], "shift column"), cols(b[sl], "shift boundary column") if n_b else None, k,
+                                        ptrs(a_valid), ptrs(b_valid), C.cast(fill, C.c_void_p), C.cast(fvalid, C.c_void_p),
+                                        src.data_ptr() if n else None, n, n_b, cols(outs[sl], "output"), ptrs(vouts),
+                                        _stream()), "qk_shift_gather")
+    return outs, vouts
+
+
 # ------------------------------------------------------------------ K9 Gram matrix
 class GramState:
     """Running Gram matrix of a stream of k-column batches (qk_gram): gram = sum (X - c)^T (X - c) (fp64 [k, k]),
