@@ -1,21 +1,34 @@
 """TEST-ONLY stand-in for quokka_b200.ops so that the HOST logic (expression compiler, planner, edge
-functions, executors' protocol handling, the SPMD driver and the gloo exchange) can be exercised in the
-CPU build container.  Every function mirrors the signature of its quokka_b200.ops counterpart and is
-implemented with the numpy oracle; nothing here ships -- the product has no CPU path, and the same tests
-run against the real kernels on the GPU box (tests/test_gpu_api.py)."""
+functions, executors' protocol handling, the SPMD driver and the gloo exchange) can be exercised without a
+GPU.  Every function mirrors the signature of its quokka_b200.ops counterpart and is implemented with the
+numpy oracle; nothing here ships -- the product has no CPU path, and the same tests run against the real
+kernels on the GPU (tests/test_gpu_api.py).  The stand-ins of the feature kernels live in modules of their
+own (tests/<feature>_shim.py), which the GPU tests also compare the kernels against; this module's namespace
+holds them all, so one install serves every program.  tests/test_shim_surface.py checks that it covers ops."""
 from __future__ import annotations
 
 import numpy as np
 import torch
 
+from gram_shim import GramState, gram_last_plan
+from knn_shim import knn_merge, knn_topk
 from oracle import relops as R
+from pattern_shim import PatternBudgetError, pattern_search
+from quantile_shim import QuantileSketch
 from quokka_b200 import _lib as L
 from quokka_b200 import expr as E
 from quokka_b200 import ops as real_ops
 from quokka_b200.executors import order_image
+from shift_shim import shift_gather, shift_plan
+from sort_shim import sort_last_plan, sort_perm
+from xchg_shim import XchgChannel
 
+# host-only helpers of ops: they run as they are on CPU tensors
 qk_dtype = real_ops.qk_dtype
 is_passthrough = real_ops.is_passthrough
+dense_agg_fits = real_ops.dense_agg_fits
+fill_bits = real_ops.fill_bits
+qsketch_quantiles = real_ops.qsketch_quantiles
 
 
 def _t(a, like=None):
@@ -152,7 +165,7 @@ class DenseAggState:
         E.check_call(len(columns), pred, agg_exprs, "scan_filter_agg_dense")
         if len(group_cols) > 4 or len(self.agg_ops) > L.MAX_AGGS or self.n_groups > real_ops.DENSE_MAX_GROUPS:
             raise L.QkError("scan_filter_agg_dense: ngroup_cols / nagg / groups out of range")
-        if not real_ops.dense_agg_fits(self.n_groups, len(self.agg_ops)):
+        if not dense_agg_fits(self.n_groups, len(self.agg_ops)):
             raise L.QkError("scan_filter_agg_dense: groups x aggregates exceed the shared-memory dense path")
         cols = [c.numpy() for c in columns]
         n = len(cols[0]) if cols else 0

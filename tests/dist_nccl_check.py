@@ -1,8 +1,11 @@
-"""Multi-GPU parity run (real kernels + NCCL all-to-all): launched with
-    python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P tests/dist_nccl_check.py
-Each rank runs the same DataStream programs (api_cases) and checks the gathered result against the oracle."""
+"""Multi-GPU parity run (real kernels + NCCL all-to-all or the peer-memory link), launched by tests/ranks.py torchrun as
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P tests/dist_nccl_check.py SUITE...
+Each argument names a case list of tests/ranks.py SUITES (`api --more`, `sort`, `shift`, `knn`, `pattern`).  Every rank runs
+the same DataStream programs and checks the gathered result against the oracle; rank 0 prints `<case>: ok` after each case
+and the marker ranks.NCCL_MARKER at the end."""
 import os
 import sys
+import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
@@ -11,51 +14,20 @@ sys.path.insert(0, os.path.dirname(HERE))
 import torch
 import torch.distributed as dist
 
+import ranks
 
-def main():
+
+def main(suites):
     local = int(os.environ.get("LOCAL_RANK", "0"))
     torch.cuda.set_device(local)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    import api_cases as A
-    from quokka_b200.df import QuokkaContext
-    golden = os.path.join(HERE, "golden")
-    cases = ["case_q1_sql", "case_q1_dict_api", "case_q3", "case_q5", "case_join_kinds", "case_asof",
-             "case_executor_protocol", "case_misc_ops", "case_scalar_aggs", "case_string_key_join", "case_agg_types", "case_windows", "case_asof_reference_result"]
-    if "--more" in sys.argv:                        # programs added after round 1's last GPU session + the opt-in plans
-        cases += ["case_q6_and_semi_anti", "case_q10_q18", "case_q4_q12", "case_q14_q17_q19", "case_case_like_extract", "case_q7_q8",
-                  "case_custom_host_executor", "cb:case_q3", "cb:case_q5", "cbmix:case_q3", "cbmix:case_q10_q18",
-                  "case_q9_q11_q13", "case_q15_q16_q20_q22", "case_q2_q21", "case_string_funcs_and_nulls", "hash:case_asof", "asof_rank_shards:51", "hash:asof_rank_shards:52"]
-    for name in cases:
-        qc = QuokkaContext()
-        qc.set_config("broadcast_rows", 100)        # shuffle (and Bloom-reduce) every join even at test sizes
-        qc.set_config("broadcast_cost_based", False)    # ... unless the case asks for cost-based replication ("cb:")
-        if name.startswith("hash:"):                # as-of joins with both streams hash-shuffled by symbol (the reference's plan)
-            qc.set_config("asof_time_ranges", False)
-            name = name[5:]
-        if name.startswith("asof_rank_shards:"):    # every rank passes its own, independently cut slice of the sorted streams
-            import test_planner_random as TPR
-            TPR.run_asof_rank_shards(qc, int(name.split(":")[1]))
-            if dist.get_rank() == 0:
-                print(f"{name}: ok", flush=True)
-            continue
-        if name.startswith("cb"):                   # cost-based replication of build sides ("cbmix": only the small ones)
-            mode, name = name.split(":", 1)
-            qc.set_config("broadcast_cost_based", True)
-            if mode == "cbmix":
-                qc.set_config("broadcast_max_rows", 5000)
-        fn = getattr(A, name)
-        if name in ("case_join_kinds", "case_asof", "case_executor_protocol", "case_windows", "case_asof_reference_result"):
-            fn(qc, golden)
-        else:
-            fn(qc)
-        g = qc.last_graph
-        if dist.get_rank() == 0:
-            print(f"{name}: ok  (exchange calls {g.exchange.calls if g else 0}, via peer memory {g.exchange.peer_calls if g else 0}, bytes sent by rank 0 {g.exchange.bytes_sent if g else 0})", flush=True)
+    with tempfile.TemporaryDirectory() as files:
+        ranks.run_cases([n for s in suites for n in ranks.SUITES[s]], dist.get_rank(), dist.get_world_size(), files)
     dist.barrier()
     dist.destroy_process_group()
     if local == 0:
-        print("DIST_NCCL_OK", flush=True)
+        print(ranks.NCCL_MARKER, flush=True)
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1:])

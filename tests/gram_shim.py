@@ -1,14 +1,10 @@
-"""TEST-ONLY numpy stand-in for quokka_b200.ops.GramState (csrc/gram.cu), on top of tests/cpu_shim.py: `install(patch)` routes the
-kernels to cpu_shim as usual and gives the executors a view of it that also has GramState, so that DataStream.gramian /
+"""TEST-ONLY numpy stand-in for quokka_b200.ops.GramState (csrc/gram.cu), part of tests/cpu_shim.py, so that DataStream.gramian /
 covariance run through the planner, the executors and the gloo exchange without a GPU."""
 from __future__ import annotations
-
-import types
 
 import numpy as np
 import torch
 
-import cpu_shim
 from quokka_b200 import _lib as L
 
 
@@ -41,25 +37,3 @@ class GramState:
 
 def gram_last_plan():
     return "cpu-shim"
-
-
-class _Ops(types.ModuleType):
-    """cpu_shim plus the Gram state."""
-
-    GramState = GramState
-    gram_last_plan = staticmethod(gram_last_plan)
-
-    def __getattr__(self, name):
-        return getattr(cpu_shim, name)
-
-
-OPS = _Ops("gram_shim_ops")
-
-
-def install(patch):
-    """cpu_shim.install(patch), then the executors see OPS.  `patch.setattr(obj, name, value)`: pytest's monkeypatch or a plain
-    setter (the gloo workers)."""
-    cpu_shim.install(patch)
-    import quokka_b200.executors as X
-    patch.setattr(X, "ops", OPS)
-    return OPS

@@ -1,15 +1,11 @@
-"""TEST-ONLY numpy stand-ins for quokka_b200.ops.knn_topk / knn_merge (csrc/knn.cu), on top of tests/cpu_shim.py: `install(patch)`
-routes the kernels to cpu_shim as usual and gives the executors a view of it that also has the nearest-neighbour kernels, so that
+"""TEST-ONLY numpy stand-ins for quokka_b200.ops.knn_topk / knn_merge (csrc/knn.cu), part of tests/cpu_shim.py, so that
 DataStream.vector_nn_join runs through the planner, the executors and the gloo exchange without a GPU.  The gather and the
 exchange of 2-D columns are cpu_shim's own (numpy fancy indexing moves whole rows)."""
 from __future__ import annotations
 
-import types
-
 import numpy as np
 import torch
 
-import cpu_shim
 from quokka_b200 import _lib as L
 
 
@@ -62,25 +58,3 @@ def knn_merge(a_score, a_key, b_score, b_key, k):
                 os_[p, o], ok[p, o], src[p, o] = Bs[p, j], Bk[p, j], q * ka + p * kb + j
                 j += 1
     return torch.from_numpy(os_), torch.from_numpy(ok), torch.from_numpy(src)
-
-
-class _Ops(types.ModuleType):
-    """cpu_shim plus the nearest-neighbour kernels."""
-
-    knn_topk = staticmethod(knn_topk)
-    knn_merge = staticmethod(knn_merge)
-
-    def __getattr__(self, name):
-        return getattr(cpu_shim, name)
-
-
-OPS = _Ops("knn_shim_ops")
-
-
-def install(patch):
-    """cpu_shim.install(patch), then the executors see OPS.  `patch.setattr(obj, name, value)`: pytest's monkeypatch or a plain
-    setter (the gloo workers)."""
-    cpu_shim.install(patch)
-    import quokka_b200.executors as X
-    patch.setattr(X, "ops", OPS)
-    return OPS

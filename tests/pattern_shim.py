@@ -1,5 +1,4 @@
-"""TEST-ONLY numpy stand-in for quokka_b200.ops.pattern_search (csrc/pattern.cu), on top of tests/cpu_shim.py, in the style of
-tests/knn_shim.py: `install(patch)` gives the executors a view of cpu_shim that also has the pattern search, so that
+"""TEST-ONLY numpy stand-in for quokka_b200.ops.pattern_search (csrc/pattern.cu), part of tests/cpu_shim.py, so that
 OrderedStream.pattern_recognize runs through the planner, the executors and the gloo exchange without a GPU.
 
 The search is the kernel's, row by row: the level scan (candidate bit, t > t(i-1), t <= t0 + maxspan, the link program), the
@@ -7,12 +6,9 @@ resume after the bound row, the end of a level no later program reads, the caps 
 budget.  tests/pattern_cases.py's brute-force enumeration is what it is checked against."""
 from __future__ import annotations
 
-import types
-
 import numpy as np
 import torch
 
-import cpu_shim
 from quokka_b200 import _lib as L
 from quokka_b200 import expr as E
 from quokka_b200.ops import PatternBudgetError
@@ -129,25 +125,3 @@ def pattern_search(time, by, seg, n_by, cand, starts, m, maxspan, link_cols, lin
     if over:
         raise PatternBudgetError(f"pattern_search: {over} start(s) tested more than {budget} rows; the first is start {first}", first)
     return torch.from_numpy(out)
-
-
-class _Ops(types.ModuleType):
-    """cpu_shim plus the pattern search."""
-
-    pattern_search = staticmethod(pattern_search)
-    PatternBudgetError = PatternBudgetError
-
-    def __getattr__(self, name):
-        return getattr(cpu_shim, name)
-
-
-OPS = _Ops("pattern_shim_ops")
-
-
-def install(patch):
-    """cpu_shim.install(patch), then the executors see OPS.  `patch.setattr(obj, name, value)`: pytest's monkeypatch or a plain
-    setter (the gloo workers)."""
-    cpu_shim.install(patch)
-    import quokka_b200.executors as X
-    patch.setattr(X, "ops", OPS)
-    return OPS

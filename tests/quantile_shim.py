@@ -1,17 +1,11 @@
-"""TEST-ONLY numpy stand-in for quokka_b200.ops.QuantileSketch (csrc/quantile.cu), on top of tests/cpu_shim.py and
-tests/gram_shim.py: `install(patch)` routes the kernels to cpu_shim as usual and gives the executors a view of it that also
-has GramState and QuantileSketch, so that DataStream.approximate_quantile (and the clip -> covariance pipeline after it)
-runs through the planner, the executors and the gloo exchange without a GPU.  The sketch is tests/quantile_cases.py's
-numpy restatement; the answers come from the product's own qsketch_quantiles (torch only)."""
+"""TEST-ONLY numpy stand-in for quokka_b200.ops.QuantileSketch (csrc/quantile.cu), part of tests/cpu_shim.py, so that
+DataStream.approximate_quantile runs through the planner, the executors and the gloo exchange without a GPU.  The sketch is
+tests/quantile_cases.py's numpy restatement; the answers come from the product's own qsketch_quantiles (torch only)."""
 from __future__ import annotations
-
-import types
 
 import numpy as np
 import torch
 
-import cpu_shim
-import gram_shim
 import quantile_cases as QC
 from quokka_b200 import _lib as L
 from quokka_b200 import ops as real_ops
@@ -63,26 +57,3 @@ class QuantileSketch:
 
     def quantiles(self, qs):
         return real_ops.qsketch_quantiles(*self.entries(), self.k, qs)
-
-
-class _Ops(types.ModuleType):
-    """cpu_shim plus the Gram state and the quantile sketch."""
-
-    GramState = gram_shim.GramState
-    gram_last_plan = staticmethod(gram_shim.gram_last_plan)
-    QuantileSketch = QuantileSketch
-
-    def __getattr__(self, name):
-        return getattr(cpu_shim, name)
-
-
-OPS = _Ops("quantile_shim_ops")
-
-
-def install(patch):
-    """cpu_shim.install(patch), then the executors see OPS.  `patch.setattr(obj, name, value)`: pytest's monkeypatch or a
-    plain setter (the gloo workers)."""
-    cpu_shim.install(patch)
-    import quokka_b200.executors as X
-    patch.setattr(X, "ops", OPS)
-    return OPS

@@ -1,15 +1,11 @@
-"""TEST-ONLY numpy stand-ins for quokka_b200.ops.shift_plan / shift_gather (csrc/shift.cu), on top of tests/sort_shim.py:
-`install(patch)` routes the kernels to the shims as sort_shim does and gives the executors a view that also shifts, so
+"""TEST-ONLY numpy stand-ins for quokka_b200.ops.shift_plan / shift_gather (csrc/shift.cu), part of tests/cpu_shim.py, so
 OrderedStream.shift runs through the planner, the executors and the gloo exchange without a GPU.  The limits are the kernel's:
 int32 row numbers, the five scalar dtypes."""
 from __future__ import annotations
 
-import types
-
 import numpy as np
 import torch
 
-import sort_shim
 from quokka_b200 import _lib as L
 
 _DTYPES = (torch.uint8, torch.int32, torch.int64, torch.float32, torch.float64)
@@ -79,24 +75,3 @@ def shift_gather(a, b, src, fills, a_valid=None, b_valid=None):
         else:
             vouts.append(None)
     return outs, vouts
-
-
-class _Ops(types.ModuleType):
-    """sort_shim's view of the kernels plus the shift."""
-
-    shift_plan = staticmethod(shift_plan)
-    shift_gather = staticmethod(shift_gather)
-
-    def __getattr__(self, name):
-        return getattr(sort_shim.OPS, name)
-
-
-OPS = _Ops("shift_shim_ops")
-
-
-def install(patch):
-    """sort_shim.install(patch), then the executors see OPS."""
-    sort_shim.install(patch)
-    import quokka_b200.executors as X
-    patch.setattr(X, "ops", OPS)
-    return OPS

@@ -145,6 +145,23 @@ def case_sort_then_pattern(qc, golden_dir):
     _frames_equal(got, exp)
 
 
+def case_sort_then_quantile_and_gram(qc):
+    """A sorted stream feeding the quantile sketch and the Gram state gives the answers of the same programs without the sort:
+    the sketch bit for bit, the Gram matrix within the summation bound of tests/gram_cases.py."""
+    import gram_cases as GC
+    rng = np.random.default_rng(29)
+    n = 9_001
+    cols = {"a": rng.normal(3e4, 5.0, n), "b": rng.integers(-1000, 1000, n),
+            "c": rng.normal(-2.0, 1e-3, n).astype(np.float32)}
+    names = list(cols)
+    d = qc.from_arrow(pa.table(cols))
+    qs = [0.0, 0.1, 0.5, 0.9, 1.0]
+    assert d.sort("b").approximate_quantile(names, qs).collect().equals(d.approximate_quantile(names, qs).collect())
+    g, bound = GC.gram_ref(np.stack([cols[c].astype(np.float64) for c in names], axis=1))
+    for s in (d, d.sort("b", descending=True)):
+        GC.assert_within(GC.table_matrix(s.gramian(names).collect(), names), g, bound, "gramian")
+
+
 def case_sort_ranges(qc):
     """What the ranks hold after the sort: each is sorted, rank r's first-column values all precede rank r + 1's, no value is on
     two ranks -- also when a rank has no rows and when every row has the same value (one rank gets everything)."""

@@ -1,17 +1,11 @@
-"""TEST-ONLY numpy stand-in for quokka_b200.ops.sort_perm (csrc/sort.cu), on top of tests/cpu_shim.py and
-tests/pattern_shim.py: `install(patch)` routes the kernels to cpu_shim as usual and gives the executors a view of it that also
-sorts (and searches patterns), so that DataStream.sort and what is built on it -- join_asof, windowed_transform,
-pattern_recognize over a sorted stream -- run through the planner, the executors and the gloo exchange without a GPU.  The
-limits are the kernel's: the five scalar dtypes, int32 row numbers."""
+"""TEST-ONLY numpy stand-in for quokka_b200.ops.sort_perm (csrc/sort.cu), part of tests/cpu_shim.py, so that DataStream.sort
+and what is built on it -- join_asof, windowed_transform, pattern_recognize over a sorted stream -- run through the planner,
+the executors and the gloo exchange without a GPU.  The limits are the kernel's: the five scalar dtypes, int32 row numbers."""
 from __future__ import annotations
-
-import types
 
 import numpy as np
 import torch
 
-import cpu_shim
-import pattern_shim
 from quokka_b200 import _lib as L
 from quokka_b200.executors import order_image
 
@@ -37,24 +31,5 @@ def sort_perm(key, valid, descending, perm_in=None, want_image=False):
     return (perm, torch.from_numpy(img[order].view(np.int64).copy())) if want_image else perm
 
 
-class _Ops(types.ModuleType):
-    """cpu_shim plus the pattern search and the sort."""
-
-    sort_perm = staticmethod(sort_perm)
-    pattern_search = staticmethod(pattern_shim.pattern_search)
-    PatternBudgetError = pattern_shim.PatternBudgetError
-
-    def __getattr__(self, name):
-        return getattr(cpu_shim, name)
-
-
-OPS = _Ops("sort_shim_ops")
-
-
-def install(patch):
-    """cpu_shim.install(patch), then the executors see OPS.  `patch.setattr(obj, name, value)`: pytest's monkeypatch or a plain
-    setter (the gloo workers)."""
-    cpu_shim.install(patch)
-    import quokka_b200.executors as X
-    patch.setattr(X, "ops", OPS)
-    return OPS
+def sort_last_plan():
+    return "cpu-shim"

@@ -1,8 +1,10 @@
 """bench.py's DataStream legs (Q3, Q5, as-of, Parquet) run end to end on the numpy kernel shim with the oracle
 generator standing in for the CUDA generator: the Python of the benchmark -- program construction, timing loop,
 result fields, flags -- is exercised in the CPU container; the numbers it prints here mean nothing."""
+import importlib.util
 import os
 import sys
+import time
 import types
 
 import numpy as np
@@ -12,7 +14,8 @@ import torch
 import cpu_shim
 from oracle import tpch_gen as G
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
 
 
 def install(patch):
@@ -40,6 +43,22 @@ def install(patch):
     patch.setattr(synth, "ticks", ticks)
     import bench
     return bench
+
+
+def load_tool(name):
+    """tools/<name>.py as a module."""
+    spec = importlib.util.spec_from_file_location(name, os.path.join(ROOT, "tools", f"{name}.py"))
+    tool = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(tool)
+    return tool
+
+
+def cpu_ms(fn, reps):
+    """The host-clock stand-in of the tools' event_ms."""
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        fn()
+    return max((time.perf_counter() - t0) * 1e3 / reps, 1e-6)
 
 
 @pytest.fixture

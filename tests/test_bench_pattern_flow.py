@@ -1,23 +1,11 @@
-"""tools/bench_pattern.py end to end on the numpy shims (tests/cpu_shim.py + tests/pattern_shim.py) at a tiny size: argument
+"""tools/bench_pattern.py end to end on the numpy shim (tests/cpu_shim.py) at a tiny size: argument
 parsing, the quantile thresholds, both legs, the one-pass bytes and the host arm's agreement checks (restated search, oracle).  The numbers it prints here
 mean nothing."""
-import importlib.util
-import os
-import time
-
 import numpy as np
 import torch
 
-import pattern_shim
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _cpu_ms(fn, reps):
-    t0 = time.perf_counter()
-    for _ in range(reps):
-        fn()
-    return (time.perf_counter() - t0) * 1e3 / reps
+import cpu_shim
+import test_bench_flow as TBF
 
 
 def _quotes(n, n_symbols, dev):
@@ -31,12 +19,10 @@ def _quotes(n, n_symbols, dev):
 
 
 def test_bench_pattern_tiny_on_the_shim(monkeypatch):
-    ops = pattern_shim.install(monkeypatch)
-    spec = importlib.util.spec_from_file_location("bench_pattern", os.path.join(ROOT, "tools", "bench_pattern.py"))
-    bp = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(bp)
-    monkeypatch.setattr(bp, "ops", ops)
-    monkeypatch.setattr(bp, "event_ms", _cpu_ms)
+    cpu_shim.install(monkeypatch)
+    bp = TBF.load_tool("bench_pattern")
+    monkeypatch.setattr(bp, "ops", cpu_shim)
+    monkeypatch.setattr(bp, "event_ms", TBF.cpu_ms)
     monkeypatch.setattr(bp, "card", lambda: "cpu")
     monkeypatch.setattr(bp, "quotes", _quotes)
     out = bp.main(["--rows", "3000", "--symbols", "7", "--reps", "1", "--sample", "1200"], dev=torch.device("cpu"))

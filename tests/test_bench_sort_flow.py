@@ -1,37 +1,21 @@
-"""tools/bench_sort.py end to end on the numpy shims (tests/cpu_shim.py + tests/sort_shim.py) with the oracle generator standing in
+"""tools/bench_sort.py end to end on the numpy shim (tests/cpu_shim.py) with the oracle generator standing in
 for the CUDA generator: argument parsing, every leg, the byte model and the check fields.  The numbers it prints here mean
 nothing; run as a program without a GPU it fails."""
-import importlib.util
 import os
 import subprocess
 import sys
-import time
 
 import pytest
 import torch
 
-import sort_shim
+import cpu_shim
 import test_bench_flow as TBF
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _cpu_ms(fn, reps):
-    t0 = time.perf_counter()
-    for _ in range(reps):
-        fn()
-    return max((time.perf_counter() - t0) * 1e3 / reps, 1e-6)
-
-
-def _load():
-    spec = importlib.util.spec_from_file_location("bench_sort", os.path.join(ROOT, "tools", "bench_sort.py"))
-    bs = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(bs)
-    return bs
-
-
 def test_byte_model():
-    bs = _load()
+    bs = TBF.load_tool("bench_sort")
     n = 1000
     assert bs.model_bytes(n, 4, 2) == n * (4 + 12) + n * 8 * 2 + n * 24 + n * 16          # pass 0, two counts, one full scatter, the last one
     assert bs.model_bytes(n, 8, 8) == n * 20 + n * 64 + n * 24 * 7 + n * 16
@@ -41,8 +25,7 @@ def test_byte_model():
 
 def test_bench_sort_on_the_shim(monkeypatch):
     TBF.install(monkeypatch)
-    ops = sort_shim.install(monkeypatch)
-    bs = _load()
+    bs = TBF.load_tool("bench_sort")
     plans = []
 
     class Ops:
@@ -50,13 +33,13 @@ def test_bench_sort_on_the_shim(monkeypatch):
         def sort_perm(key, valid, descending, perm_in=None, want_image=False):
             distinct_bytes = sum(len(set(((int(v) >> (8 * d)) & 0xff) for v in key.view(torch.int64 if key.element_size() == 8 else torch.int32).tolist())) > 1 for d in range(key.element_size()))
             plans.append(f"d8 passes={distinct_bytes}/8 nulls=0")
-            return ops.sort_perm(key, valid, descending, perm_in, want_image)
+            return cpu_shim.sort_perm(key, valid, descending, perm_in, want_image)
 
         @staticmethod
         def sort_last_plan():
             return plans[-1]
     monkeypatch.setattr(bs, "ops", Ops)
-    monkeypatch.setattr(bs, "event_ms", _cpu_ms)
+    monkeypatch.setattr(bs, "event_ms", TBF.cpu_ms)
     monkeypatch.setattr(bs, "card", lambda: "cpu")
     line = bs.main(["--sf", "0.01", "--rows", "3001", "--api-sf", "0.01", "--asof-quotes", "5000", "--reps", "1", "--steps", "1"],
                    dev=torch.device("cpu"))

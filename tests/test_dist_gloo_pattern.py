@@ -1,46 +1,8 @@
-"""OrderedStream.pattern_recognize on two gloo ranks (kernels replaced by tests/cpu_shim.py + tests/pattern_shim.py): every rank
+"""OrderedStream.pattern_recognize on two gloo ranks (kernels replaced by tests/cpu_shim.py): every rank
 reads its share of the sorted rows, the hash edge by key brings each key's rows to one channel, and collect() gathers the matches
 to every rank.  Each rank must get the one-rank result of the API cases."""
-import os
-import sys
-import traceback
-
-import torch.multiprocessing as mp
-
-from test_dist_gloo import _free_port, _Patch
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _worker(rank, world, port, out_dir):
-    try:
-        sys.path.insert(0, HERE)
-        sys.path.insert(0, os.path.dirname(HERE))
-        os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-        import torch.distributed as dist
-        dist.init_process_group("gloo", rank=rank, world_size=world)
-        import pattern_shim
-        pattern_shim.install(_Patch())
-        import pattern_cases as P
-        from quokka_b200.df import QuokkaContext
-        for case in P.API_CASES:
-            case(QuokkaContext())
-        dist.barrier()
-        dist.destroy_process_group()
-        open(os.path.join(out_dir, f"ok{rank}"), "w").write("ok")
-    except Exception:
-        open(os.path.join(out_dir, f"fail{rank}"), "w").write(traceback.format_exc())
-        raise
+import ranks
 
 
 def test_pattern_two_ranks_gloo(tmp_path):
-    port = _free_port()
-    ctx = mp.get_context("spawn")
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, str(tmp_path))) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(timeout=600)
-    fails = [open(os.path.join(tmp_path, f)).read() for f in os.listdir(tmp_path) if f.startswith("fail")]
-    assert not fails, "\n".join(fails)
-    assert all(os.path.exists(os.path.join(tmp_path, f"ok{r}")) for r in range(2)), [p.exitcode for p in procs]
+    ranks.spawn(tmp_path, 2, ranks.gloo_rank, ranks.SUITES["pattern"])

@@ -1,52 +1,8 @@
-"""DataStream.sort on two gloo ranks (kernels replaced by tests/cpu_shim.py + tests/sort_shim.py): the sample sort leaves rank r
+"""DataStream.sort on two gloo ranks (kernels replaced by tests/cpu_shim.py): the sample sort leaves rank r
 with the r-th range of the first sort column, the gathered result equals the one-rank answer row for row, and a sorted stream
-feeds join_asof (over the ranks' time ranges), windowed_transform and pattern_recognize."""
-import os
-import sys
-import traceback
-
-import torch.multiprocessing as mp
-
-from test_dist_gloo import _free_port, _Patch
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _worker(rank, world, port, out_dir):
-    try:
-        sys.path.insert(0, HERE)
-        sys.path.insert(0, os.path.dirname(HERE))
-        os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-        import torch.distributed as dist
-        dist.init_process_group("gloo", rank=rank, world_size=world)
-        import sort_shim
-        sort_shim.install(_Patch())
-        import sort_api_cases as A
-        from quokka_b200.df import QuokkaContext
-        golden = os.path.join(HERE, "golden")
-        A.case_sort_ranges(QuokkaContext())
-        A.case_sort_collect(QuokkaContext())
-        A.case_sort_select_filter_keep_order(QuokkaContext())
-        A.case_sort_nulls_from_left_join(QuokkaContext())
-        A.case_sort_then_asof(QuokkaContext(), golden)
-        A.case_sort_then_window(QuokkaContext(), golden)
-        A.case_sort_then_pattern(QuokkaContext(), golden)
-        dist.barrier()
-        dist.destroy_process_group()
-        open(os.path.join(out_dir, f"ok{rank}"), "w").write("ok")
-    except Exception:
-        open(os.path.join(out_dir, f"fail{rank}"), "w").write(traceback.format_exc())
-        raise
+feeds join_asof (over the ranks' time ranges), windowed_transform, pattern_recognize, approximate_quantile and gramian."""
+import ranks
 
 
 def test_sort_two_ranks_gloo(tmp_path):
-    port = _free_port()
-    ctx = mp.get_context("spawn")
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, str(tmp_path))) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(timeout=600)
-    fails = [open(os.path.join(tmp_path, f)).read() for f in os.listdir(tmp_path) if f.startswith("fail")]
-    assert not fails, "\n".join(fails)
-    assert all(os.path.exists(os.path.join(tmp_path, f"ok{r}")) for r in range(2)), [p.exitcode for p in procs]
+    ranks.spawn(tmp_path, 2, ranks.gloo_rank, ranks.SUITES["sort"])

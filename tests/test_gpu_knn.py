@@ -5,6 +5,7 @@ import pytest
 import torch
 
 import knn_cases as K
+import ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -183,9 +184,7 @@ def test_vector_empty_chunk(): K.case_vector_empty_chunk(torch.device("cuda"))
 
 
 def test_api_two_nccl_ranks():
-    """When the box shows >= 2 GPUs: the vector and vector_nn_join API cases on 2 NCCL ranks (tests/dist_nccl_knn_check.py)."""
+    """When the box shows >= 2 GPUs: the vector and vector_nn_join API cases on 2 NCCL ranks (tests/dist_nccl_check.py knn)."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    from test_gpu_multirank import _torchrun
-    rc, out = _torchrun("dist_nccl_knn_check.py", 2)
-    assert rc == 0 and "DIST_NCCL_KNN_OK" in out, out[-4000:]
+    ranks.nccl_suites("knn")

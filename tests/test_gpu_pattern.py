@@ -8,6 +8,7 @@ import torch
 
 import pattern_cases as P
 import pattern_shim
+import ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -169,9 +170,7 @@ def test_api_case(qc, case):
 
 
 def test_api_two_nccl_ranks():
-    """When the box shows >= 2 GPUs: the pattern_recognize API cases on 2 NCCL ranks (tests/dist_nccl_pattern_check.py)."""
+    """When the box shows >= 2 GPUs: the pattern_recognize API cases on 2 NCCL ranks (tests/dist_nccl_check.py pattern)."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    from test_gpu_multirank import _torchrun
-    rc, out = _torchrun("dist_nccl_pattern_check.py", 2)
-    assert rc == 0 and "DIST_NCCL_PATTERN_OK" in out, out[-4000:]
+    ranks.nccl_suites("pattern")

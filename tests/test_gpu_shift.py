@@ -2,22 +2,18 @@
 edge flags, order-check counts, every dtype with and without validity, both gather sources, up to 2^24 + 3 rows -- and
 OrderedStream.shift through the API on the device."""
 import ctypes as C
-import os
-import socket
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
+import ranks
 import shift_api_cases as A
 import shift_cases as SC
 import shift_shim
 from quokka_b200 import _lib as L
 
 pytestmark = pytest.mark.gpu
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def _dev(a):
@@ -171,12 +167,4 @@ def test_shift_errors(qc): A.case_shift_errors(qc)
 def test_shift_two_ranks_nccl():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), os.path.join(HERE, "dist_nccl_shift_check.py")]
-    r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=600)
-    out = r.stdout.decode(errors="replace")
-    assert r.returncode == 0 and "DIST_NCCL_SHIFT_OK" in out, out[-4000:]
+    ranks.nccl_suites("shift")

@@ -1,20 +1,16 @@
 """The sort kernel (csrc/sort.cu) on the GPU against the exact reference of tests/sort_cases.py -- permutation equality, which
 stability makes unique -- and DataStream.sort through the API on the device."""
 import ctypes as C
-import os
-import socket
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
+import ranks
 import sort_api_cases as A
 import sort_cases as SC
 
 pytestmark = pytest.mark.gpu
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def _dev(a):
@@ -151,6 +147,7 @@ def test_sort_nulls_from_left_join(qc): A.case_sort_nulls_from_left_join(qc)
 def test_sort_then_asof(qc, golden_dir): A.case_sort_then_asof(qc, golden_dir)
 def test_sort_then_window(qc, golden_dir): A.case_sort_then_window(qc, golden_dir)
 def test_sort_then_pattern(qc, golden_dir): A.case_sort_then_pattern(qc, golden_dir)
+def test_sort_then_quantile_and_gram(qc): A.case_sort_then_quantile_and_gram(qc)
 def test_sort_ranges(qc): A.case_sort_ranges(qc)
 def test_sort_errors(qc): A.case_sort_errors(qc)
 
@@ -158,12 +155,4 @@ def test_sort_errors(qc): A.case_sort_errors(qc)
 def test_sort_two_ranks_nccl():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), os.path.join(HERE, "dist_nccl_sort_check.py")]
-    r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=600)
-    out = r.stdout.decode(errors="replace")
-    assert r.returncode == 0 and "DIST_NCCL_SORT_OK" in out, out[-4000:]
+    ranks.nccl_suites("sort")

@@ -7,13 +7,14 @@ from fractions import Fraction
 import numpy as np
 import pytest
 
+import cpu_shim
 import gram_cases as GC
 import gram_shim
 
 
 @pytest.fixture
 def qc(monkeypatch):
-    gram_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.df import QuokkaContext
     return QuokkaContext()
 

@@ -6,13 +6,14 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import cpu_shim
 import knn_cases as K
 import knn_shim
 
 
 @pytest.fixture
 def qc(monkeypatch):
-    knn_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.df import QuokkaContext
     return QuokkaContext()
 
@@ -30,7 +31,7 @@ def test_vector_parquet(qc, tmp_path): K.case_vector_parquet(qc, tmp_path)
 
 def test_vector_empty_chunk(monkeypatch):
     import torch
-    knn_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     K.case_vector_empty_chunk(torch.device("cpu"))
 
 

@@ -8,6 +8,7 @@ import pyarrow as pa
 import pytest
 import torch
 
+import cpu_shim
 import pattern_cases as P
 import pattern_shim
 from quokka_b200 import _lib as L
@@ -167,7 +168,7 @@ def test_compile_link():
 def test_link_errors_while_the_plan_is_built(monkeypatch):
     """Ops outside the link subset and programs over the kernel's limits fail when pattern_recognize is called, before any row is
     read; a string column read across events (its type is known only when rows arrive) fails when the search runs."""
-    pattern_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.df import QuokkaContext
     qc = QuokkaContext()
     tab = pa.table({"t": np.arange(4, dtype=np.int64), "k": np.zeros(4, np.int64), "v": np.arange(4.0), "s": ["x", "y", "x", "y"]})
@@ -183,7 +184,7 @@ def test_link_errors_while_the_plan_is_built(monkeypatch):
 
 
 def test_maxspan_and_by_arguments(monkeypatch):
-    pattern_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.df import QuokkaContext
     qc = QuokkaContext()
     s = qc.from_arrow_sorted(_t([0, 1], [1, 2]), "t")
@@ -198,7 +199,7 @@ def test_maxspan_and_by_arguments(monkeypatch):
 
 
 def test_explain_and_prefilter_pushdown(monkeypatch, capsys):
-    pattern_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.df import QuokkaContext
     qc = QuokkaContext()
     s = qc.from_arrow_sorted(_t([0, 1], [1, 2]), "t").pattern_recognize("t", [("a", "v > 1"), ("b", "v < 0 and b.v < a.v")], 5, "k")
@@ -212,7 +213,7 @@ def test_explain_and_prefilter_pushdown(monkeypatch, capsys):
 # ------------------------------------------------------------------ the API on the shim
 @pytest.fixture
 def qc(monkeypatch):
-    pattern_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.df import QuokkaContext
     return QuokkaContext()
 

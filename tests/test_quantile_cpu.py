@@ -7,13 +7,14 @@ import numpy as np
 import pytest
 import torch
 
+import cpu_shim
 import quantile_cases as QC
 import quantile_shim
 
 
 @pytest.fixture
 def qc(monkeypatch):
-    quantile_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.df import QuokkaContext
     return QuokkaContext()
 

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+import cpu_shim
 import shift_api_cases as A
 import shift_cases as SC
 import shift_shim
@@ -15,7 +16,6 @@ def _plan(keys, n, nrows, **kw):
     """shift_shim.shift_plan over `keys` (None = one key), with the stable code partition the executor feeds it."""
     if keys is None:
         return shift_shim.shift_plan(n, nrows, **kw)
-    import cpu_shim
     codes = torch.from_numpy(keys)
     n_by = int(keys.max()) + 1 if len(keys) else 1
     dest, seg = cpu_shim.partition_plan(codes, n_by, L.PART_CODE)
@@ -128,7 +128,7 @@ def test_fill_conversion():
 
 @pytest.fixture
 def qc(monkeypatch):
-    shift_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.df import QuokkaContext
     return QuokkaContext()
 

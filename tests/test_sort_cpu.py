@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+import cpu_shim
 import sort_api_cases as A
 import sort_cases as SC
 import sort_shim
@@ -73,7 +74,7 @@ def test_no_cpu_fallback():
 
 
 def test_sort_executor_batching_invariance(monkeypatch):
-    sort_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.columns import DeviceTable
     from quokka_b200.executors import SortExecutor
     keys, valids, desc, dicts = SC.multi_column_case(3000, 4, 1)
@@ -93,7 +94,7 @@ def test_sort_executor_batching_invariance(monkeypatch):
 
 @pytest.fixture
 def qc(monkeypatch):
-    sort_shim.install(monkeypatch)
+    cpu_shim.install(monkeypatch)
     from quokka_b200.df import QuokkaContext
     return QuokkaContext()
 
@@ -104,6 +105,7 @@ def test_sort_nulls_from_left_join(qc): A.case_sort_nulls_from_left_join(qc)
 def test_sort_then_asof(qc, golden_dir): A.case_sort_then_asof(qc, golden_dir)
 def test_sort_then_window(qc, golden_dir): A.case_sort_then_window(qc, golden_dir)
 def test_sort_then_pattern(qc, golden_dir): A.case_sort_then_pattern(qc, golden_dir)
+def test_sort_then_quantile_and_gram(qc): A.case_sort_then_quantile_and_gram(qc)
 def test_sort_ranges(qc): A.case_sort_ranges(qc)
 def test_sort_errors(qc): A.case_sort_errors(qc)
 

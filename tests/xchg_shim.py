@@ -1,4 +1,4 @@
-"""TEST-ONLY numpy restatement of quokka_b200.ops.XchgChannel (csrc/exchange.cu, the K6 shuffle's four channel calls), on top
+"""TEST-ONLY numpy restatement of quokka_b200.ops.XchgChannel (csrc/exchange.cu, the K6 shuffle's four channel calls), part
 of tests/cpu_shim.py, so that the in-process link (tests/inproc_link.py) and runtime.Exchange's link path run without a GPU.
 
 Control blocks and mailboxes are the same raw memory the kernels address (here: a CPU tensor's), read and written through
@@ -13,7 +13,6 @@ import ctypes
 import numpy as np
 import torch
 
-import cpu_shim
 import inproc_link as IL
 from quokka_b200 import _lib as L
 
@@ -187,4 +186,5 @@ class XchgChannel:
 
 def install(patch):
     """cpu_shim.install(patch): the rest of the kernels (partition plans, scatter, ...) in numpy on CPU tensors."""
+    import cpu_shim                     # cpu_shim imports this module for XchgChannel
     cpu_shim.install(patch)

@@ -14,18 +14,19 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+TOOLS = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(TOOLS))
+sys.path.insert(0, TOOLS)                                                     # benchkit, also when loaded as a module
 
 import torch
 
+from benchkit import HBM_PEAK_TBS, card, event_ms, wall
 from quokka_b200 import ops
 
 GRAM_COLS = ["l_quantity", "l_extendedprice", "l_discount", "l_tax"]
-HBM_PEAK_TBS, FP64_TC_PEAK_TFLOPS = 3.35, 67.0   # H100 SXM data sheet (700 W card): HBM3 bandwidth; FP64 tensor core, dense
+FP64_TC_PEAK_TFLOPS = 67.0                         # H100 SXM data sheet (700 W card): FP64 tensor core, dense
 
 
 def roofline(nbytes, flops, seconds, what):
@@ -34,40 +35,6 @@ def roofline(nbytes, flops, seconds, what):
             "gb_per_s": nbytes / seconds / 1e9, "tflops": flops / seconds / 1e12, "algorithmic_bytes": nbytes, "algorithmic_flops": flops,
             "peaks": {"hbm_tb_per_s": HBM_PEAK_TBS, "fp64_tensor_core_tflops": FP64_TC_PEAK_TFLOPS,
                       "source": "H100 SXM data sheet (700 W), not measured"}, "what": what}
-
-
-def card():
-    """name and power limit of the card (a read-only query)."""
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                              timeout=30).stdout.strip()
-    except Exception as e:
-        return f"unknown ({type(e).__name__})"
-
-
-def event_ms(fn, reps):
-    """CUDA-event time of one call of fn, averaged over reps calls."""
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def wall(fn, steps):
-    """(last result, best seconds, all seconds) of fn() after one untimed call, each call ending in a device synchronise."""
-    fn()
-    times = []
-    for _ in range(max(1, steps)):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        res = fn()
-        torch.cuda.synchronize()
-        times.append(time.perf_counter() - t0)
-    return res, min(times), times
 
 
 def bound_ratio(G, cols):

@@ -14,16 +14,18 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+TOOLS = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(TOOLS))
+sys.path.insert(0, TOOLS)                                                     # benchkit, also when loaded as a module
 
 import torch
 
+from benchkit import HBM_PEAK_TBS, card, event_ms
 from quokka_b200 import ops
 
-HBM_PEAK_TBS, TF32_PEAK_TFLOPS = 3.35, 495.0   # H100 SXM data sheet (700 W card): HBM3 bandwidth; TF32 tensor core, dense
+TF32_PEAK_TFLOPS = 495.0                       # H100 SXM data sheet (700 W card): TF32 tensor core, dense
 TERMS = {"f32": 3, "f16": 2}                     # TF32 MMAs per product: 3xTF32 for f32 rows, two probe terms for f16 rows
 
 
@@ -33,27 +35,6 @@ def roofline(nbytes, flops, seconds):
             "tflops": flops / seconds / 1e12, "algorithmic_bytes": nbytes, "algorithmic_flops": flops,
             "peaks": {"hbm_tb_per_s": HBM_PEAK_TBS, "tf32_tensor_core_tflops": TF32_PEAK_TFLOPS,
                       "source": "H100 SXM data sheet (700 W), not measured"}}
-
-
-def card():
-    """name and power limit of the card (a read-only query)."""
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                              timeout=30).stdout.strip()
-    except Exception as e:
-        return f"unknown ({type(e).__name__})"
-
-
-def event_ms(fn, reps):
-    """CUDA-event time of one call of fn, averaged over reps calls."""
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def torch_topk(x, phat, k, chunk_elems=1 << 29):

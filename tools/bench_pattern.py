@@ -20,40 +20,19 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time as _time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, os.path.join(ROOT, "tools"))                               # benchkit, also when loaded as a module
 
 import torch
 
+from benchkit import HBM_PEAK_TBS, card, event_ms
 from quokka_b200 import ops, synth
 
-HBM_PEAK_TBS = 3.35          # H100 SXM data sheet (700 W card): HBM3 bandwidth
-
-
-def card():
-    """name and power limit of the card (a read-only query)."""
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                              timeout=30).stdout.strip()
-    except Exception as e:
-        return f"unknown ({type(e).__name__})"
-
-
-def event_ms(fn, reps):
-    """CUDA-event time of one call of fn, averaged over reps calls."""
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def sync(dev):

@@ -16,54 +16,21 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+TOOLS = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(TOOLS))
+sys.path.insert(0, TOOLS)                                                     # benchkit, also when loaded as a module
 
 import numpy as np
 import torch
 
+from benchkit import HBM_PEAK_TBS, card, event_ms, wall
 from quokka_b200 import ops
 
 COV_COLS = ["l_quantity", "l_extendedprice", "l_discount", "l_tax"]         # apps/tpc-h/tpch.py:600-602
 QS = [0.1, 0.5, 0.9]
-HBM_PEAK_TBS = 3.35                                                           # H100 SXM data sheet (700 W card)
-
-
-def card():
-    """name and power limit of the card (a read-only query)."""
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                              timeout=30).stdout.strip()
-    except Exception as e:
-        return f"unknown ({type(e).__name__})"
-
-
-def event_ms(fn, reps):
-    """CUDA-event time of one call of fn, averaged over reps calls."""
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def wall(fn, steps):
-    """(last result, best seconds) of fn() after one untimed call, each call ending in a device synchronise."""
-    fn()
-    best, res = float("inf"), None
-    for _ in range(max(1, steps)):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        res = fn()
-        torch.cuda.synchronize()
-        best = min(best, time.perf_counter() - t0)
-    return res, best
 
 
 def roofline(nbytes, seconds, what):
@@ -93,8 +60,8 @@ def run_narrow(args, dev):
     cols = {c: synth.column(c, args.sf, device=dev) for c in COV_COLS}
     n = cols["l_tax"].numel()
     table = DeviceTable({c: DeviceColumn(v) for c, v in cols.items()})
-    res606, t606 = wall(lambda: QuokkaContext().from_device(table).approximate_quantile(["l_tax"], 0.9).collect(), args.steps)
-    res4, t4 = wall(lambda: QuokkaContext().from_device(table).approximate_quantile(COV_COLS, QS).collect(), args.steps)
+    res606, t606, _ = wall(lambda: QuokkaContext().from_device(table).approximate_quantile(["l_tax"], 0.9).collect(), args.steps)
+    res4, t4, _ = wall(lambda: QuokkaContext().from_device(table).approximate_quantile(COV_COLS, QS).collect(), args.steps)
     xs = [cols[c] for c in COV_COLS]
     sk = ops.QuantileSketch(len(xs), dev)
     sk.update(xs)
@@ -104,9 +71,9 @@ def run_narrow(args, dev):
     # torch's exact path: kthvalue per quantile, and one sort per column
     def kth():
         return [[float(torch.kthvalue(x.to(torch.float64), nearest_rank(n, q) + 1).values) for q in QS] for x in xs]
-    exact, kth_s = wall(kth, 1)
-    _, sort_s = wall(lambda: [torch.sort(x)[0][[nearest_rank(n, q) for q in QS]] for x in xs], 1)
-    _, kth606_s = wall(lambda: float(torch.kthvalue(cols["l_tax"], nearest_rank(n, 0.9) + 1).values), 1)
+    exact, kth_s, _ = wall(kth, 1)
+    _, sort_s, _ = wall(lambda: [torch.sort(x)[0][[nearest_rank(n, q) for q in QS]] for x in xs], 1)
+    _, kth606_s, _ = wall(lambda: float(torch.kthvalue(cols["l_tax"], nearest_rank(n, 0.9) + 1).values), 1)
     got = [[res4[c][i].as_py() for c in COV_COLS] for i in range(len(QS))]
     rel = max(abs(got[i][j] - exact[j][i]) / max(abs(exact[j][i]), 1e-300) for i in range(len(QS)) for j in range(len(COV_COLS)))
     out = {"workload": f"SF-{args.sf:g} lineitem, {n} rows, fp64 columns resident in HBM",
@@ -162,7 +129,7 @@ def run_wide(args, dev):
         for lo in range(0, k, 256):
             outs.append(torch.stack([torch.kthvalue(X[lo:lo + 256], r, dim=1).values for r in ranks]))
         return torch.cat(outs, dim=1)
-    exact, kth_s = wall(kth, 1)
+    exact, kth_s, _ = wall(kth, 1)
     rel = float(((vals.to(torch.float64) - exact.to(torch.float64)).abs() / exact.to(torch.float64).abs().clamp_min(1e-300)).max())
     return {"workload": f"{n} rows x {k} f32 columns (seeded normal) at [0.1, 0.9]", "entries": sk.entries()[0].numel(), "capacity": getattr(sk, "capacity", None),
             "fresh_sketch_seconds": fresh_s, "deferral_rounds": sk.rounds, "grows": sk.grows, "kernel_ms_grown": kms,

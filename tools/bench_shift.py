@@ -17,54 +17,23 @@ limit and SM clock are read in the same run; without a GPU the script fails.  No
 from __future__ import annotations
 
 import argparse
+import functools
 import json
 import os
-import subprocess
 import sys
-import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+TOOLS = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(TOOLS))
+sys.path.insert(0, TOOLS)                                                     # benchkit, also when loaded as a module
 
 import torch
 
+import benchkit
+from benchkit import HBM_PEAK_TBS, event_ms, wall
 from quokka_b200 import _lib as L
 from quokka_b200 import ops
 
-HBM_PEAK_TBS = 3.35                                                           # H100 SXM data sheet (700 W card)
-
-
-def card():
-    """name, power limit and the SM clock now / at most (a read-only query)."""
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as e:
-        return f"unknown ({type(e).__name__})"
-
-
-def event_ms(fn, reps):
-    """CUDA-event time of one call of fn, averaged over reps calls."""
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def wall(fn, steps):
-    """(last result, best seconds) of fn() after one untimed call, each call ending in a device synchronise."""
-    fn()
-    best, res = float("inf"), None
-    for _ in range(max(1, steps)):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        res = fn()
-        torch.cuda.synchronize()
-        best = min(best, time.perf_counter() - t0)
-    return res, best
+card = functools.partial(benchkit.card, clocks=True)                         # with the SM clock now and at most
 
 
 def model_bytes(n: int, value_bytes: int, keyed: bool) -> int:
@@ -145,7 +114,7 @@ def main(argv=None, dev=None):
                 qc = QuokkaContext()
                 s = qc.from_device(table, sorted_by="time").shift(1, by="symbol" if name == "D" else None, columns=["asize"], suffix="_prev")
                 return qc.execute_node(s.node, to_arrow=False)
-            res, secs = wall(program, args.steps)
+            res, secs, _ = wall(program, args.steps)
             v = res["asize_prev"].valid
             line["legs"].append({"leg": name + (" DataStream shift by symbol" if name == "D" else " DataStream shift, no key"), "rows": n,
                                  "seconds": secs, "rows_per_s": n / secs, "null_rows": int((v == 0).sum().item()) if v is not None else 0})

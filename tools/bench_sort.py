@@ -17,54 +17,23 @@ without a GPU the script fails.  Nothing is written to disk."""
 from __future__ import annotations
 
 import argparse
+import functools
 import json
 import os
 import re
-import subprocess
 import sys
-import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+TOOLS = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(TOOLS))
+sys.path.insert(0, TOOLS)                                                     # benchkit, also when loaded as a module
 
 import torch
 
+import benchkit
+from benchkit import HBM_PEAK_TBS, event_ms, wall
 from quokka_b200 import ops
 
-HBM_PEAK_TBS = 3.35                                                           # H100 SXM data sheet (700 W card)
-
-
-def card():
-    """name, power limit and the SM clock now / at most (a read-only query)."""
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as e:
-        return f"unknown ({type(e).__name__})"
-
-
-def event_ms(fn, reps):
-    """CUDA-event time of one call of fn, averaged over reps calls."""
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def wall(fn, steps):
-    """(last result, best seconds) of fn() after one untimed call, each call ending in a device synchronise."""
-    fn()
-    best, res = float("inf"), None
-    for _ in range(max(1, steps)):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        res = fn()
-        torch.cuda.synchronize()
-        best = min(best, time.perf_counter() - t0)
-    return res, best
+card = functools.partial(benchkit.card, clocks=True)                         # with the SM clock now and at most
 
 
 def model_bytes(n: int, key_bytes: int, passes: int, null_pass: bool = False) -> int:
@@ -108,7 +77,7 @@ def run_api(args, dev):
         qc = QuokkaContext()
         s = qc.from_device(table).sort(["l_shipdate", "l_extendedprice"], [False, True])
         return qc.execute_node(s.node, to_arrow=False)
-    res, secs = wall(program, args.steps)
+    res, secs, _ = wall(program, args.steps)
     d, p = res["l_shipdate"].data, res["l_extendedprice"].data
     ok = bool(((d[1:] > d[:-1]) | ((d[1:] == d[:-1]) & (p[1:] <= p[:-1]))).all().item()) if n > 1 else True
     return {"leg": "D", "workload": f"SF-{args.api_sf:g} lineitem.sort([l_shipdate, l_extendedprice desc]), 2 key + 4 payload columns, {n} rows",
@@ -141,8 +110,8 @@ def run_asof(args, dev):
         qc = QuokkaContext()
         s = qc.from_device(tu).sort("time").join_asof(qc.from_device(qu).sort("time"), on="time", by="symbol")
         return qc.execute_node(s.node, to_arrow=False)
-    a, sa = wall(presorted, args.steps)
-    b, sb = wall(sorted_here, args.steps)
+    a, sa, _ = wall(presorted, args.steps)
+    b, sb, _ = wall(sorted_here, args.steps)
     # quotes of one symbol have distinct times here, so both programs match every trade with the same quote
     same = len(a) == len(b) == nt and bool(torch.equal(torch.sort(a["bid"].data.double() + a["time"].data).values,
                                                        torch.sort(b["bid"].data.double() + b["time"].data).values))
