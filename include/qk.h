@@ -128,8 +128,6 @@ QK_API const char* qk_last_error(void);
 QK_API int qk_version(void);
 /* number of kernel launches issued by this library in this process (bench.py's gpu_launches) */
 QK_API int64_t qk_launch_count(void);
-/* SM count of the current device (grids are sized in multiples of it) */
-QK_API int qk_sm_count(void);
 
 /* ---- K1: scan -> filter -> project --------------------------------------------------------
  * Replaces: Arrow `dataset.to_table(filter, columns)` (pyquokka/dataset/unordered_readers.py:98-99),
@@ -627,9 +625,10 @@ QK_API int qk_parquet_decode(const uint8_t* bytes, int64_t n_bytes, const qk_pq_
  *     at runs[run_offsets[i] ...]; V1 definition levels are checked here (pages[i].status bit 1 = nulls);
  *   qk_parquet_decode then reads the scratch buffer as its `bytes`.
  *   ZSTD pages (the default of the Polars writer, apps/convert.py:5-19) are decoded by one thread per page (a
- *     sequential RFC 8878 frame decoder, csrc/zstd_core.h) and need a workspace: `work` holds `work_bytes /
- *     qk_parquet_inflate_slot_bytes()` slots (decoding tables + a 128 KB literals buffer each); that many pages are in
- *     flight at once, the rest follow round-robin.  GZIP pages use the same slots (their state is ~1.5 KB).
+ *     sequential RFC 8878 frame decoder, csrc/zstd_core.h) and need a workspace of slots (decoding tables + a 128 KB
+ *     literals buffer each), one per page in flight; the rest follow round-robin.  qk_parquet_inflate_workspace_bytes(n)
+ *     sizes it for n such pages: min(n, 8 per SM) slots in whole CTAs of the inflate kernel, 0 for n <= 0.  A smaller
+ *     `work` (at least one CTA's slots) puts fewer pages in flight.  GZIP pages use the same slots (their state is ~1.5 KB).
  * compression: QK_PQ_CODEC_* ; other codecs: QK_ERR_UNSUPPORTED. */
 #define QK_PQ_CODEC_NONE 0
 #define QK_PQ_CODEC_SNAPPY 1
@@ -660,7 +659,7 @@ QK_API int qk_parquet_walk_pages(const uint8_t* bytes, int64_t chunk_offset, int
                           int32_t physical_type, int32_t max_def_level, int32_t compression, int32_t dict_base,
                           qk_pq_page* pages, int64_t pages_cap, int64_t* n_pages, int64_t* dense,
                           int64_t* scratch_bytes, qk_pq_chunk_info* info);
-QK_API size_t qk_parquet_inflate_slot_bytes(void);
+QK_API size_t qk_parquet_inflate_workspace_bytes(int64_t n_zstd_pages);
 QK_API int qk_parquet_inflate(const uint8_t* bytes, int64_t n_bytes, qk_pq_page* pages, int64_t n_pages, uint8_t* scratch,
                        int64_t scratch_bytes, void* work, int64_t work_bytes, void* stream);
 QK_API int qk_parquet_page_runs(const uint8_t* scratch, int64_t scratch_bytes, qk_pq_page* pages, int64_t n_pages,

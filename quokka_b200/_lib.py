@@ -23,7 +23,6 @@ MAX_EXPR_NODES, MAX_TOTAL_NODES, MAX_STACK = 48, 112, 8      # include/qk.h QK_M
 PQ_RUN_PLAIN, PQ_RUN_RLE, PQ_RUN_PACKED, PQ_RUN_BOOL = 0, 1, 2, 3
 PQ_PAGE_DATA_V1, PQ_PAGE_DATA_V2, PQ_PAGE_DICT = 0, 1, 2
 PQ_CODEC_NONE, PQ_CODEC_SNAPPY, PQ_CODEC_ZSTD, PQ_CODEC_GZIP = 0, 1, 2, 3
-PQ_INFLATE_WARPS = 4
 (PQ_BOOLEAN, PQ_INT32, PQ_INT64, PQ_INT96, PQ_FLOAT, PQ_DOUBLE, PQ_BYTE_ARRAY, PQ_FIXED_LEN_BYTE_ARRAY) = range(8)
 ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_CAPACITY = -1, -2, -3, -4
 
@@ -87,7 +86,6 @@ _SIGNATURES = {
     "qk_last_variant_config": (C.c_char_p, []),
     "qk_version": (C.c_int, []),
     "qk_launch_count": (C.c_int64, []),
-    "qk_sm_count": (C.c_int, []),
     "qk_scan_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "qk_scan_filter_project": (C.c_int, [_P(qk_column), C.c_int32, C.c_int64, _P(qk_expr), _P(qk_expr), C.c_int32,
                                          _P(qk_column), C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -166,7 +164,7 @@ _SIGNATURES = {
                                         C.c_void_p, C.c_int64, _P(C.c_int64), _P(C.c_int64), _P(qk_pq_chunk_info)]),
     "qk_parquet_walk_pages": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_void_p, C.c_int64, _P(C.c_int64), _P(C.c_int64), _P(C.c_int64), _P(qk_pq_chunk_info)]),
-    "qk_parquet_inflate_slot_bytes": (C.c_size_t, []),
+    "qk_parquet_inflate_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "qk_parquet_inflate": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                      C.c_void_p]),
     "qk_parquet_page_runs": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,

@@ -31,5 +31,4 @@ extern "C" {
 const char* qk_last_error(void) { return qk::last_err(); }
 int qk_version(void) { return QK_VERSION; }
 int64_t qk_launch_count(void) { return qk::g_launches.load(); }
-int qk_sm_count(void) { return qk::sm_count(); }
 }

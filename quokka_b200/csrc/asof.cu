@@ -233,21 +233,40 @@ __global__ void __launch_bounds__(AS_NT) k_asof_sweep(const long long* __restric
     }
 }
 
+// the backward path's workspace: the right rows' partition destinations, the key segments, the right rows in key order
+// (time, row number), then the partition's own workspace
+struct AsofWs {
+    int32_t* dest; int64_t* seg; long long* sorted_time; int32_t* sorted_idx; void* part; size_t part_bytes, bytes;
+    AsofWs(int64_t n_right, int32_t n_by, void* base) : part_bytes(qk_partition_workspace_bytes(n_right, n_by)) {
+        Carve c(base);
+        dest = c.take<int32_t>(n_right);
+        seg = c.take<int64_t>((size_t)(n_by + 1));
+        sorted_time = c.take<long long>(n_right);
+        sorted_idx = c.take<int32_t>(n_right);
+        part = c.take<char>(part_bytes);
+        bytes = c.bytes;
+    }
+};
+
+// the merge's workspace: the bounds of every window (wr[nwin + 1], then wl[nwin + 1]), then one key table per chunk
+struct AsofMergeWs {
+    long long* bounds; int32_t* tables; size_t bytes;
+    AsofMergeWs(int64_t nwin, int P, int32_t n_by, void* base) {
+        Carve c(base);
+        bounds = c.take<long long>((size_t)(nwin + 1) * 2);
+        tables = c.take<int32_t>((size_t)P * n_by);
+        bytes = c.bytes;
+    }
+};
+
 }  // namespace
 }  // namespace qk
 
 using namespace qk;
 
-static size_t asof_fixed_bytes(int64_t n_right, int32_t n_by) {
-    return align_up((size_t)n_right * 4, 256)            // dest
-         + align_up((size_t)(n_by + 1) * 8, 256)         // segment offsets
-         + align_up((size_t)n_right * 8, 256)            // sorted_time
-         + align_up((size_t)n_right * 4, 256);           // sorted_idx
-}
-
 extern "C" size_t qk_asof_workspace_bytes(int64_t n_right, int32_t n_by) {
     if (n_right < 0 || n_by <= 0) return 0;
-    return asof_fixed_bytes(n_right, n_by) + qk_partition_workspace_bytes(n_right, n_by);
+    return AsofWs(n_right, n_by, nullptr).bytes;
 }
 
 extern "C" int qk_asof_backward(const qk_column* l_time, const qk_column* l_by, const qk_column* r_time,
@@ -265,20 +284,16 @@ extern "C" int qk_asof_backward(const qk_column* l_time, const qk_column* l_by, 
     const int64_t nl = l_time->length, nr = r_time->length;
     if (nl == 0) return QK_OK;
     if (!out_ridx) QK_FAIL(QK_ERR_INVALID, "%s: null output", who);
-    if (!workspace || ws_bytes < qk_asof_workspace_bytes(nr, n_by)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
-    char* w = (char*)workspace;
-    int32_t* dest = (int32_t*)w; w += align_up((size_t)nr * 4, 256);
-    int64_t* seg = (int64_t*)w; w += align_up((size_t)(n_by + 1) * 8, 256);
-    long long* sorted_time = (long long*)w; w += align_up((size_t)nr * 8, 256);
-    int32_t* sorted_idx = (int32_t*)w; w += align_up((size_t)nr * 4, 256);
-    if (int rc = qk_partition_plan(r_by, n_by, QK_PART_CODE, dest, seg, w, ws_bytes - asof_fixed_bytes(nr, n_by), stream)) return rc;
+    const AsofWs w(nr, n_by, workspace);
+    if (!workspace || ws_bytes < w.bytes) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
+    if (int rc = qk_partition_plan(r_by, n_by, QK_PART_CODE, w.dest, w.seg, w.part, w.part_bytes, stream)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (nr > 0) {
-        k_asof_prepare<<<grid_size(nr, 16), 256, 0, st>>>((const long long*)r_time->data, dest, nr, sorted_time, sorted_idx);
+        k_asof_prepare<<<grid_size(nr, 16), 256, 0, st>>>((const long long*)r_time->data, w.dest, nr, w.sorted_time, w.sorted_idx);
         QK_LAUNCH_CHECK("k_asof_prepare");
     }
     k_asof_search<<<grid_size(nl, 16), 256, 0, st>>>((const long long*)l_time->data, (const int32_t*)l_by->data, nl, n_by,
-                                                sorted_time, sorted_idx, seg, out_ridx);
+                                                w.sorted_time, w.sorted_idx, w.seg, out_ridx);
     QK_LAUNCH_CHECK("k_asof_search");
     return QK_OK;
 }
@@ -300,7 +315,7 @@ extern "C" size_t qk_asof_merge_workspace_bytes(int64_t n_left, int64_t n_right,
     size_t smem;
     const int P = n_by > 0 ? asof_merge_chunks(n_by, &smem) : 0;
     if (P == 0 || n_left < 0 || n_right < 0) return 0;
-    return align_up((size_t)(asof_windows(n_left + n_right) + 1) * 16, 256) + align_up((size_t)P * n_by * 4, 256);
+    return AsofMergeWs(asof_windows(n_left + n_right), P, n_by, nullptr).bytes;
 }
 
 extern "C" int qk_asof_merge(const qk_column* l_time, const qk_column* l_by, const qk_column* r_time, const qk_column* r_by,
@@ -321,14 +336,15 @@ extern "C" int qk_asof_merge(const qk_column* l_time, const qk_column* l_by, con
     const int P0 = asof_merge_chunks(n_by, &smem);
     if (P0 == 0) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: %d keys do not fit a shared-memory table; use qk_asof_backward", who, n_by);
     if (nl > 0 && !out_ridx) QK_FAIL(QK_ERR_INVALID, "%s: null output", who);
-    if (!workspace || ws_bytes < qk_asof_merge_workspace_bytes(nl, nr, n_by)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
     const int64_t nwin = asof_windows(nl + nr);
+    const AsofMergeWs w(nwin, P0, n_by, workspace);
+    if (!workspace || ws_bytes < w.bytes) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
     const int64_t wpc = (nwin + P0 - 1) / P0;                      // windows per chunk (CTA)
     const int P = (int)((nwin + wpc - 1) / wpc);                   // chunks that have a window: <= P0
     cudaStream_t st = (cudaStream_t)stream;
-    long long* wr = (long long*)workspace;
+    long long* wr = w.bounds;
     long long* wl = wr + (nwin + 1);
-    int32_t* tables = (int32_t*)((char*)workspace + align_up((size_t)(nwin + 1) * 16, 256));
+    int32_t* tables = w.tables;
     k_asof_bounds<<<(unsigned)((nwin + 1 + 127) / 128), 128, 0, st>>>((const long long*)r_time->data, nr, (const long long*)l_time->data, nl, nwin, wr, wl);
     QK_LAUNCH_CHECK("k_asof_bounds");
     const size_t table_bytes = align_up((size_t)n_by * 4, 16);

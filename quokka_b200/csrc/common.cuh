@@ -68,6 +68,22 @@ static inline int check_col(const qk_column* c, const char* what) {
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// A caller-provided workspace, laid out once.  A kernel's layout function takes its pieces in order from one Carve:
+// over a null base it only adds up the bytes (what its qk_*_workspace_bytes returns), over the caller's buffer it also
+// hands out every piece, at the same offsets.  Each piece is rounded up to `align` bytes (256 unless said otherwise).
+// A nested layout (another kernel's workspace) is taken as one piece of its total.
+struct Carve {
+    char* base;
+    size_t bytes = 0;
+    explicit Carve(void* b) : base((char*)b) {}
+    template <typename T>
+    T* take(size_t count, size_t align = 256) {
+        T* p = base ? (T*)(base + bytes) : nullptr;
+        bytes += align_up(count * sizeof(T), align);
+        return p;
+    }
+};
+
 // grid of a grid-stride launch: one CTA per `per_cta` work items, at most `per_sm` CTAs per SM, at least one CTA
 static inline unsigned grid_size(int64_t n, int per_sm, int64_t per_cta = 256) {
     const int64_t nb = (n + per_cta - 1) / per_cta, cap = (int64_t)sm_count() * per_sm;

@@ -332,7 +332,23 @@ __global__ void __launch_bounds__(C_NT, 3) k_filter_compact_tma(const __grid_con
     }
 }
 
+constexpr int C_MAX_CHUNKS = 1024;
+
+// the workspace: per-chunk survivor counts, their offsets (8 spare), then the survivor bitmap (1 bit per row, 8 spare words)
+struct CompactWs {
+    int64_t* counts; int64_t* offsets; unsigned* bitmap; size_t bytes;
+    CompactWs(int64_t nrows, void* base) {
+        Carve c(base);
+        counts = c.take<int64_t>(C_MAX_CHUNKS, 8);
+        offsets = c.take<int64_t>(C_MAX_CHUNKS + 8, 8);
+        bitmap = c.take<unsigned>((nrows + 31) / 32 + 8);
+        bytes = c.bytes;
+    }
+};
+
 }  // namespace
+
+size_t compact_workspace_bytes(int64_t nrows) { return CompactWs(nrows, nullptr).bytes; }
 
 int try_filter_compact_tma(const qk_column* cols, int ncols, int64_t nrows, const qk_expr* pred, const qk_expr* proj, int nproj,
                            qk_column* out, int64_t* out_rows, void* workspace, size_t ws_bytes, const qk_bloom* bloom, cudaStream_t st) {
@@ -384,15 +400,15 @@ int try_filter_compact_tma(const qk_column* cols, int ncols, int64_t nrows, cons
     // contiguous chunks of whole tiles, one per CTA
     const int64_t ntiles = (nrows + tile - 1) / tile;
     int64_t want = (int64_t)sms * ctas_per_sm;
-    if (want > 1024) want = 1024;                        // the workspace below holds 1024 chunk counts and offsets
+    if (want > C_MAX_CHUNKS) want = C_MAX_CHUNKS;        // the workspace holds C_MAX_CHUNKS chunk counts and offsets
     const int64_t tiles_per_chunk = (ntiles + want - 1) / want;
     const int64_t chunk_rows = tiles_per_chunk * tile;
     const int nb = (int)((nrows + chunk_rows - 1) / chunk_rows);
-    const size_t bitmap_bytes = align_up((size_t)((nrows + 31) / 32 + 8) * 4, 256);
-    if (ws_bytes < (size_t)(2 * 1024 + 8) * 8 + bitmap_bytes || !workspace) return 1;
-    int64_t* counts = (int64_t*)workspace;
-    int64_t* offsets = counts + 1024;
-    unsigned* bitmap = (unsigned*)((char*)workspace + (size_t)(2 * 1024 + 8) * 8);
+    const CompactWs w(nrows, workspace);
+    if (ws_bytes < w.bytes || !workspace) return 1;
+    int64_t* counts = w.counts;
+    int64_t* offsets = w.offsets;
+    unsigned* bitmap = w.bitmap;
     if (A.bloom) {
         const int kd = cols[proj[A.bloom_col].nodes[0].a0].dtype;
         if (kd != QK_I64 && kd != QK_I32) QK_FAIL(QK_ERR_UNSUPPORTED, "qk_scan_filter_project_sj: the join key must be int64 / int32");

@@ -278,10 +278,19 @@ Plan make_plan(int64_t nrows, int32_t kext) {
     return p;
 }
 
-size_t plan_bytes(const Plan& p, int32_t k) {
-    return align_up((size_t)k * sizeof(GramCol), 256) + align_up((size_t)p.ntiles * sizeof(int2), 256) +
-           (size_t)p.nsplit * p.ntiles * p.T * p.T * sizeof(double);
-}
+// the workspace: the column table and the tile order (the first `head` bytes, written from the host in one copy), then
+// every split's partial tiles
+struct GramWs {
+    GramCol* cols; int2* tiles; double* part; size_t head, bytes;
+    GramWs(const Plan& p, int32_t k, void* base) {
+        Carve c(base);
+        cols = c.take<GramCol>(k);
+        tiles = c.take<int2>(p.ntiles);
+        head = c.bytes;
+        part = c.take<double>((size_t)p.nsplit * p.ntiles * p.T * p.T);
+        bytes = c.bytes;
+    }
+};
 
 template <class C, int MMA>
 int launch_tiles(const TileArgs& a, int ntiles, int nsplit, cudaStream_t st) {
@@ -302,7 +311,7 @@ using namespace qk;
 
 extern "C" size_t qk_gram_workspace_bytes(int64_t nrows, int32_t k) {
     if (nrows < 0 || k < 1) return 0;
-    const size_t a = plan_bytes(make_plan(nrows, k), k), b = plan_bytes(make_plan(nrows, k + 1), k);
+    const size_t a = GramWs(make_plan(nrows, k), k, nullptr).bytes, b = GramWs(make_plan(nrows, k + 1), k, nullptr).bytes;
     return a > b ? a : b;                                                  // with or without the column of ones
 }
 
@@ -325,27 +334,25 @@ extern "C" int qk_gram(const qk_column* cols, int32_t k, int64_t nrows, const do
     if (nrows == 0) return QK_OK;
     const int32_t kext = k + (sums ? 1 : 0);
     const Plan p = make_plan(nrows, kext);
-    if (!workspace || ws_bytes < plan_bytes(p, k)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small (%zu < %zu)", who, ws_bytes,
-                                                           plan_bytes(p, k));
-    // column table and tile order travel in the workspace, so any k fits
-    const size_t off_tiles = align_up((size_t)k * sizeof(GramCol), 256);
-    const size_t off_part = off_tiles + align_up((size_t)p.ntiles * sizeof(int2), 256);
-    std::vector<unsigned char> host(off_part, 0);
+    const GramWs w(p, k, workspace);
+    if (!workspace || ws_bytes < w.bytes) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small (%zu < %zu)", who, ws_bytes, w.bytes);
+    // column table and tile order travel in the workspace, so any k fits; the host copy has the workspace's layout
+    std::vector<unsigned char> host(w.head, 0);
     GramCol* hc = (GramCol*)host.data();
     for (int32_t i = 0; i < k; ++i) hc[i] = GramCol{cols[i].data, cols[i].dtype, 0};
-    int2* ht = (int2*)(host.data() + off_tiles);
+    int2* ht = (int2*)(host.data() + ((char*)w.tiles - (char*)w.cols));
     int n = 0;
     for (int bi = 0; bi < p.nb; bi += GROUP)
         for (int bj = bi; bj < p.nb; bj += GROUP)
             for (int I = bi; I < bi + GROUP && I < p.nb; ++I)
                 for (int J = (I > bj ? I : bj); J < bj + GROUP && J < p.nb; ++J) ht[n++] = make_int2(I, J);
     cudaStream_t st = (cudaStream_t)stream;
-    QK_CUDA(cudaMemcpyAsync(workspace, host.data(), off_part, cudaMemcpyHostToDevice, st));
+    QK_CUDA(cudaMemcpyAsync(workspace, host.data(), w.head, cudaMemcpyHostToDevice, st));
     TileArgs a;
-    a.cols = (const GramCol*)workspace;
+    a.cols = w.cols;
     a.shift = shift;
-    a.tiles = (const int2*)((char*)workspace + off_tiles);
-    a.part = (double*)((char*)workspace + off_part);
+    a.tiles = w.tiles;
+    a.part = w.part;
     a.k = k; a.kext = kext; a.ntiles = p.ntiles; a.nops = p.nb > 1 ? 2 : 1;
     a.nrows = nrows; a.rows_per_split = p.rows_per_split;
     const int mma = variant == 0 ? 2 : variant;                            // m16n8k16 measured faster (DESIGN.md section 4)

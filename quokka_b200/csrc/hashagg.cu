@@ -24,17 +24,15 @@ struct State {              // carved out of the caller's buffer
     unsigned* tag; unsigned long long* k0; unsigned long long* k1; long long* cnt; double* acc;
 };
 
-size_t carve(const qk_hashagg_desc* d, void* base, State* s) {
-    size_t off = 0;
+size_t carve(const qk_hashagg_desc* d, void* base, State& s) {
+    Carve c(base);
     const size_t cap = (size_t)d->capacity;
-    auto take = [&](size_t bytes) { size_t o = off; off += align_up(bytes, 256); return o; };
-    size_t o_tag = take(cap * 4), o_k0 = take(cap * 8), o_k1 = take(cap * 8), o_cnt = take(cap * 8), o_acc = take(cap * 8 * (d->nagg > 0 ? d->nagg : 1));
-    if (s && base) {
-        char* b = (char*)base;
-        s->tag = (unsigned*)(b + o_tag); s->k0 = (unsigned long long*)(b + o_k0); s->k1 = (unsigned long long*)(b + o_k1);
-        s->cnt = (long long*)(b + o_cnt); s->acc = (double*)(b + o_acc);
-    }
-    return off;
+    s.tag = c.take<unsigned>(cap);
+    s.k0 = c.take<unsigned long long>(cap);
+    s.k1 = c.take<unsigned long long>(cap);
+    s.cnt = c.take<long long>(cap);
+    s.acc = c.take<double>(cap * (d->nagg > 0 ? d->nagg : 1));
+    return c.bytes;
 }
 
 int make_layout(const qk_hashagg_desc* d, KeyLayout* L, const char* who) {
@@ -178,14 +176,15 @@ using namespace qk;
 
 extern "C" size_t qk_hashagg_state_bytes(const qk_hashagg_desc* desc) {
     if (!desc || desc->capacity <= 0) return 0;
-    return carve(desc, nullptr, nullptr);
+    State S;
+    return carve(desc, nullptr, S);
 }
 
 extern "C" int qk_hashagg_init(const qk_hashagg_desc* desc, void* state, void* stream) {
     KeyLayout L;
     if (int rc = make_layout(desc, &L, "qk_hashagg_init")) return rc;
     if (!state || ((uintptr_t)state & 15)) QK_FAIL(QK_ERR_INVALID, "qk_hashagg_init: state must be a 16-byte aligned device buffer");
-    State S; carve(desc, state, &S);
+    State S; carve(desc, state, S);
     k_ha_init<<<grid_size(desc->capacity, 16), 256, 0, (cudaStream_t)stream>>>(S, desc->capacity, desc->nagg, *desc);
     QK_LAUNCH_CHECK("k_ha_init");
     return QK_OK;
@@ -211,7 +210,7 @@ extern "C" int qk_hashagg_update(const qk_hashagg_desc* desc, void* state, const
     }
     U.nagg = desc->nagg;
     if (nrows == 0) return QK_OK;
-    State S; carve(desc, state, &S);
+    State S; carve(desc, state, S);
     k_ha_update<<<grid_size(nrows, 16), 256, 0, (cudaStream_t)stream>>>(S, (uint64_t)desc->capacity - 1, L, U, nrows, overflow);
     QK_LAUNCH_CHECK("k_ha_update");
     return QK_OK;
@@ -237,7 +236,7 @@ extern "C" int qk_hashagg_finalize(const qk_hashagg_desc* desc, const void* stat
     F.nagg = desc->nagg;
     cudaStream_t st = (cudaStream_t)stream;
     QK_CUDA(cudaMemsetAsync(out_groups, 0, sizeof(int64_t), st));
-    State S; carve(desc, (void*)state, &S);
+    State S; carve(desc, (void*)state, S);
     k_ha_finalize<<<grid_size(desc->capacity, 16), 256, 0, st>>>(S, desc->capacity, L, F, (long long*)out_cnt, out_capacity, (unsigned long long*)out_groups);
     QK_LAUNCH_CHECK("k_ha_finalize");
     return QK_OK;

@@ -386,6 +386,18 @@ int launch_scan(const KnnArgs& A, cudaStream_t st) {
     return vec ? launch_cfg<T, true, Large>(A, st) : launch_cfg<T, false, Large>(A, st);
 }
 
+// the workspace: every row slice's k best scores per probe, then their rows, then 256 spare bytes
+struct KnnWs {
+    int row_ctas; float* score; int32_t* row; size_t bytes;
+    KnnWs(int64_t n, int q, int k, void* base) : row_ctas(n > 0 ? row_ctas_for(n, q, k) : 0) {
+        Carve c(base);
+        score = c.take<float>((size_t)row_ctas * q * k);
+        row = c.take<int32_t>((size_t)row_ctas * q * k);
+        c.take<char>(256);                              // spare
+        bytes = c.bytes;
+    }
+};
+
 }  // namespace
 }  // namespace qk
 
@@ -393,8 +405,7 @@ using namespace qk;
 
 extern "C" size_t qk_knn_workspace_bytes(int64_t n, int32_t d, int32_t q, int32_t k) {
     if (n < 0 || d < 1 || q < 1 || k < 1 || k > QK_KNN_MAX_K) return 0;
-    const int rc = n > 0 ? row_ctas_for(n, q, k) : 0;
-    return align_up((size_t)rc * q * k * 4, 256) * 2 + 256;
+    return KnnWs(n, q, k, nullptr).bytes;
 }
 
 extern "C" int qk_knn_topk(const qk_column* x, const float* probes, int32_t q, int32_t k, float* out_score, int64_t* out_row,
@@ -407,14 +418,14 @@ extern "C" int qk_knn_topk(const qk_column* x, const float* probes, int32_t q, i
     if (q < 1) QK_FAIL(QK_ERR_INVALID, "%s: q must be >= 1", who);
     if (k < 1 || k > QK_KNN_MAX_K) QK_FAIL(QK_ERR_INVALID, "%s: k must be in [1, %d]", who, QK_KNN_MAX_K);
     if (!probes || !out_score || !out_row) QK_FAIL(QK_ERR_INVALID, "%s: null probes / outputs", who);
-    const size_t need = qk_knn_workspace_bytes(x->length, d, q, k);
-    if (!workspace || ws_bytes < need) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace of %zu bytes, %zu needed", who, ws_bytes, need);
+    const KnnWs w(x->length, q, k, workspace);
+    if (!workspace || ws_bytes < w.bytes) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace of %zu bytes, %zu needed", who, ws_bytes, w.bytes);
     cudaStream_t st = (cudaStream_t)stream;
     KnnArgs A;
     A.x = x->data; A.probes = probes; A.n = x->length; A.d = d; A.q = q; A.k = k;
-    A.ws_score = (float*)workspace;
-    A.ws_row = (int32_t*)((char*)workspace + (need - 256) / 2);
-    A.row_ctas = x->length > 0 ? row_ctas_for(x->length, q, k) : 0;
+    A.ws_score = w.score;
+    A.ws_row = w.row;
+    A.row_ctas = w.row_ctas;
     if (A.row_ctas > 0) {
         if (int rc = x->dtype == QK_F32 ? launch_scan<float>(A, st) : launch_scan<unsigned short>(A, st)) return rc;
     }

@@ -435,7 +435,13 @@ int qk_parquet_walk_pages(const uint8_t* bytes, int64_t chunk_offset, int64_t ch
     return QK_OK;
 }
 
-size_t qk_parquet_inflate_slot_bytes(void) { return ZSTD_SLOT_BYTES; }
+// one slot per ZSTD / GZIP page in flight: at most 8 per SM, in whole CTAs
+size_t qk_parquet_inflate_workspace_bytes(int64_t n_zstd_pages) {
+    if (n_zstd_pages <= 0) return 0;
+    const int64_t cap = (int64_t)qk::sm_count() * 8;
+    const int64_t slots = n_zstd_pages < cap ? n_zstd_pages : cap;
+    return (size_t)((slots + INFLATE_WARPS - 1) / INFLATE_WARPS * INFLATE_WARPS) * ZSTD_SLOT_BYTES;
+}
 
 int qk_parquet_inflate(const uint8_t* bytes, int64_t n_bytes, qk_pq_page* pages, int64_t n_pages, uint8_t* scratch,
                        int64_t scratch_bytes, void* work, int64_t work_bytes, void* stream) {

@@ -181,17 +181,20 @@ int fill_move(MoveArgs& M, const qk_column* cols, int ncols, qk_column* out, int
     return 0;
 }
 
-}  // namespace
-}  // namespace qk
-
-using namespace qk;
-
-// workspace of one shared-memory partition (nparts <= P_SMEM_PARTS)
-static size_t smem_plan_bytes(int64_t nrows, int32_t nparts) {
-    const int64_t cr = chunk_rows_for(nrows, nparts);
-    const int64_t nchunks = (nrows + cr - 1) / cr + 1;
-    return align_up((size_t)nchunks * nparts * 4, 256) + align_up((size_t)nchunks * nparts * 8, 256) + align_up((size_t)nparts * 8, 256);
-}
+// workspace of one shared-memory partition (nparts <= P_SMEM_PARTS): the partition-major per-chunk histogram, its offsets
+// (one spare chunk each) and every partition's total
+struct SmemPlanWs {
+    unsigned* hist; int64_t* offsets; int64_t* totals; size_t bytes;
+    SmemPlanWs(int64_t nrows, int32_t nparts, void* base) {
+        const int64_t cr = chunk_rows_for(nrows, nparts);
+        const int64_t nchunks = (nrows + cr - 1) / cr + 1;
+        Carve c(base);
+        hist = c.take<unsigned>((size_t)nchunks * nparts);
+        offsets = c.take<int64_t>((size_t)nchunks * nparts);
+        totals = c.take<int64_t>(nparts);
+        bytes = c.bytes;
+    }
+};
 
 // partitions of the radix pass that handles the digit at `shift` (the top digit needs fewer than P_SMEM_PARTS)
 static int radix_pass_parts(int32_t nparts, int shift) {
@@ -205,20 +208,34 @@ static int radix_passes(int32_t nparts) {
     return (bits + P_DIGIT_BITS - 1) / P_DIGIT_BITS;
 }
 
-// radix path: digit, pass destination, two code buffers (n x int32 each), the pass's part_offsets, then one
-// shared-memory partition's workspace
-static size_t radix_plan_bytes(int64_t nrows, int32_t nparts) {
-    size_t inner = 0;
-    for (int d = 0; d < radix_passes(nparts); ++d) {
-        const size_t b = smem_plan_bytes(nrows, radix_pass_parts(nparts, d * P_DIGIT_BITS));
-        inner = b > inner ? b : inner;
+// workspace of the radix path: digit, pass destination, two code buffers (n x int32 each), the pass's part_offsets, then
+// the largest workspace of one pass's shared-memory partition
+struct RadixPlanWs {
+    int32_t* digit; int32_t* pass_dest; int32_t* codes[2]; int64_t* pass_offsets; void* inner; size_t bytes;
+    RadixPlanWs(int64_t nrows, int32_t nparts, void* base) {
+        size_t inner_bytes = 0;
+        for (int d = 0; d < radix_passes(nparts); ++d) {
+            const size_t b = SmemPlanWs(nrows, radix_pass_parts(nparts, d * P_DIGIT_BITS), nullptr).bytes;
+            inner_bytes = b > inner_bytes ? b : inner_bytes;
+        }
+        Carve c(base);
+        digit = c.take<int32_t>(nrows);
+        pass_dest = c.take<int32_t>(nrows);
+        for (int b = 0; b < 2; ++b) codes[b] = c.take<int32_t>(nrows);
+        pass_offsets = c.take<int64_t>(P_SMEM_PARTS + 1);
+        inner = c.take<char>(inner_bytes);
+        bytes = c.bytes;
     }
-    return 4 * align_up((size_t)nrows * 4, 256) + align_up((size_t)(P_SMEM_PARTS + 1) * 8, 256) + inner;
-}
+};
+
+}  // namespace
+}  // namespace qk
+
+using namespace qk;
 
 extern "C" size_t qk_partition_workspace_bytes(int64_t nrows, int32_t nparts) {
     if (nrows < 0 || nparts <= 0) return 0;
-    return nparts <= P_SMEM_PARTS ? smem_plan_bytes(nrows, nparts) : radix_plan_bytes(nrows, nparts);
+    return nparts <= P_SMEM_PARTS ? SmemPlanWs(nrows, nparts, nullptr).bytes : RadixPlanWs(nrows, nparts, nullptr).bytes;
 }
 
 // one stable partition with its per-chunk histograms in shared memory (nparts <= P_SMEM_PARTS)
@@ -227,21 +244,19 @@ static int smem_plan(const qk_column* key, int32_t nparts, int32_t mode, int32_t
     const int64_t n = key->length;
     const int64_t chunk_rows = chunk_rows_for(n, nparts);
     const int64_t nchunks = (n + chunk_rows - 1) / chunk_rows;
-    unsigned* hist = (unsigned*)workspace;
-    int64_t* offsets = (int64_t*)((char*)workspace + align_up((size_t)(nchunks + 1) * nparts * 4, 256));
-    int64_t* totals = (int64_t*)((char*)offsets + align_up((size_t)(nchunks + 1) * nparts * 8, 256));
+    const SmemPlanWs w(n, nparts, workspace);
     const unsigned nb = grid_size(nchunks, 8, 1);                      // grid-stride over the chunks
     const size_t smem = (size_t)nparts * 4;
     QK_CUDA(cudaFuncSetAttribute(k_part_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_part_hist<<<nb, P_NT, smem, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, hist);
+    k_part_hist<<<nb, P_NT, smem, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, w.hist);
     QK_LAUNCH_CHECK("k_part_hist");
     // pass 2: every partition's per-chunk counts (a row of the partition-major histogram) -> offsets relative to the
     // partition's start and the partition's total; then the totals -> part_offsets[nparts + 1]
-    if (int rc = count_offsets(hist, nparts, nchunks, offsets, totals, st)) return rc;
-    if (int rc = count_offsets(totals, 1, nparts, part_offsets, part_offsets + nparts, st)) return rc;
+    if (int rc = count_offsets(w.hist, nparts, nchunks, w.offsets, w.totals, st)) return rc;
+    if (int rc = count_offsets(w.totals, 1, nparts, part_offsets, part_offsets + nparts, st)) return rc;
     const size_t smem_dest = (size_t)nparts * 12;
     QK_CUDA(cudaFuncSetAttribute(k_part_dest, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_dest));
-    k_part_dest<<<nb, P_NT, smem_dest, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, offsets, part_offsets, dest);
+    k_part_dest<<<nb, P_NT, smem_dest, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, w.offsets, part_offsets, dest);
     QK_LAUNCH_CHECK("k_part_dest");
     return QK_OK;
 }
@@ -250,27 +265,22 @@ static int smem_plan(const qk_column* key, int32_t nparts, int32_t mode, int32_t
 // low digit first, then part_offsets by binary search in the sorted codes
 static int radix_plan(const qk_column* key, int32_t nparts, int32_t* dest, int64_t* part_offsets, void* workspace, cudaStream_t st) {
     const int64_t n = key->length;
-    char* w = (char*)workspace;
-    const size_t col_bytes = align_up((size_t)n * 4, 256);
-    int32_t* digit = (int32_t*)w; w += col_bytes;
-    int32_t* pass_dest = (int32_t*)w; w += col_bytes;
-    int32_t* codes[2] = {(int32_t*)w, (int32_t*)(w + col_bytes)}; w += 2 * col_bytes;
-    int64_t* pass_offsets = (int64_t*)w; w += align_up((size_t)(P_SMEM_PARTS + 1) * 8, 256);
+    const RadixPlanWs w(n, nparts, workspace);
     const unsigned grid = grid_size(n, 16);
     const void* src = key->data;
     int src_dt = key->dtype;
     const int passes = radix_passes(nparts);
     for (int d = 0; d < passes; ++d) {
         const int shift = d * P_DIGIT_BITS;
-        k_radix_digit<<<grid, 256, 0, st>>>(src, src_dt, n, nparts, shift, digit);
+        k_radix_digit<<<grid, 256, 0, st>>>(src, src_dt, n, nparts, shift, w.digit);
         QK_LAUNCH_CHECK("k_radix_digit");
         qk_column dcol = *key;
-        dcol.data = digit; dcol.dtype = QK_I32;
-        int32_t* out = d == 0 ? dest : pass_dest;
-        if (int rc = smem_plan(&dcol, radix_pass_parts(nparts, shift), QK_PART_CODE, out, pass_offsets, w, st)) return rc;
-        k_radix_move<<<grid, 256, 0, st>>>(src, src_dt, n, nparts, out, codes[d & 1], dest, d > 0);
+        dcol.data = w.digit; dcol.dtype = QK_I32;
+        int32_t* out = d == 0 ? dest : w.pass_dest;
+        if (int rc = smem_plan(&dcol, radix_pass_parts(nparts, shift), QK_PART_CODE, out, w.pass_offsets, w.inner, st)) return rc;
+        k_radix_move<<<grid, 256, 0, st>>>(src, src_dt, n, nparts, out, w.codes[d & 1], dest, d > 0);
         QK_LAUNCH_CHECK("k_radix_move");
-        src = codes[d & 1]; src_dt = QK_I32;
+        src = w.codes[d & 1]; src_dt = QK_I32;
     }
     k_radix_offsets<<<grid_size((int64_t)nparts + 1, 16), 256, 0, st>>>((const int32_t*)src, n, nparts, part_offsets);
     QK_LAUNCH_CHECK("k_radix_offsets");

@@ -1197,13 +1197,38 @@ static int launch_dyn(DyArgs& D, const DenseArgs& A, int64_t nrows, double* part
 
 constexpr int MAX_PART_BLOCKS = 1024;
 
+// the stable path's workspace: per-chunk survivor counts and their offsets (one spare chunk each)
+struct StableWs {
+    uint32_t* counts; int64_t* offsets; size_t bytes;
+    StableWs(int64_t nrows, void* base) {
+        const int64_t nchunks = (nrows + STABLE_CHUNK - 1) / STABLE_CHUNK + 1;
+        Carve c(base);
+        counts = c.take<uint32_t>(nchunks);
+        offsets = c.take<int64_t>(nchunks);
+        bytes = c.bytes;
+    }
+};
+
+// the dense aggregate's workspace: every partial block's accumulators and counts
+struct DenseAggWs {
+    double* part_acc; long long* part_cnt; size_t bytes;
+    DenseAggWs(int64_t n_groups, int32_t nagg, void* base) {
+        Carve c(base);
+        part_acc = c.take<double>((size_t)MAX_PART_BLOCKS * n_groups * (nagg > 0 ? nagg : 1));
+        part_cnt = c.take<long long>((size_t)MAX_PART_BLOCKS * n_groups);
+        bytes = c.bytes;
+    }
+};
+
 }  // namespace
 }  // namespace qk
 
 using namespace qk;
 
 namespace qk {
-// compact.cu: TMA-staged filter + column compaction; returns 1 when the request does not fit the fast path
+// compact.cu: TMA-staged filter + column compaction; returns 1 when the request does not fit the fast path (also when
+// the workspace is smaller than compact_workspace_bytes(nrows))
+size_t compact_workspace_bytes(int64_t nrows);
 int try_filter_compact_tma(const qk_column* cols, int ncols, int64_t nrows, const qk_expr* pred, const qk_expr* proj, int nproj,
                            qk_column* out, int64_t* out_rows, void* workspace, size_t ws_bytes, const qk_bloom* bloom, cudaStream_t st);
 int bloom_build(const qk_column* key, unsigned* bits, long long words_per_part, int nparts, cudaStream_t st);
@@ -1213,11 +1238,8 @@ extern "C" const char* qk_last_variant(void) { return g_variant.c_str(); }
 extern "C" const char* qk_last_variant_config(void) { return g_variant_cfg.c_str(); }
 
 extern "C" size_t qk_scan_workspace_bytes(int64_t nrows) {
-    const int64_t nchunks = (nrows + STABLE_CHUNK - 1) / STABLE_CHUNK + 1;
-    const size_t generic = align_up((size_t)nchunks * 4, 256) + align_up((size_t)nchunks * 8, 256);
-    // chunk counts + offsets + the 1-bit-per-row survivor bitmap of the TMA compaction path
-    const size_t compact = (size_t)(2 * 1024 + 8) * 8 + align_up((size_t)((nrows + 31) / 32 + 8) * 4, 256);
-    return generic > compact ? generic : compact;
+    const size_t stable = StableWs(nrows, nullptr).bytes, compact = compact_workspace_bytes(nrows);
+    return stable > compact ? stable : compact;
 }
 
 extern "C" int qk_bloom_build(const qk_column* key, uint32_t* bits, int64_t words_per_part, int32_t nparts, void* stream) {
@@ -1279,21 +1301,20 @@ static int scan_filter_project_impl(const qk_column* cols, int32_t ncols, int64_
         return QK_OK;
     }
     const int64_t nchunks = (nrows + STABLE_CHUNK - 1) / STABLE_CHUNK;
-    if (ws_bytes < qk_scan_workspace_bytes(nrows) || !workspace) QK_FAIL(QK_ERR_CAPACITY, "qk_scan_filter_project: workspace too small (%zu < %zu)", ws_bytes, qk_scan_workspace_bytes(nrows));
-    uint32_t* counts = (uint32_t*)workspace;
-    int64_t* offsets = (int64_t*)((char*)workspace + align_up((size_t)(nchunks + 1) * 4, 256));
+    const StableWs w(nrows, workspace);
+    const size_t need = qk_scan_workspace_bytes(nrows);               // one size for both paths: at least this layout's
+    if (ws_bytes < need || !workspace) QK_FAIL(QK_ERR_CAPACITY, "qk_scan_filter_project: workspace too small (%zu < %zu)", ws_bytes, need);
     const unsigned nb = grid_size(nchunks, 8, 1);                      // grid-stride over the chunks
-    k_filter_count<<<nb, 256, 0, st>>>(P, nrows, counts);
+    k_filter_count<<<nb, 256, 0, st>>>(P, nrows, w.counts);
     QK_LAUNCH_CHECK("k_filter_count");
-    if (int rc = count_offsets(counts, 1, nchunks, offsets, out_rows, st)) return rc;
-    k_filter_project_stable<<<nb, 256, 0, st>>>(P, O, nproj, nrows, offsets);
+    if (int rc = count_offsets(w.counts, 1, nchunks, w.offsets, out_rows, st)) return rc;
+    k_filter_project_stable<<<nb, 256, 0, st>>>(P, O, nproj, nrows, w.offsets);
     QK_LAUNCH_CHECK("k_filter_project_stable");
     return QK_OK;
 }
 
 extern "C" size_t qk_scan_agg_workspace_bytes(int32_t n_groups, int32_t nagg) {
-    if (n_groups <= 0 || nagg < 0) return 0;
-    return align_up((size_t)MAX_PART_BLOCKS * n_groups * (nagg > 0 ? nagg : 1) * 8, 256) + align_up((size_t)MAX_PART_BLOCKS * n_groups * 8, 256);
+    return n_groups <= 0 || nagg < 0 ? 0 : DenseAggWs(n_groups, nagg, nullptr).bytes;
 }
 
 extern "C" int qk_scan_filter_agg_dense(const qk_column* cols, int32_t ncols, int64_t nrows, const qk_expr* pred,
@@ -1325,9 +1346,10 @@ extern "C" int qk_scan_filter_agg_dense(const qk_column* cols, int32_t ncols, in
         A.agg_op[j] = agg_op[j];
     }
     if (nrows == 0) return QK_OK;
-    if (!workspace || ws_bytes < qk_scan_agg_workspace_bytes((int)ng, nagg)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
-    double* part_acc = (double*)workspace;
-    long long* part_cnt = (long long*)((char*)workspace + align_up((size_t)MAX_PART_BLOCKS * ng * (nagg > 0 ? nagg : 1) * 8, 256));
+    const DenseAggWs w(ng, nagg, workspace);
+    if (!workspace || ws_bytes < w.bytes) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
+    double* part_acc = w.part_acc;
+    long long* part_cnt = w.part_cnt;
     cudaStream_t st = (cudaStream_t)stream;
     int nblocks = 0;
     bool done = false;

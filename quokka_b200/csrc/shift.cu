@@ -98,14 +98,24 @@ __global__ void __launch_bounds__(256) k_shift_gather(const __grid_constant__ Ga
     }
 }
 
+// the keyed plan's workspace: the inverse permutation, then 256 spare bytes
+struct ShiftWs {
+    int32_t* inv; size_t bytes;
+    ShiftWs(int64_t n, void* base) {
+        Carve c(base);
+        inv = c.take<int32_t>(n);
+        c.take<char>(256);                              // spare
+        bytes = c.bytes;
+    }
+};
+
 }  // namespace
 }  // namespace qk
 
 using namespace qk;
 
 extern "C" size_t qk_shift_workspace_bytes(int64_t nrows) {
-    if (nrows < 0) return 0;
-    return align_up((size_t)nrows * 4, 256) + 256;
+    return nrows < 0 ? 0 : ShiftWs(nrows, nullptr).bytes;
 }
 
 extern "C" int qk_shift_plan(const int32_t* by, int32_t n_by, const int32_t* dest, const int64_t* seg, int64_t nrows, int64_t n,
@@ -125,8 +135,9 @@ extern "C" int qk_shift_plan(const int32_t* by, int32_t n_by, const int32_t* des
     if (nrows == 0) return QK_OK;
     int32_t* inv = nullptr;
     if (by) {
-        if (!workspace || ws_bytes < qk_shift_workspace_bytes(nrows)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
-        inv = (int32_t*)workspace;
+        const ShiftWs w(nrows, workspace);
+        if (!workspace || ws_bytes < w.bytes) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
+        inv = w.inv;
         k_shift_invert<<<grid_size(nrows, 16), 256, 0, st>>>(dest, inv, nrows);
         QK_LAUNCH_CHECK("k_shift_invert");
     }

@@ -218,6 +218,21 @@ __global__ void __launch_bounds__(256) k_sort_finish(const SortState* S, const u
     }
 }
 
+// the workspace: both (image, row number) buffers, the plan, then the per-chunk bin counts, their offsets and the bin totals
+struct SortWs {
+    unsigned long long* img[2]; unsigned* row[2]; SortState* S; unsigned* counts; int64_t* offsets; int64_t* totals; size_t bytes;
+    SortWs(int64_t n, void* base) {
+        Carve c(base);
+        for (int b = 0; b < 2; ++b) img[b] = c.take<unsigned long long>(n);
+        for (int b = 0; b < 2; ++b) row[b] = c.take<unsigned>(n);
+        S = c.take<SortState>(1);
+        counts = c.take<unsigned>((size_t)S_MAX_CHUNKS * 256);
+        offsets = c.take<int64_t>((size_t)S_MAX_CHUNKS * 256);
+        totals = c.take<int64_t>(256);
+        bytes = c.bytes;
+    }
+};
+
 thread_local char g_sort_plan_text[48] = "";
 thread_local int g_sort_device = -1;
 
@@ -234,9 +249,7 @@ static int64_t sort_chunk_rows(int64_t n) {
 }
 
 extern "C" size_t qk_sort_workspace_bytes(int64_t nrows) {
-    if (nrows < 0) return 0;
-    return 2 * align_up((size_t)nrows * 8, 256) + 2 * align_up((size_t)nrows * 4, 256) + align_up(sizeof(SortState), 256) +
-           align_up((size_t)S_MAX_CHUNKS * 256 * 4, 256) + align_up((size_t)S_MAX_CHUNKS * 256 * 8, 256) + 256 * 8;
+    return nrows < 0 ? 0 : SortWs(nrows, nullptr).bytes;
 }
 
 extern "C" int qk_sort_perm(const qk_column* key, const uint8_t* valid, int32_t descending, const int32_t* perm_in,
@@ -248,35 +261,27 @@ extern "C" int qk_sort_perm(const qk_column* key, const uint8_t* valid, int32_t 
     const int64_t n = nrows;
     if (n == 0) return QK_OK;
     if (!perm_out) QK_FAIL(QK_ERR_INVALID, "%s: null perm_out", who);
-    if (!workspace || ws_bytes < qk_sort_workspace_bytes(n)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
+    const SortWs w(n, workspace);
+    if (!workspace || ws_bytes < w.bytes) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
     cudaStream_t st = (cudaStream_t)stream;
-    char* w = (char*)workspace;
-    unsigned long long* img[2];
-    unsigned* row[2];
-    for (int b = 0; b < 2; ++b) { img[b] = (unsigned long long*)w; w += align_up((size_t)n * 8, 256); }
-    for (int b = 0; b < 2; ++b) { row[b] = (unsigned*)w; w += align_up((size_t)n * 4, 256); }
-    SortState* S = (SortState*)w; w += align_up(sizeof(SortState), 256);
-    unsigned* counts = (unsigned*)w; w += align_up((size_t)S_MAX_CHUNKS * 256 * 4, 256);
-    int64_t* offsets = (int64_t*)w; w += align_up((size_t)S_MAX_CHUNKS * 256 * 8, 256);
-    int64_t* totals = (int64_t*)w;
     // the digits below the key's width are the same in every image; the NULL digit exists only with a mask
     const int d_lo = 8 - dtype_size(key->dtype), d_hi = valid ? 9 : 8;
-    QK_CUDA(cudaMemsetAsync(S->hist, 0, sizeof(S->hist), st));
-    k_sort_image_hist<<<grid_size(n, 8), 256, 0, st>>>(key->data, key->dtype, valid, descending, perm_in, n, d_lo, d_hi, img[0], row[0], S);
+    QK_CUDA(cudaMemsetAsync(w.S->hist, 0, sizeof(w.S->hist), st));
+    k_sort_image_hist<<<grid_size(n, 8), 256, 0, st>>>(key->data, key->dtype, valid, descending, perm_in, n, d_lo, d_hi, w.img[0], w.row[0], w.S);
     QK_LAUNCH_CHECK("k_sort_image_hist");
-    k_sort_plan<<<1, 256, 0, st>>>(S, n, d_lo, d_hi, descending ? 0xff : 0);
+    k_sort_plan<<<1, 256, 0, st>>>(w.S, n, d_lo, d_hi, descending ? 0xff : 0);
     QK_LAUNCH_CHECK("k_sort_plan");
     const int64_t chunk_rows = sort_chunk_rows(n), nchunks = (n + chunk_rows - 1) / chunk_rows;
     QK_CUDA(cudaFuncSetAttribute(k_sort_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S_SCATTER_SMEM));
     for (int d = d_lo; d < d_hi; ++d) {
-        k_sort_count<<<(unsigned)nchunks, S_NT, 0, st>>>(S, d, img[0], img[1], row[0], row[1], n, chunk_rows, nchunks, counts);
+        k_sort_count<<<(unsigned)nchunks, S_NT, 0, st>>>(w.S, d, w.img[0], w.img[1], w.row[0], w.row[1], n, chunk_rows, nchunks, w.counts);
         QK_LAUNCH_CHECK("k_sort_count");
-        if (int rc = count_offsets(counts, 256, nchunks, offsets, totals, st)) return rc;
-        k_sort_scatter<<<(unsigned)nchunks, S_NT, S_SCATTER_SMEM, st>>>(S, d, img[0], img[1], row[0], row[1], perm_out,
-                                                                       (unsigned long long*)image_out, n, chunk_rows, nchunks, offsets);
+        if (int rc = count_offsets(w.counts, 256, nchunks, w.offsets, w.totals, st)) return rc;
+        k_sort_scatter<<<(unsigned)nchunks, S_NT, S_SCATTER_SMEM, st>>>(w.S, d, w.img[0], w.img[1], w.row[0], w.row[1], perm_out,
+                                                                       (unsigned long long*)image_out, n, chunk_rows, nchunks, w.offsets);
         QK_LAUNCH_CHECK("k_sort_scatter");
     }
-    k_sort_finish<<<grid_size(n, 8), 256, 0, st>>>(S, img[0], row[0], perm_out, (unsigned long long*)image_out, n);
+    k_sort_finish<<<grid_size(n, 8), 256, 0, st>>>(w.S, w.img[0], w.row[0], perm_out, (unsigned long long*)image_out, n);
     QK_LAUNCH_CHECK("k_sort_finish");
     cudaGetDevice(&g_sort_device);
     return QK_OK;

@@ -70,14 +70,24 @@ __global__ void __launch_bounds__(256) k_topk_emit(const unsigned long long* img
     }
 }
 
+// the workspace: every row's order image, then the selection state
+struct TopkWs {
+    unsigned long long* img; SelState* S; size_t bytes;
+    TopkWs(int64_t n, void* base) {
+        Carve c(base);
+        img = c.take<unsigned long long>(n);
+        S = c.take<SelState>(1);
+        bytes = c.bytes;
+    }
+};
+
 }  // namespace
 }  // namespace qk
 
 using namespace qk;
 
 extern "C" size_t qk_topk_workspace_bytes(int64_t nrows) {
-    if (nrows < 0) return 0;
-    return align_up((size_t)nrows * 8, 256) + align_up(sizeof(SelState), 256);
+    return nrows < 0 ? 0 : TopkWs(nrows, nullptr).bytes;
 }
 
 extern "C" int qk_topk_candidates(const qk_column* key, int32_t k, int32_t descending, int32_t* out_idx,
@@ -91,9 +101,10 @@ extern "C" int qk_topk_candidates(const qk_column* key, int32_t k, int32_t desce
     const int64_t n = key->length;
     if (n == 0) return QK_OK;
     if (!out_idx) QK_FAIL(QK_ERR_INVALID, "%s: null out_idx", who);
-    if (!workspace || ws_bytes < qk_topk_workspace_bytes(n)) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
-    unsigned long long* img = (unsigned long long*)workspace;
-    SelState* S = (SelState*)((char*)workspace + align_up((size_t)n * 8, 256));
+    const TopkWs w(n, workspace);
+    if (!workspace || ws_bytes < w.bytes) QK_FAIL(QK_ERR_CAPACITY, "%s: workspace too small", who);
+    unsigned long long* img = w.img;
+    SelState* S = w.S;
     const unsigned nb = grid_size(n, 8);
     k_topk_image<<<nb, 256, 0, st>>>(key->data, key->dtype, n, descending, img);
     QK_LAUNCH_CHECK("k_topk_image");

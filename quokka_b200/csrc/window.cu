@@ -111,6 +111,17 @@ __global__ void __launch_bounds__(S_NT) k_scan_apply(const int32_t* in, int64_t 
     }
 }
 
+// the session workspace: one new-session flag per row, then one sum per tile and the total (scanned in place to offsets)
+struct SessionWs {
+    int32_t* flag; int64_t* sums; size_t bytes;
+    SessionWs(int64_t n, void* base) {
+        Carve c(base);
+        flag = c.take<int32_t>(n);
+        sums = c.take<int64_t>((n + S_TILE - 1) / S_TILE + 1);
+        bytes = c.bytes;
+    }
+};
+
 }  // namespace
 }  // namespace qk
 
@@ -168,8 +179,7 @@ extern "C" int qk_window_hop_expand(const qk_column* time, const qk_column* by, 
 }
 
 extern "C" size_t qk_window_session_workspace_bytes(int64_t nrows) {
-    if (nrows < 0) return 0;
-    return align_up((size_t)nrows * 4, 256) + align_up((size_t)((nrows + S_TILE - 1) / S_TILE + 1) * 8, 256);
+    return nrows < 0 ? 0 : SessionWs(nrows, nullptr).bytes;
 }
 
 extern "C" int qk_window_session_ids(const qk_column* time, const qk_column* by, int64_t timeout, int64_t* ids, void* workspace,
@@ -179,9 +189,10 @@ extern "C" int qk_window_session_ids(const qk_column* time, const qk_column* by,
     if (timeout < 0) QK_FAIL(QK_ERR_INVALID, "%s: negative timeout", who);
     const int64_t n = time->length;
     if (n == 0) return QK_OK;
-    if (!ids || !workspace || ws_bytes < qk_window_session_workspace_bytes(n)) QK_FAIL(QK_ERR_CAPACITY, "%s: null output / workspace too small", who);
-    int32_t* flag = (int32_t*)workspace;
-    int64_t* sums = (int64_t*)((char*)workspace + align_up((size_t)n * 4, 256));    // nb + 1: offsets, then the total
+    const SessionWs w(n, workspace);
+    if (!ids || !workspace || ws_bytes < w.bytes) QK_FAIL(QK_ERR_CAPACITY, "%s: null output / workspace too small", who);
+    int32_t* flag = w.flag;
+    int64_t* sums = w.sums;                                                           // nb + 1: offsets, then the total
     cudaStream_t st = (cudaStream_t)stream;
     k_win_session_flag<<<grid_size(n, 16), 256, 0, st>>>((const long long*)time->data, (const int32_t*)by->data, n, timeout, flag);
     QK_LAUNCH_CHECK("k_win_session_flag");

@@ -786,14 +786,10 @@ def parquet_decode(raw: torch.Tensor, runs: torch.Tensor, n_runs: int, n_values:
 
 
 def parquet_inflate_workspace(n_zstd_pages: int, device) -> torch.Tensor | None:
-    """Workspace for the ZSTD / GZIP pages of one inflate call: one slot (decoding tables + literals buffer) per page in flight,
-    at most 8 per SM, in whole CTAs.  None when the call has no ZSTD page."""
-    if n_zstd_pages <= 0:
-        return None
-    slot = int(L.lib().qk_parquet_inflate_slot_bytes())
-    slots = min(n_zstd_pages, 8 * int(L.lib().qk_sm_count()))
-    slots = (slots + L.PQ_INFLATE_WARPS - 1) // L.PQ_INFLATE_WARPS * L.PQ_INFLATE_WARPS
-    return torch.empty(slots * slot, dtype=torch.uint8, device=device)
+    """Workspace for the ZSTD / GZIP pages of one inflate call, as qk_parquet_inflate_workspace_bytes sizes it.  None when the
+    call has no ZSTD page."""
+    nbytes = int(L.lib().qk_parquet_inflate_workspace_bytes(n_zstd_pages))
+    return torch.empty(nbytes, dtype=torch.uint8, device=device) if nbytes else None
 
 
 def parquet_inflate(raw: torch.Tensor, pages: torch.Tensor, n_pages: int, scratch: torch.Tensor, work: torch.Tensor | None = None):
