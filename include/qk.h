@@ -304,6 +304,24 @@ QK_API int qk_join_build(void* table, int64_t capacity, const qk_column* key, in
  * retries with a larger buffer).  semi/anti write probe indices only.  Pair order is unspecified. */
 QK_API int qk_join_probe(const void* table, int64_t capacity, const qk_column* key, int32_t how, int32_t* out_probe_idx,
                   int32_t* out_build_idx, int64_t out_capacity, int64_t* out_count, void* stream);
+/* Ordered probe, behind DataStream.join(maintain_sort_order="left" | "right") (pyquokka/datastream.py:1453-1469, :1536-1553,
+ * where the reference keeps the order by joining batch by batch in its executor).  The same table, arguments and pairs as
+ * qk_join_probe, in a fixed order: by probe row, a row's matches in ascending build-row number; a left join's unmatched row
+ * is one pair with build -1; semi / anti write probe indices only, ascending.  Deterministic for any number of matches per
+ * row.  *out_count = total pairs (may exceed out_capacity: then nothing past out_capacity is written and the caller retries).
+ * Workspace: qk_join_probe_ordered_workspace_bytes(key->length) (16 B per probe row; too small: QK_ERR_CAPACITY). */
+QK_API size_t qk_join_probe_ordered_workspace_bytes(int64_t nrows);
+QK_API int qk_join_probe_ordered(const void* table, int64_t capacity, const qk_column* key, int32_t how, int32_t* out_probe_idx,
+                                 int32_t* out_build_idx, int64_t out_capacity, int64_t* out_count, void* workspace,
+                                 size_t ws_bytes, void* stream);
+/* Placement of an ordered join's rows that come back to the rank holding the left rows: pos (device int32[nrecv]) = the left
+ * position of every received row, in [0, nleft); each sender's run is ascending and all rows of one position are contiguous.
+ * Output row d, in left order (rows of one position in the order they arrived): out_src[d] = the received row,
+ * out_left[d] (optional) = its position; nrecv rows in all.  Deterministic, no sort.
+ * Workspace: qk_join_place_workspace_bytes(nleft) (16 B per left row; too small: QK_ERR_CAPACITY). */
+QK_API size_t qk_join_place_workspace_bytes(int64_t nleft);
+QK_API int qk_join_place(const int32_t* pos, int64_t nrecv, int64_t nleft, int32_t* out_src, int32_t* out_left, void* workspace,
+                         size_t ws_bytes, void* stream);
 
 /* ---- K7: backward as-of join by key ---------------------------------------------------------
  * Replaces Polars `join_asof(by=..., strategy="backward")` in SortedAsofExecutor

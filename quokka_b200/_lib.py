@@ -117,6 +117,11 @@ _SIGNATURES = {
     "qk_join_build": (C.c_int, [C.c_void_p, C.c_int64, _P(qk_column), C.c_int32, C.c_void_p, C.c_void_p]),
     "qk_join_probe": (C.c_int, [C.c_void_p, C.c_int64, _P(qk_column), C.c_int32, C.c_void_p, C.c_void_p,
                                 C.c_int64, C.c_void_p, C.c_void_p]),
+    "qk_join_probe_ordered_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "qk_join_probe_ordered": (C.c_int, [C.c_void_p, C.c_int64, _P(qk_column), C.c_int32, C.c_void_p, C.c_void_p,
+                                        C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "qk_join_place_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "qk_join_place": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "qk_asof_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32]),
     "qk_asof_backward": (C.c_int, [_P(qk_column), _P(qk_column), _P(qk_column), _P(qk_column), C.c_int32,
                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

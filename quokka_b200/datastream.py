@@ -16,7 +16,7 @@ import pyarrow as pa
 from . import _lib as L
 from . import expr as E
 from .edge import EdgeOps, PartialAgg
-from .executors import (BuildProbeJoinExecutor, ConcatThenSQLExecutor, DistinctExecutor, OutputExecutor,
+from .executors import (BuildProbeJoinExecutor, ConcatThenSQLExecutor, DistinctExecutor, OrderedJoinExecutor, OutputExecutor,
                         SortedAsofExecutor, SortExecutor, SQLAggExecutor, top_k_table)
 from .placement_strategy import CustomChannelsStrategy, SingleChannelStrategy
 from .target_info import BroadcastPartitioner, HashPartitioner, PassThroughPartitioner, TargetInfo
@@ -132,11 +132,12 @@ class RenameNode(Node):
 class JoinNode(Node):
     kind = "join"
 
-    def __init__(self, left, right, left_on, right_on, how, suffix):
+    def __init__(self, left, right, left_on, right_on, how, suffix, maintain_sort_order=None):
         _reject_vectors(left.vectors, [left_on], "join key")
         _reject_vectors(right.vectors, [right_on], "join key")
         _reject_vectors(left.vectors | right.vectors, left.vectors | right.vectors, "join (hash-partitioned edge)")
         self.left_on, self.right_on, self.how, self.suffix = left_on, right_on, how, suffix
+        self.maintain_sort_order = maintain_sort_order      # None, or the side ("left" / "right") whose order the rows keep
         if how in ("semi", "anti"):
             schema, self.right_names = list(left.schema), {}
         else:
@@ -191,10 +192,11 @@ class SortNode(Node):
 
 def ends_in_sort(node: Node) -> bool:
     """True when the rows of `node` are a sort's output seen through row-wise operators (filter / select / rename / map), or
-    the output of an executor that keeps its rows in stream order (`ordered_output`, e.g. shift)."""
+    the output of an executor that keeps its rows in stream order (`ordered_output`, e.g. shift, or an order-preserving join)."""
     while node.kind in ("filter", "select", "rename", "map"):
         node = node.parents[0]
-    return node.kind == "sort" or (node.kind == "stateful" and bool(getattr(node.executor, "ordered_output", False)))
+    return (node.kind == "sort" or (node.kind == "stateful" and bool(getattr(node.executor, "ordered_output", False)))
+            or (node.kind == "join" and node.maintain_sort_order is not None))
 
 
 class DistinctNode(Node):
@@ -267,7 +269,9 @@ def push_filters(node: Node, pending: list) -> Node:
                 rp.append(E.rename(p, renamed))
             else:
                 stay.append(p)
-        j = JoinNode(push_filters(left, lp), push_filters(right, rp), node.left_on, node.right_on, node.how, node.suffix)
+        # an order-preserving join's edges are stable, so filters pushed below it keep both sides' order
+        j = JoinNode(push_filters(left, lp), push_filters(right, rp), node.left_on, node.right_on, node.how, node.suffix,
+                     node.maintain_sort_order)
         return wrap(j, stay)
     # barriers: aggregates, top-k, distinct, as-of, custom executors
     new_parents = [push_filters(p, []) for p in node.parents]
@@ -403,17 +407,15 @@ class Lowering:
         if keep != vis:
             ops.select(keep, raw)
 
-    def _join(self, node: JoinNode, need, stage):
-        left, right = node.parents
+    def _join_needs(self, node: JoinNode, need):
+        left = node.parents[0]
         need_all = set(node.schema) if need is None else set(need)
         need_left = {c for c in left.schema if c in need_all} | {node.left_on}
         inv = {v: k for k, v in node.right_names.items()}
-        need_right = {inv[c] for c in need_all if c in inv} | {node.right_on}
-        swap = node.how == "inner" and right.est_rows() > left.est_rows() and not (set(left.schema) & set(right.schema))
-        probe, build = (right, left) if swap else (left, right)
-        probe_on, build_on = (node.right_on, node.left_on) if swap else (node.left_on, node.right_on)
-        need_probe, need_build = (need_right, need_left) if swap else (need_left, need_right)
-        pa_, pops, praw = self.lower(probe, need_probe, stage)
+        return need_left, {inv[c] for c in need_all if c in inv} | {node.right_on}
+
+    def _replicate(self, probe: Node, build: Node):
+        """(tiny, broadcast): whether the build side is small enough to replicate outright, and whether it is replicated."""
         cfg = getattr(self.g.context, "exec_config", {}) if self.g.context is not None else {}
         tiny = build.est_rows() <= cfg.get("broadcast_rows", BROADCAST_ROWS)
         # Cost-based replication (opt-in): shuffling moves probe + build rows once; replicating moves the build rows to
@@ -422,7 +424,30 @@ class Lowering:
         from .runtime import world_size as _ws
         replicate = (cfg.get("broadcast_cost_based", False) and _ws() > 1 and build.est_rows() <= cfg.get("broadcast_max_rows", 1 << 26)
                      and build.est_rows() * _ws() <= probe.est_rows())
-        broadcast = tiny or replicate
+        return tiny, tiny or replicate
+
+    @staticmethod
+    def _join_renames(node: JoinNode, lvis: list, rvis: list) -> dict:
+        """Output names of the right columns the executor appended after the left ones ("_right" on clashes)."""
+        mapping = {}
+        for c in rvis:
+            produced = c + "_right" if c in lvis else c
+            if node.right_names.get(c, c) != produced:
+                mapping[produced] = node.right_names[c]
+        return mapping
+
+    def _join(self, node: JoinNode, need, stage):
+        if node.maintain_sort_order is not None:
+            return self._ordered_join(node, need, stage)
+        left, right = node.parents
+        need_left, need_right = self._join_needs(node, need)
+        swap = node.how == "inner" and right.est_rows() > left.est_rows() and not (set(left.schema) & set(right.schema))
+        probe, build = (right, left) if swap else (left, right)
+        probe_on, build_on = (node.right_on, node.left_on) if swap else (node.left_on, node.right_on)
+        need_probe, need_build = (need_right, need_left) if swap else (need_left, need_right)
+        pa_, pops, praw = self.lower(probe, need_probe, stage)
+        cfg = getattr(self.g.context, "exec_config", {}) if self.g.context is not None else {}
+        tiny, broadcast = self._replicate(probe, build)
         want_bloom = (not tiny and node.how in ("inner", "semi") and cfg.get("bloom_join", True)
                       and probe.est_rows() >= 2 * max(1, build.est_rows()))
         # Transitive semi-join reduction: if the probe side is itself an inner join and this join's key comes
@@ -459,10 +484,36 @@ class Lowering:
             if probe_on != node.left_on:
                 mapping[probe_on] = node.left_on       # the user's left key names the surviving key column
         else:
-            for c in bvis:
-                produced = c + "_right" if c in pvis else c
-                if node.right_names.get(c, c) != produced:
-                    mapping[produced] = node.right_names[c]
+            mapping = self._join_renames(node, pvis, bvis)
+        if mapping:
+            ops.rename(mapping, raw)
+        return aid, ops, raw
+
+    def _ordered_join(self, node: JoinNode, need, stage):
+        """join(maintain_sort_order=side): the ordered side is the probe and never leaves its rank (a stable pass-through
+        edge); the build side is replicated or hash-partitioned by the rule of the unordered join.  The sides are never
+        swapped and no Bloom filter reduces the probe side."""
+        left, right = node.parents
+        need_left, need_right = self._join_needs(node, need)
+        keep_left = node.maintain_sort_order == "left"
+        probe, build = (left, right) if keep_left else (right, left)
+        probe_on, build_on = (node.left_on, node.right_on) if keep_left else (node.right_on, node.left_on)
+        need_probe, need_build = (need_left, need_right) if keep_left else (need_right, need_left)
+        pa_, pops, praw = self.lower(probe, need_probe, stage)
+        ba_, bops, braw = self.lower(build, need_build, stage - 1)
+        self._prune(pops, praw, need_probe)
+        self._prune(bops, braw, need_build)
+        _, broadcast = self._replicate(probe, build)
+        from .runtime import world_size as _ws
+        ti0 = TargetInfo(PassThroughPartitioner(), None, None, [], edge_ops=pops, stable=True)
+        ti1 = TargetInfo(BroadcastPartitioner() if broadcast else HashPartitioner(build_on), None, None, [], edge_ops=bops, stable=True)
+        ex = OrderedJoinExecutor(probe_on, build_on, node.how, keep_left, streaming=broadcast or _ws() == 1)
+        aid = self.g.new_non_blocking_node({0: pa_, 1: ba_}, ex, stage, CustomChannelsStrategy(1), {0: ti0, 1: ti1})
+        pvis, bvis = pops.visible(praw), bops.visible(braw)
+        lvis, rvis = (pvis, [c for c in bvis if c != build_on]) if keep_left else (bvis, [c for c in pvis if c != probe_on])
+        raw = list(lvis) + [c + "_right" if c in lvis else c for c in rvis]
+        ops = EdgeOps()
+        mapping = self._join_renames(node, lvis, rvis)
         if mapping:
             ops.rename(mapping, raw)
         return aid, ops, raw
@@ -611,7 +662,23 @@ class DataStream:
 
     # ---- joins
     def join(self, right, on=None, left_on=None, right_on=None, suffix="_2", how="inner", maintain_sort_order=None):
-        """pyquokka/datastream.py:1420-1603: single-column equi-join, how in inner/left/semi/anti."""
+        """pyquokka/datastream.py:1420-1603: single-column equi-join, how in inner/left/semi/anti.  `right` is a DataStream, a
+        pyarrow.Table or a pandas DataFrame.  Without maintain_sort_order the rows come out in no fixed order.
+
+        maintain_sort_order="left" (:1453-1469): this stream must be an OrderedStream.  The rows follow its order -- rank
+        order, then arrival order, the order collect() returns -- and the matches of one left row follow the right stream's
+        order; a left join's unmatched row keeps its place with NULL right columns.  The result is an OrderedStream sorted
+        by what this stream is sorted by.
+        maintain_sort_order="right" (:1536-1553): how="inner" only, and `right` must be an OrderedStream.  The rows follow
+        the right stream's order, a right row's matches follow this stream's order; the columns are the same as without
+        it.  The result is sorted by the right stream's sort column under its output name (the left key when that column
+        is the right key, which the output drops).
+        Either way the ordered side stays on its rank.  With a build side too large to replicate, the other ranks see only
+        its keys and positions, and the matches come back to it (OrderedJoinExecutor); the rank then holds its share of the
+        ordered side in device memory until the build side is complete.
+        Deviations from the reference: how="left" with "right" raises NotImplementedError (an unmatched left row has no
+        place in the right stream's order; the reference allows only that combination); how="left", "semi" and "anti" with
+        "left" are accepted (the reference asserts them away)."""
         assert how in {"inner", "left", "semi", "anti"}
         if on is not None:
             assert left_on is None and right_on is None
@@ -621,7 +688,24 @@ class DataStream:
             right = self.quokka_context.from_arrow(right if isinstance(right, pa.Table) else pa.Table.from_pandas(right))
         assert left_on in self.schema, f"join key {left_on} not in left schema"
         assert right_on in right.schema, f"join key {right_on} not in right schema"
-        return DataStream(self.quokka_context, JoinNode(self.node, right.node, left_on, right_on, how, suffix))
+        if maintain_sort_order is None:
+            return DataStream(self.quokka_context, JoinNode(self.node, right.node, left_on, right_on, how, suffix))
+        if maintain_sort_order == "left":
+            assert isinstance(self, OrderedStream), "maintain_sort_order='left' needs this stream to be an OrderedStream"
+            node = JoinNode(self.node, right.node, left_on, right_on, how, suffix, "left")
+            return OrderedStream(self.quokka_context, node, self.sorted_by)
+        if maintain_sort_order == "right":
+            if how == "left":
+                raise NotImplementedError("join(how='left', maintain_sort_order='right'): an unmatched left row has no place "
+                                          "in the right stream's order")
+            assert how == "inner", "maintain_sort_order='right' is only supported for inner joins"
+            assert isinstance(right, OrderedStream), "maintain_sort_order='right' needs the right stream to be an OrderedStream"
+            node = JoinNode(self.node, right.node, left_on, right_on, how, suffix, "right")
+            sorted_by = right.sorted_by
+            if sorted_by is not None:
+                sorted_by = left_on if sorted_by == right_on else node.right_names[sorted_by]
+            return OrderedStream(self.quokka_context, node, sorted_by)
+        raise ValueError(f"maintain_sort_order must be None, 'left' or 'right', not {maintain_sort_order!r}")
 
     # ---- aggregation
     def groupby(self, groupby, orderby=None):
@@ -983,7 +1067,8 @@ class DataStream:
             print(self.quokka_context.plan(self.node).describe())
             return
         def walk(n, d=0):
-            extra = {"filter": lambda: n.pred.sql(), "join": lambda: f"{n.how} {n.left_on}={n.right_on}",
+            extra = {"filter": lambda: n.pred.sql(), "join": lambda: f"{n.how} {n.left_on}={n.right_on}"
+                     + (f" keeps {n.maintain_sort_order} order" if n.maintain_sort_order else ""),
                      "agg": lambda: f"keys={n.keys}", "topk": lambda: f"{n.by} k={n.k}",
                      "sort": lambda: ", ".join(c + (" desc" if d else "") for c, d in zip(n.by, n.desc)),
                      "stateful": lambda: getattr(n.executor, "explain", lambda: "")()}.get(n.kind, lambda: "")()

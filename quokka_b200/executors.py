@@ -217,16 +217,22 @@ class _HashedBuild:
         self.hashed.build(key.data.to(torch.int32) if key.dictionary is not None else _float_key(key.data))
         self.hashed.check_flags()
 
-    def probe(self, batch: DeviceTable, probe_on: str, how: str, suffix: str) -> DeviceTable:
-        key = _probe_key(batch[probe_on], self.table[self.on], f"join {probe_on} = {self.on}")
-        pi, bi = self.hashed.probe(key, _HOW[how])
-        out = batch.gather(pi)
-        if how in ("semi", "anti"):
-            return out
+    def key(self, batch: DeviceTable, probe_on: str) -> torch.Tensor:
+        return _probe_key(batch[probe_on], self.table[self.on], f"join {probe_on} = {self.on}")
+
+    def rows(self, bi: torch.Tensor, how: str) -> DeviceTable:
+        """The build rows `bi` without the key column; a left join's -1 rows are NULL."""
         right = self.table.drop([self.on]).gather(bi)
         if how == "left":
             right = right.with_validity((bi >= 0).to(torch.uint8))
-        return _append_right(out, right.columns, suffix)
+        return right
+
+    def probe(self, batch: DeviceTable, probe_on: str, how: str, suffix: str) -> DeviceTable:
+        pi, bi = self.hashed.probe(self.key(batch, probe_on), _HOW[how])
+        out = batch.gather(pi)
+        if how in ("semi", "anti"):
+            return out
+        return _append_right(out, self.rows(bi, how).columns, suffix)
 
 
 class BuildProbeJoinExecutor(Executor):
@@ -302,6 +308,132 @@ class BuildProbeJoinExecutor(Executor):
 
     def done(self, executor_id):
         pass
+
+
+class OrderedJoinExecutor(Executor):
+    """DataStream.join(maintain_sort_order=...) (pyquokka/datastream.py:1453-1469, :1536-1553): a hash join whose rows follow
+    the order of one side.  Stream 0 is that side (the probe; it never leaves its rank), stream 1 the build side, numbered in
+    the build stream's order (rank order, then arrival order).  The ordered probe (qk_join_probe_ordered) writes a probe row's
+    matches in build-row order, so the output is in probe order with each row's matches in build order.  With
+    probe_is_left the output is the probe's columns and the build's without its key; otherwise (maintain_sort_order="right",
+    inner only) the build's columns and the probe's without its key -- the unordered join's columns either way.
+      * streaming (the build side replicated, or one rank): every probe batch is joined as it arrives.
+      * otherwise (the build side hash-partitioned across ranks), in done(): each rank sends (key, position) of its probe
+        rows to the rank that owns the key's build rows; the owner probes what it received, source rank by source rank, and
+        answers every source with (position, build columns) -- positions only for semi / anti; the source puts the rows into
+        its order (qk_join_place) and gathers its own columns.  Only keys, positions and matched build rows cross ranks.  The
+        rank holds its whole probe side in device memory until then.
+    As in BuildProbeJoinExecutor, an anti join against an empty build side passes the probe side through and the other
+    joins emit nothing."""
+
+    ordered_output = True            # rows stay on their rank, in the probe side's order
+    POS = "__qk_pos"
+
+    def __init__(self, probe_on, build_on, how, probe_is_left=True, streaming=True) -> None:
+        assert how in {"inner", "left", "semi", "anti"} and (probe_is_left or how == "inner")
+        self.probe_on, self.build_on, self.how, self.probe_is_left, self.streaming = probe_on, build_on, how, probe_is_left, streaming
+        self.silent_streams = (1,) if streaming else "all"
+        self.emits_on_done = not streaming
+        self._right = _SourceRanks()
+        self._left = []
+        self._build, self._frozen = None, False
+
+    def explain(self) -> str:
+        return (f"ordered {self.how} join {self.probe_on} = {self.build_on}, keeps the {'left' if self.probe_is_left else 'right'} "
+                f"order, {'streaming' if self.streaming else 'keys to the owners and back'}")
+
+    def _freeze(self):
+        if not self._frozen:
+            t = self._right.take()
+            self._build = _HashedBuild(t, self.build_on) if t is not None and len(t) else None
+            self._frozen = True
+
+    def _payload(self, bi: torch.Tensor) -> DeviceTable:
+        """What the build side contributes to the output rows `bi`."""
+        return self._build.rows(bi, self.how) if self.probe_is_left else self._build.table.gather(bi)
+
+    def _combine(self, probe_rows: DeviceTable, payload: DeviceTable | None) -> DeviceTable:
+        """probe_rows: the probe side's rows of the output (all columns).  The output's columns in the unordered join's order."""
+        if payload is None:
+            return probe_rows
+        if self.probe_is_left:
+            return _append_right(probe_rows, payload.columns, "_right")
+        return _append_right(payload, probe_rows.drop([self.probe_on]).columns, "_right")
+
+    def _probe(self, keys: DeviceTable):
+        """(probe rows, build rows | None) of the ordered probe of `keys` (a table holding the probe key column)."""
+        return self._build.hashed.probe_ordered(self._build.key(keys, self.probe_on), _HOW[self.how])
+
+    def execute(self, batches, stream_id, executor_id):
+        batches = _clean(batches)
+        if stream_id == 1:
+            self._right.add(batches)
+            return None
+        if not batches:
+            return None
+        if not self.streaming:
+            self._left.extend(batches)
+            return None
+        batch = concat_tables(batches)
+        self._freeze()
+        if self._build is None:
+            return batch if self.how == "anti" else None
+        pi, bi = self._probe(batch)
+        return self._combine(batch.gather(pi), None if bi is None else self._payload(bi))
+
+    def done(self, executor_id):
+        return None if self.streaming else self._round_trip()
+
+    def _round_trip(self):
+        from . import runtime as RT
+        from .edge import apply_partitioner
+        from .target_info import HashPartitioner
+        w, me, dev = RT.world_size(), RT.rank(), default_device()
+        ex = RT.Exchange(dev)
+        P, self._left = (concat_tables(self._left) if self._left else None), []
+        self._freeze()
+        n = len(P) if P is not None else 0
+        # 1. (key, position) of every probe row to the rank that owns the key's build rows -- the build edge's partition
+        parts = {}
+        if n:
+            keys = DeviceTable({self.probe_on: P[self.probe_on], self.POS: DeviceColumn(torch.arange(n, dtype=torch.int32, device=dev))})
+            parts = apply_partitioner(HashPartitioner(self.probe_on), keys, me, w)
+        got = sorted(ex(parts, w, edge_key=("ordered-join-keys", id(self))), key=lambda g: g.src_rank)
+        # a left join's unmatched rows need the build columns' types where a rank owns no build rows: one row from any rank
+        # that has some (none anywhere: the build side is empty, and a left join emits nothing, as the unordered join does)
+        template = None
+        if self.how == "left":
+            one = self._build.rows(torch.zeros(1, dtype=torch.int32, device=dev), "inner") if self._build is not None else None
+            samples = ex({r: one for r in range(w)} if one is not None else {}, w, edge_key=("ordered-join-template", id(self)))
+            template = samples[0] if samples else None
+        # 2. the owner probes the received keys in source-rank order and answers each source with (position, build columns)
+        replies = {}
+        if got:
+            K = concat_tables(got)
+            reply = None
+            if self._build is not None:
+                pi, bi = self._probe(K)
+                reply = K.select([self.POS]).gather(pi)
+                if bi is not None:
+                    reply = _append_right(reply, self._payload(bi).columns, "")
+            elif self.how == "anti":
+                pi, reply = torch.arange(len(K), dtype=torch.int32, device=dev), K.select([self.POS])
+            elif self.how == "left" and template is not None:
+                pi = torch.arange(len(K), dtype=torch.int32, device=dev)
+                none = torch.full((len(K),), -1, dtype=torch.int32, device=dev)
+                reply = _append_right(K.select([self.POS]), template.gather(none).with_validity(torch.zeros(len(K), dtype=torch.uint8, device=dev)).columns, "")
+            if reply is not None and len(reply):
+                starts = torch.tensor([0] + [len(g) for g in got], device=dev).cumsum(0)
+                cut = torch.searchsorted(pi.to(torch.int64), starts).tolist()     # the reply is in source order
+                replies = {g.src_rank: reply.slice(cut[i], cut[i + 1]) for i, g in enumerate(got) if cut[i + 1] > cut[i]}
+        back = sorted(ex(replies, w, edge_key=("ordered-join-rows", id(self))), key=lambda g: g.src_rank)
+        # 3. the source puts what came back into its order and gathers its own columns
+        if not n or not back:
+            return None
+        B = concat_tables(back)
+        src, pos = ops.JoinTable.place(B[self.POS].data.to(torch.int32).contiguous(), n)
+        payload = None if self.how in ("semi", "anti") else B.drop([self.POS]).gather(src)
+        return self._combine(P.gather(pos), payload)
 
 
 class BroadcastJoinExecutor(Executor):

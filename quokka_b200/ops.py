@@ -424,6 +424,41 @@ class JoinTable:
                 return pi[:m], (bi[:m] if bi is not None else None)
             cap = m
 
+    def probe_ordered(self, key: torch.Tensor, how: int = L.JOIN_INNER, expect: int | None = None):
+        """probe() in a fixed order (qk_join_probe_ordered): by probe row, a row's matches in ascending build-row number (the
+        order the build rows arrived in), a left join's unmatched row once with build -1."""
+        n = key.numel()
+        cap = max(1, expect if expect is not None else n)
+        kc = col(key, "probe key")
+        ws = _ws(L.lib().qk_join_probe_ordered_workspace_bytes(n), key.device)
+        while True:
+            pi = torch.empty(cap, dtype=torch.int32, device=key.device)
+            bi = torch.empty(cap, dtype=torch.int32, device=key.device) if how in (L.JOIN_INNER, L.JOIN_LEFT) else None
+            cnt = torch.zeros(1, dtype=torch.int64, device=key.device)
+            L.check(L.lib().qk_join_probe_ordered(self.table.data_ptr(), self.capacity, C.byref(kc), how, pi.data_ptr(),
+                                                  bi.data_ptr() if bi is not None else None, cap, cnt.data_ptr(),
+                                                  ws.data_ptr(), ws.numel(), _stream()), "qk_join_probe_ordered")
+            m = int(cnt.item())
+            if m <= cap:
+                return pi[:m], (bi[:m] if bi is not None else None)
+            cap = m
+
+    @staticmethod
+    def place(pos: torch.Tensor, nleft: int) -> tuple[torch.Tensor, torch.Tensor]:
+        """Probe order for the pairs of an ordered probe that ran on other ranks (qk_join_place): pos (int32) = each received
+        row's probe position, ascending within each sender's run, one position's rows contiguous -> (src, left): output row d
+        is received row src[d], at probe position left[d]; positions in ascending order, one position's rows in arrival order."""
+        _require_cuda(pos, "join positions")
+        if pos.dtype != torch.int32:
+            raise L.QkError("JoinTable.place: positions must be int32")
+        n = pos.numel()
+        src = torch.empty(n, dtype=torch.int32, device=pos.device)
+        left = torch.empty(n, dtype=torch.int32, device=pos.device)
+        ws = _ws(L.lib().qk_join_place_workspace_bytes(nleft), pos.device)
+        L.check(L.lib().qk_join_place(pos.data_ptr(), n, nleft, src.data_ptr(), left.data_ptr(), ws.data_ptr(), ws.numel(), _stream()),
+                "qk_join_place")
+        return src, left
+
 
 # ------------------------------------------------------------------ K7 as-of
 def asof_backward(l_time: torch.Tensor, l_by: torch.Tensor, r_time: torch.Tensor, r_by: torch.Tensor, n_by: int):
