@@ -348,6 +348,40 @@ QK_API int qk_asof_merge(const qk_column* l_time, const qk_column* l_by, const q
                          int32_t n_by, const int32_t* carry_in, int32_t r_base, int32_t* carry_out, int32_t* out_ridx,
                          void* workspace, size_t ws_bytes, void* stream);
 
+/* As-of joins in the other directions, and with a match tolerance: OrderedStream.join_asof(strategy=..., tolerance=...)
+ * (pyquokka/orderedstream.py:114-191 offers backward only; the reference's apps/rottnest/backtester.py:60 fills every
+ * signal at the next trade tick with Polars' strategy="forward").  The target is pandas.merge_asof(direction=strategy,
+ * tolerance=tolerance):
+ *   QK_ASOF_BACKWARD  the LAST right row of the key with r_time <= l_time (the join above);
+ *   QK_ASOF_FORWARD   the FIRST right row of the key with r_time >= l_time (the earliest in stream order among equal times);
+ *   QK_ASOF_NEAREST   of the backward and the forward candidate the one with the smaller |r_time - l_time|; a distance tie goes
+ *                     to the backward one (an exact match takes the LAST right row at that time).
+ * tolerance >= 0 keeps the chosen row only if |r_time - l_time| <= tolerance (else -1); tolerance < 0 = none.  The nearest pick
+ * and the tolerance are applied where the answer is written. */
+#define QK_ASOF_BACKWARD 0
+#define QK_ASOF_FORWARD 1
+#define QK_ASOF_NEAREST 2
+/* The sorted-merge form (n_by within the shared-memory table; 0 from the sizing function otherwise, or for an unknown strategy).
+ * Forward is the mirror of qk_asof_merge's sweep: left rows first on merge-path ties, a table of the OLDEST right row at or after
+ * the current point, walked from the end.  Nearest runs both sweeps.  Local right rows are numbered r_base + i.
+ * carry_back (device int32[n_by] or NULL): the answer of a key with no local right row at or before l_time; its rows are below
+ * r_base.  carry_fwd: the same for no local right row at or after l_time; its rows are at or past r_base + n_right (and below
+ * 2^31 - 1).  carry_back_time / carry_fwd_time (device int64[n_by]) are the times of those rows, required with their table.
+ * Backward takes carry_back only, forward carry_fwd only, nearest both.  carry_out (device int32[n_by] or NULL; not for nearest):
+ * backward = the newest row of every key after this call's rows (as qk_asof_merge), forward = the OLDEST row of every key
+ * (local or carry_fwd), -1 none; n_left = 0 computes it alone.  Workspace: qk_asof_join_workspace_bytes (QK_ERR_CAPACITY when
+ * short, before any launch). */
+QK_API size_t qk_asof_join_workspace_bytes(int64_t n_left, int64_t n_right, int32_t n_by, int32_t strategy);
+QK_API int qk_asof_join(const qk_column* l_time, const qk_column* l_by, const qk_column* r_time, const qk_column* r_by,
+                        int32_t n_by, int32_t strategy, int64_t tolerance, const int32_t* carry_back, const int64_t* carry_back_time,
+                        const int32_t* carry_fwd, const int64_t* carry_fwd_time, int32_t r_base, int32_t* carry_out,
+                        int32_t* out_ridx, void* workspace, size_t ws_bytes, void* stream);
+/* The partition + search form for any n_by (the large symbol sets): lower bound for forward, both neighbours of the upper
+ * bound for nearest, the tolerance at the write.  out_ridx[i] = right row, or -1.  Workspace: qk_asof_workspace_bytes. */
+QK_API int qk_asof_search_join(const qk_column* l_time, const qk_column* l_by, const qk_column* r_time, const qk_column* r_by,
+                               int32_t n_by, int32_t strategy, int64_t tolerance, int32_t* out_ridx, void* workspace,
+                               size_t ws_bytes, void* stream);
+
 /* ---- time-series windows over a key-segmented, time-sorted stream ------------------------------------------------
  * Replace Polars groupby_rolling / groupby_dynamic and the DuckDB window SQL of HoppingWindowExecutor,
  * SlidingWindowExecutor and SessionWindowExecutor (pyquokka/executors/ts_executors.py:12-288).  Inputs are in KEY-SEGMENTED

@@ -18,6 +18,7 @@ AGG_SUM, AGG_MIN, AGG_MAX = 1, 2, 3
 WIN_SUM, WIN_MIN, WIN_MAX, WIN_COUNT, WIN_AVG = 1, 2, 3, 4, 5
 PART_MOD, PART_CODE = 0, 1
 JOIN_INNER, JOIN_LEFT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3
+ASOF_BACKWARD, ASOF_FORWARD, ASOF_NEAREST = 0, 1, 2
 MAX_COLS, MAX_AGGS, MAX_PROJ = 16, 8, 16
 MAX_EXPR_NODES, MAX_TOTAL_NODES, MAX_STACK = 48, 112, 8      # include/qk.h QK_MAX_EXPR_NODES / csrc/scan.cu MAX_NODES / QK_MAX_STACK
 PQ_RUN_PLAIN, PQ_RUN_RLE, PQ_RUN_PACKED, PQ_RUN_BOOL = 0, 1, 2, 3
@@ -128,6 +129,12 @@ _SIGNATURES = {
     "qk_asof_merge_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int32]),
     "qk_asof_merge": (C.c_int, [_P(qk_column), _P(qk_column), _P(qk_column), _P(qk_column), C.c_int32, C.c_void_p, C.c_int32,
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "qk_asof_join_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int32, C.c_int32]),
+    "qk_asof_join": (C.c_int, [_P(qk_column), _P(qk_column), _P(qk_column), _P(qk_column), C.c_int32, C.c_int32, C.c_int64,
+                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_size_t, C.c_void_p]),
+    "qk_asof_search_join": (C.c_int, [_P(qk_column), _P(qk_column), _P(qk_column), _P(qk_column), C.c_int32, C.c_int32, C.c_int64,
+                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "qk_window_sliding": (C.c_int, [_P(qk_column), _P(qk_column), C.c_void_p, C.c_int32, C.c_int64, _P(qk_column), C.c_int32, _P(C.c_int32),
                                     _P(C.c_int32), C.c_int32, _P(qk_column), C.c_void_p]),
     "qk_window_hop_expand": (C.c_int, [_P(qk_column), _P(qk_column), C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_void_p,

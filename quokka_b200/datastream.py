@@ -17,7 +17,7 @@ from . import _lib as L
 from . import expr as E
 from .edge import EdgeOps, PartialAgg
 from .executors import (BuildProbeJoinExecutor, ConcatThenSQLExecutor, DistinctExecutor, OrderedJoinExecutor, OutputExecutor,
-                        SortedAsofExecutor, SortExecutor, SQLAggExecutor, top_k_table)
+                        SortedAsofExecutor, SortExecutor, SQLAggExecutor, check_asof_args, top_k_table)
 from .placement_strategy import CustomChannelsStrategy, SingleChannelStrategy
 from .target_info import BroadcastPartitioner, HashPartitioner, PassThroughPartitioner, TargetInfo
 
@@ -211,7 +211,7 @@ class DistinctNode(Node):
 class AsofNode(Node):
     kind = "asof"
 
-    def __init__(self, left, right, left_on, right_on, left_by, right_by, suffix):
+    def __init__(self, left, right, left_on, right_on, left_by, right_by, suffix, strategy="backward", tolerance=None):
         _reject_vectors(left.vectors | right.vectors, left.vectors | right.vectors, "as-of join")
         schema = list(left.schema)
         self.right_names = {}
@@ -223,6 +223,7 @@ class AsofNode(Node):
             schema.append(name)
         super().__init__(schema, [left, right])
         self.left_on, self.right_on, self.left_by, self.right_by, self.suffix = left_on, right_on, left_by, right_by, suffix
+        self.strategy, self.tolerance = strategy, tolerance
 
 
 class StatefulNode(Node):
@@ -562,11 +563,13 @@ class Lowering:
             # (executors.SortedAsofExecutor._join_time_ranges) -- the reference's hash shuffle by symbol moves both streams
             ti0 = TargetInfo(PassThroughPartitioner(), None, None, [], edge_ops=lops, stable=True)
             ti1 = TargetInfo(PassThroughPartitioner(), None, None, [], edge_ops=rops, stable=True)
-            ex = SortedAsofExecutor(node.left_on, node.right_on, node.left_by, node.right_by, node.suffix, time_ranges=True)
+            ex = SortedAsofExecutor(node.left_on, node.right_on, node.left_by, node.right_by, node.suffix, time_ranges=True,
+                                    strategy=node.strategy, tolerance=node.tolerance)
         else:
             ti0 = TargetInfo(HashPartitioner(node.left_by), None, None, [], edge_ops=lops, stable=True)
             ti1 = TargetInfo(HashPartitioner(node.right_by), None, None, [], edge_ops=rops, stable=True)
-            ex = SortedAsofExecutor(node.left_on, node.right_on, node.left_by, node.right_by, node.suffix)
+            ex = SortedAsofExecutor(node.left_on, node.right_on, node.left_by, node.right_by, node.suffix, strategy=node.strategy,
+                                    tolerance=node.tolerance)
         aid = self.g.new_non_blocking_node({0: la, 1: ra}, ex, stage, CustomChannelsStrategy(1), {0: ti0, 1: ti1},
                                            assume_sorted={0: True, 1: True})
         return aid, EdgeOps(), list(node.schema)
@@ -1070,6 +1073,8 @@ class DataStream:
             extra = {"filter": lambda: n.pred.sql(), "join": lambda: f"{n.how} {n.left_on}={n.right_on}"
                      + (f" keeps {n.maintain_sort_order} order" if n.maintain_sort_order else ""),
                      "agg": lambda: f"keys={n.keys}", "topk": lambda: f"{n.by} k={n.k}",
+                     "asof": lambda: f"{n.left_on} by {n.left_by} strategy={n.strategy}"
+                     + (f" tolerance={n.tolerance}" if n.tolerance is not None else ""),
                      "sort": lambda: ", ".join(c + (" desc" if d else "") for c, d in zip(n.by, n.desc)),
                      "stateful": lambda: getattr(n.executor, "explain", lambda: "")()}.get(n.kind, lambda: "")()
             print("  " * d + f"{n.kind} {extra} -> {n.schema}")
@@ -1176,10 +1181,21 @@ class OrderedStream(DataStream):
         sorted_by = None if suffix is None and self.sorted_by in columns else self.sorted_by
         return OrderedStream(self.quokka_context, node, sorted_by)
 
-    def join_asof(self, right, on=None, left_on=None, right_on=None, by=None, left_by=None, right_by=None, suffix="_2"):
-        """Backward as-of join by key (orderedstream.py:114-191); `by` is mandatory (:127-128); the right
-        `on` / `by` columns are dropped from the output (:160-162)."""
+    def join_asof(self, right, on=None, left_on=None, right_on=None, by=None, left_by=None, right_by=None, suffix="_2",
+                  strategy="backward", tolerance=None):
+        """As-of join by key (orderedstream.py:114-191); `by` is mandatory (:127-128); the right `on` / `by` columns are
+        dropped from the output (:160-162).  Every left row is kept, in the left stream's order, with NULL right columns when
+        nothing matches.  As pandas.merge_asof(direction=strategy, tolerance=tolerance):
+          "backward"  the LAST right row with the same key and r_time <= l_time;
+          "forward"   the FIRST right row with the same key and r_time >= l_time (the earliest in stream order -- rank order,
+                      then arrival order -- among equal times);
+          "nearest"   of the backward and the forward candidate the one with the smaller |r_time - l_time|; a distance tie goes
+                      to the backward candidate, so an exact match takes the LAST right row at that time.
+        tolerance: None, or an int >= 0 in the time column's unit, or a datetime.timedelta for a timestamp time column; the
+        chosen row is kept only if |r_time - l_time| <= tolerance (for nearest: the pick first, then the tolerance).
+        Forward and nearest join when both inputs are complete: a rank's input must fit in device memory."""
         assert isinstance(right, OrderedStream), "join_asof needs two ordered streams"
+        check_asof_args(strategy, tolerance)
         if on is not None:
             assert left_on is None and right_on is None
             left_on = right_on = on
@@ -1188,7 +1204,7 @@ class OrderedStream(DataStream):
             left_by = right_by = by
         assert left_on is not None and right_on is not None
         assert left_by is not None and right_by is not None, "Must specify by or left_by and right_by"
-        node = AsofNode(self.node, right.node, left_on, right_on, left_by, right_by, suffix)
+        node = AsofNode(self.node, right.node, left_on, right_on, left_by, right_by, suffix, strategy, tolerance)
         return OrderedStream(self.quokka_context, node, self.sorted_by)
 
     def pattern_recognize(self, time_col, events, maxspan, by):

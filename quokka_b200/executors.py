@@ -1203,6 +1203,18 @@ def _time_unit(tcol: DeviceColumn) -> str | None:
 
 
 # ---------------------------------------------------------------------------------------------- as-of
+def check_asof_args(strategy, tolerance):
+    """join_asof's strategy and tolerance, as the time-unit conversion of pattern_recognize's maxspan accepts it."""
+    import datetime
+    if strategy not in ("backward", "forward", "nearest"):
+        raise ValueError(f"join_asof: strategy must be 'backward', 'forward' or 'nearest', not {strategy!r}")
+    if tolerance is not None:
+        if isinstance(tolerance, bool) or not isinstance(tolerance, (int, datetime.timedelta)):
+            raise ValueError("join_asof: tolerance must be None, an int in the time column's unit or a datetime.timedelta")
+        if (tolerance.total_seconds() if isinstance(tolerance, datetime.timedelta) else tolerance) < 0:
+            raise ValueError("join_asof: tolerance must be >= 0")
+
+
 class SortedAsofExecutor(Executor):
     """ts_executors.py:324-383: streaming backward as-of join of two time-sorted streams per symbol.
     stream 0 = trades (left), stream 1 = quotes (right).  A trade can be joined as soon as a quote NEWER
@@ -1213,19 +1225,39 @@ class SortedAsofExecutor(Executor):
     the newest quote.  The table is CARRIED between calls, so every quote row is swept once however the two streams
     are batched, and -- like the reference, which trims its quote state to the last quote per symbol (:371-376) -- quotes
     that can no longer be the newest of their symbol are dropped from the state.  Symbol sets too large for the
-    shared-memory table use the partition + search kernels (qk_asof_backward) over the whole quote state."""
+    shared-memory table use the partition + search kernels (qk_asof_backward) over the whole quote state.
+
+    strategy / tolerance (pandas.merge_asof's direction / tolerance): "backward" = the last quote of the symbol at or before
+    the trade; "forward" = the first quote at or after it (the earliest in stream order among equal times); "nearest" = of
+    those two the one closer in time, a distance tie going to the backward one.  tolerance (None, an int in the time
+    column's unit, or a datetime.timedelta for a timestamp column) keeps a match only if |quote time - trade time| <= it.
+    Backward with a tolerance streams as above (qk_asof_join).  Forward and nearest hold both streams and join in done():
+    a trade's forward match may be any later quote, so nothing can be released before the quotes end.
+
+    Across ranks over time ranges (_join_time_ranges), a trade goes to one owner rank:
+      * backward: the last rank whose first quote time <= t, carrying the newest quote per symbol of earlier ranks;
+      * forward: the first rank whose last quote time >= t, carrying the oldest quote per symbol of later ranks.  Equal quote
+        times may straddle a boundary (last of rank k == first of rank k + 1); the backward rule would then send a trade at
+        exactly that time to rank k + 1 and miss the first quotes at that time on rank k;
+      * nearest: the backward owner, with both carries.  (1) Its backward candidate is exact, as for backward.  (2) A forward
+        candidate later than t can only be on the owner or a later rank, since every earlier rank ends at or before the
+        owner's first quote <= t.  (3) A forward candidate AT t on an earlier rank means a quote of the symbol exactly at t:
+        then the backward candidate is at t too, its distance is 0 and it wins the tie.  So the owner sees both true
+        candidates."""
 
     TRIM_ROWS = 1 << 20          # fold swept quotes into <= n_symbols carried rows once this many have piled up
 
     @property
-    def silent_streams(self):      # across ranks over time ranges everything is held until done(); streaming otherwise
-        return "all" if self._over_time_ranges() else ()
+    def silent_streams(self):      # across ranks over time ranges, or forward / nearest: everything is held until done()
+        return "all" if self._over_time_ranges() or self.strategy != "backward" else ()
 
     def _over_time_ranges(self) -> bool:
         return bool(self.time_ranges) and world_size() > 1
 
     def __init__(self, time_col_trades="time", time_col_quotes="time", symbol_col_trades="symbol",
-                 symbol_col_quotes="symbol", suffix="_right", time_ranges=False) -> None:
+                 symbol_col_quotes="symbol", suffix="_right", time_ranges=False, strategy="backward", tolerance=None) -> None:
+        check_asof_args(strategy, tolerance)
+        self.strategy, self.tolerance = strategy, tolerance
         self.time_ranges = time_ranges   # several ranks, each holding a contiguous time range of both streams: join in place (done())
         self._held = None
         self.trade_state = None
@@ -1242,6 +1274,22 @@ class SortedAsofExecutor(Executor):
         self._by_source = None       # several producer ranks: {stream: _SourceRanks}, joined at done()
 
     BY = "__by"                      # hidden column: the symbol in the executor's code space
+
+    def explain(self) -> str:
+        return f"as-of join strategy={self.strategy}" + (f" tolerance={self.tolerance}" if self.tolerance is not None else "")
+
+    def _tolerance_ticks(self, tcol: DeviceColumn) -> int | None:
+        """The tolerance in the time column's unit (a timedelta needs a timestamp column)."""
+        import datetime
+        from .windowtypes import Window
+        if isinstance(self.tolerance, datetime.timedelta) and _time_unit(tcol) is None:
+            raise ValueError("join_asof: a timedelta tolerance needs a timestamp time column")
+        return None if self.tolerance is None else Window.ticks(self.tolerance, _time_unit(tcol))
+
+    def _strategy_args(self, tcol: DeviceColumn) -> dict:
+        """The keyword arguments of ops.asof_merge / asof_backward for this join: none for the plain backward join."""
+        tol = self._tolerance_ticks(tcol)
+        return {} if self.strategy == "backward" and tol is None else {"strategy": self.strategy, "tolerance": tol}
 
     def _append(self, state, batch, tcol):
         if state is None or len(state) == 0:
@@ -1267,10 +1315,18 @@ class SortedAsofExecutor(Executor):
         _require_int64_time(lt, rt)
         lby, rby = trades[self.BY].data, quotes[self.BY].data
         n_by = max(1, self._codes.n_by)
+        kw = self._strategy_args(trades[self.time_col_trades])
         ridx = None
-        if not self._whole_state:
+        if not self._whole_state and self.strategy != "backward":     # held until done(): one join over both whole streams
+            ridx, _ = ops.asof_merge(lt, lby, rt, rby, n_by, **kw)
+            self._whole_state = ridx is None
+        elif not self._whole_state:
             carry = self._carry_table(lt.device)
-            ridx, carry_out = ops.asof_merge(lt, lby, rt[self._swept:upto], rby[self._swept:upto], n_by, carry, self._swept, want_carry=True)
+            if kw:
+                kw["carry_time"] = rt[carry.clamp(min=0).long()] if len(rt) else torch.zeros(n_by, dtype=torch.int64, device=lt.device)
+            ridx, carry_out = ops.asof_merge(lt, lby, rt[self._swept:upto], rby[self._swept:upto], n_by, carry, self._swept, want_carry=True,
+                                             **kw)
+            kw.pop("carry_time", None)
             if ridx is None:
                 if self._swept:
                     raise L.QkError("as-of: the symbol set outgrew the merge kernel's table after quotes were trimmed")
@@ -1278,7 +1334,7 @@ class SortedAsofExecutor(Executor):
             else:
                 self._carry, self._swept = carry_out, upto
         if ridx is None:
-            ridx = ops.asof_backward(lt, lby, rt, rby, n_by)
+            ridx = ops.asof_backward(lt, lby, rt, rby, n_by, **kw)
         right = quotes.drop([self.time_col_quotes, self.symbol_col_quotes, self.BY]).gather(ridx)
         right = right.with_validity((ridx >= 0).to(torch.uint8))
         out = _append_right(trades.drop([self.BY]), right.columns, self.suffix)
@@ -1308,9 +1364,9 @@ class SortedAsofExecutor(Executor):
                 self._held = {0: [], 1: []}
             self._held[stream_id].extend(batches)
             return
-        if self._by_source is not None or any(getattr(b, "src_rank", None) is not None for b in batches):
+        if self._by_source is not None or self.strategy != "backward" or any(getattr(b, "src_rank", None) is not None for b in batches):
             # the batches come from several producer ranks: once one has said so, both streams are put back together
-            # per source rank (_SourceRanks) and joined when they are complete
+            # per source rank (_SourceRanks) and joined when they are complete; so are those of a forward / nearest join
             if self._by_source is None:
                 self._by_source = {0: _SourceRanks(), 1: _SourceRanks()}
             self._by_source[stream_id].add(batches)
@@ -1380,23 +1436,27 @@ class SortedAsofExecutor(Executor):
                     raise L.QkError(f"as-of join: the ranks do not hold consecutive time ranges of the sorted {what} stream")
                 if n:
                     last = end
-        # ---- newest quote per symbol of every rank, to everybody
-        newest = None
+        # ---- newest quote per symbol of every rank (backward, nearest), oldest (forward, nearest), to everybody
+        newest = oldest = None
         if quotes is not None and len(quotes) > 0:
             codes = self._codes.codes(quotes[self.symbol_col_quotes])
             n_by = max(1, self._codes.n_by)
-            empty_t, empty_b = torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int32, device=dev)
-            _, table = ops.asof_merge(empty_t, empty_b, quotes[qt].data, codes, n_by, want_carry=True)
-            if table is None:                                       # symbol set too large for the table: the last row of each code
-                order = torch.arange(len(codes), device=dev, dtype=torch.int64)
-                table = torch.full((n_by,), -1, dtype=torch.int64, device=dev).scatter_reduce(0, codes.long(), order, "amax", include_self=True)
-            idx = torch.sort(table[table >= 0]).values.to(torch.int32)          # row order = time order
-            newest = quotes.gather(idx)
-        got = ex({r: newest for r in range(w)} if newest is not None and len(newest) > 0 else {}, w, edge_key=("asof-newest", id(self)))
-        earlier = [g for g in sorted(got, key=lambda g: g.src_rank) if g.src_rank < me]
+            if self.strategy != "forward":
+                newest = quotes.gather(self._end_rows(quotes[qt].data, codes, n_by, forward=False))
+            if self.strategy != "backward":
+                oldest = quotes.gather(self._end_rows(quotes[qt].data, codes, n_by, forward=True))
+        earlier, later = [], []
+        if self.strategy != "forward":
+            got = ex({r: newest for r in range(w)} if newest is not None and len(newest) > 0 else {}, w, edge_key=("asof-newest", id(self)))
+            earlier = [g for g in sorted(got, key=lambda g: g.src_rank) if g.src_rank < me]
+        if self.strategy != "backward":
+            got = ex({r: oldest for r in range(w)} if oldest is not None and len(oldest) > 0 else {}, w, edge_key=("asof-oldest", id(self)))
+            later = [g for g in sorted(got, key=lambda g: g.src_rank) if g.src_rank > me]
         # ---- trades to the rank whose quote range holds them: the k-th rank that has quotes takes the trades from its first quote
         #      time up to the next such rank's (the first one also takes everything earlier: those trades match nothing, but
-        #      only a rank with quotes knows the columns to fill with NULLs); ranks without quotes take none
+        #      only a rank with quotes knows the columns to fill with NULLs); ranks without quotes take none.  Forward: the k-th
+        #      rank with quotes takes the trades after the previous such rank's last quote time up to its own (the last one
+        #      also takes everything later)
         owners = [r for r in range(w) if rows[r][4]]
         if not owners:
             if any(rows[r][0] for r in range(w)):
@@ -1404,8 +1464,9 @@ class SortedAsofExecutor(Executor):
             return None
         parts, own = {}, None
         if trades is not None and len(trades) > 0:
-            cuts = [rows[o][5] for o in owners[1:]]
-            pos = torch.searchsorted(trades[tt].data, torch.tensor(cuts, dtype=torch.int64, device=dev)).tolist() if cuts else []
+            fwd = self.strategy == "forward"
+            cuts = [rows[o][6] for o in owners[:-1]] if fwd else [rows[o][5] for o in owners[1:]]
+            pos = torch.searchsorted(trades[tt].data, torch.tensor(cuts, dtype=torch.int64, device=dev), right=fwd).tolist() if cuts else []
             ends = {o: int(p_) for o, p_ in zip(owners[:-1], pos)} | {owners[-1]: len(trades)}
             bounds = [0]
             for r in range(w):
@@ -1419,11 +1480,11 @@ class SortedAsofExecutor(Executor):
         mine = sorted(mine, key=lambda g: g.src_rank)
         self.trade_state = self.quote_state = None
         self._carry, self._swept, self._whole_state = None, 0, False
-        all_q = earlier + ([quotes] if quotes is not None and len(quotes) > 0 else [])
+        all_q = earlier + ([quotes] if quotes is not None and len(quotes) > 0 else []) + later
         if not mine:
             return None
         t = concat_tables(mine)
-        out = self._join_carried(t, earlier, quotes) if earlier and quotes is not None and len(quotes) > 0 else None
+        out = self._join_carried(t, earlier, later, quotes) if (earlier or later) and quotes is not None and len(quotes) > 0 else None
         if out is not None:
             return out
         q = concat_tables(all_q)
@@ -1431,39 +1492,76 @@ class SortedAsofExecutor(Executor):
         t = t.with_column(self.BY, DeviceColumn(self._codes.codes(t[self.symbol_col_trades])))
         return self._join(t, None)
 
-    def _join_carried(self, trades, earlier, quotes):
-        """trades joined against [the few carried rows of earlier ranks] + [this rank's quotes] WITHOUT putting the two into one
-        table (that copy is the whole quote shard): the carried rows become the merge kernel's carry-in table, the answer's row
-        numbers below len(carried) point into them, the others into the shard, and the payload is gathered from both.  None when
-        the shapes call for the plain path (dictionary payload columns that differ, symbol sets beyond the kernel's table)."""
-        E = concat_tables(earlier)
+    def _end_rows(self, time: torch.Tensor, codes: torch.Tensor, n_by: int, forward: bool) -> torch.Tensor:
+        """Rows (int32, in time order) of the newest quote of every symbol, or with `forward` the oldest: the merge kernel's
+        table pass (no left rows)."""
+        dev = time.device
+        empty_t, empty_b = torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int32, device=dev)
+        _, table = ops.asof_merge(empty_t, empty_b, time, codes, n_by, want_carry=True, **({"strategy": "forward"} if forward else {}))
+        if table is None:                                           # symbol set too large for the table: the last / first row of each code
+            order = torch.arange(len(codes), device=dev, dtype=torch.int64)
+            fill = len(codes) if forward else -1
+            table = torch.full((n_by,), fill, dtype=torch.int64, device=dev).scatter_reduce(0, codes.long(), order, "amin" if forward else "amax",
+                                                                                           include_self=True)
+            table = torch.where(table == len(codes), -1, table) if forward else table
+        return torch.sort(table[table >= 0]).values.to(torch.int32)          # row order = time order
+
+    def _join_carried(self, trades, earlier, later, quotes):
+        """trades joined against [the few carried rows of earlier ranks] + [this rank's quotes] + [those of later ranks] WITHOUT
+        putting them into one table (that copy is the whole quote shard): the carried rows become the merge kernel's carry
+        tables, the answer's row numbers below len(earlier rows) point into them, then the shard's, then the later ones, and the
+        payload is gathered from all three.  None when the shapes call for the plain path (dictionary payload columns that
+        differ, symbol sets beyond the kernel's table)."""
+        E = concat_tables(earlier) if earlier else None
+        F = concat_tables(later) if later else None
+        carried = [x for x in (E, F) if x is not None]
         payload = [c for c in quotes.column_names if c not in (self.time_col_quotes, self.symbol_col_quotes)]
-        if any((E[c].dictionary is not None or quotes[c].dictionary is not None) and E[c].dictionary != quotes[c].dictionary for c in payload):
+        if any((x[c].dictionary is not None or quotes[c].dictionary is not None) and x[c].dictionary != quotes[c].dictionary
+               for x in carried for c in payload):
             return None
-        sq, st_ = quotes[self.symbol_col_quotes], trades[self.symbol_col_trades]
-        if sq.dictionary is not None or st_.dictionary is not None or E[self.symbol_col_quotes].dictionary is not None:
-            both = concat_tables([E.select([self.symbol_col_quotes]), quotes.select([self.symbol_col_quotes])])     # one dictionary for both
-            codes = self._codes.codes(both[self.symbol_col_quotes])
-            e_codes, q_codes = codes[:len(E)], codes[len(E):]
+        sym = self.symbol_col_quotes
+        sq, st_ = quotes[sym], trades[self.symbol_col_trades]
+        parts = [x for x in (E, quotes, F) if x is not None]
+        if sq.dictionary is not None or st_.dictionary is not None or any(x[sym].dictionary is not None for x in carried):
+            both = concat_tables([x.select([sym]) for x in parts])     # one dictionary for all
+            codes = self._codes.codes(both[sym])
+            split = list(torch.split(codes, [len(x) for x in parts]))
         else:
-            e_codes, q_codes = self._codes.codes(E[self.symbol_col_quotes]), self._codes.codes(sq)
+            split = [self._codes.codes(x[sym]) for x in parts]
+        e_codes = split.pop(0) if E is not None else None
+        q_codes = split.pop(0)
+        f_codes = split.pop(0) if F is not None else None
         t_codes = self._codes.codes(st_)
         n_by, dev = max(1, self._codes.n_by), trades.device
         lt, rt = trades[self.time_col_trades].data, quotes[self.time_col_quotes].data
         _require_int64_time(lt, rt)
+        ne, nq = len(E) if E is not None else 0, len(quotes)
         none_t, none_b = torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int32, device=dev)
-        _, carried = ops.asof_merge(none_t, none_b, E[self.time_col_quotes].data, e_codes, n_by, want_carry=True)
-        if carried is None:
-            return None
-        ridx, _ = ops.asof_merge(lt, t_codes, rt, q_codes, n_by, carried, len(E))
+        kw = self._strategy_args(trades[self.time_col_trades])
+        back = fwd = None
+        if E is not None:
+            _, back = ops.asof_merge(none_t, none_b, E[self.time_col_quotes].data, e_codes, n_by, want_carry=True)
+            if back is None:
+                return None
+            if kw:
+                kw["carry_time"] = E[self.time_col_quotes].data[back.clamp(min=0).long()]
+        if F is not None:
+            _, fwd = ops.asof_merge(none_t, none_b, F[self.time_col_quotes].data, f_codes, n_by, None, ne + nq, want_carry=True,
+                                    strategy="forward")
+            if fwd is None:
+                return None
+            kw["carry_fwd"], kw["carry_fwd_time"] = fwd, F[self.time_col_quotes].data[(fwd - ne - nq).clamp(min=0).long()]
+        ridx, _ = ops.asof_merge(lt, t_codes, rt, q_codes, n_by, back, ne, **kw)
         if ridx is None:
             return None
-        in_shard = ridx >= len(E)
-        from_shard = quotes.select(payload).gather(torch.where(in_shard, ridx - len(E), torch.full_like(ridx, -1)))
-        from_carry = E.select(payload).gather(torch.where(in_shard, torch.full_like(ridx, -1), ridx))
+        in_shard = (ridx >= ne) & (ridx < ne + nq)
+        side = concat_tables([x.select(payload) for x in carried]) if len(carried) > 1 else carried[0].select(payload)
+        from_shard = quotes.select(payload).gather(torch.where(in_shard, ridx - ne, torch.full_like(ridx, -1)))
+        from_carry = side.gather(torch.where(in_shard, torch.full_like(ridx, -1), torch.where(ridx >= ne + nq, ridx - nq, ridx)))
         valid = (ridx >= 0).to(torch.uint8)
         if os.environ.get("QK_DEBUG_ASOF"):
-            print(f"[asof] carried join: {len(E)} carried rows, {int((~in_shard & (ridx >= 0)).sum())} answers from them", flush=True)
+            print(f"[asof] carried join: {ne + len(F) if F is not None else ne} carried rows, {int((~in_shard & (ridx >= 0)).sum())} answers from them",
+                  flush=True)
         right = {n: DeviceColumn(torch.where(in_shard, from_shard[n].data, from_carry[n].data), from_shard[n].dictionary,
                                  from_shard[n].arrow_type, valid) for n in payload}
         return _append_right(trades, right, self.suffix)

@@ -461,31 +461,60 @@ class JoinTable:
 
 
 # ------------------------------------------------------------------ K7 as-of
-def asof_backward(l_time: torch.Tensor, l_by: torch.Tensor, r_time: torch.Tensor, r_by: torch.Tensor, n_by: int):
+ASOF_STRATEGIES = {"backward": L.ASOF_BACKWARD, "forward": L.ASOF_FORWARD, "nearest": L.ASOF_NEAREST}
+
+
+def _asof_strategy(strategy: str) -> int:
+    if strategy not in ASOF_STRATEGIES:
+        raise ValueError(f"as-of strategy must be one of {sorted(ASOF_STRATEGIES)}, not {strategy!r}")
+    return ASOF_STRATEGIES[strategy]
+
+
+def asof_backward(l_time: torch.Tensor, l_by: torch.Tensor, r_time: torch.Tensor, r_by: torch.Tensor, n_by: int, *,
+                  strategy: str = "backward", tolerance: int | None = None):
+    """Partition + search as-of join, any n_by: out[i] = right row or -1.  The default is the backward join
+    (qk_asof_backward); another strategy or a tolerance (an int, inclusive) runs qk_asof_search_join."""
     out = torch.empty(l_time.numel(), dtype=torch.int32, device=l_time.device)
     ws = _ws(L.lib().qk_asof_workspace_bytes(r_time.numel(), n_by), l_time.device)
     a, b, c, d = col(l_time), col(l_by), col(r_time), col(r_by)
-    L.check(L.lib().qk_asof_backward(C.byref(a), C.byref(b), C.byref(c), C.byref(d), n_by, out.data_ptr(),
-                                     ws.data_ptr(), ws.numel(), _stream()), "qk_asof_backward")
+    if strategy == "backward" and tolerance is None:
+        L.check(L.lib().qk_asof_backward(C.byref(a), C.byref(b), C.byref(c), C.byref(d), n_by, out.data_ptr(),
+                                         ws.data_ptr(), ws.numel(), _stream()), "qk_asof_backward")
+        return out
+    L.check(L.lib().qk_asof_search_join(C.byref(a), C.byref(b), C.byref(c), C.byref(d), n_by, _asof_strategy(strategy),
+                                        -1 if tolerance is None else int(tolerance), out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                        _stream()), "qk_asof_search_join")
     return out
 
 
 def asof_merge(l_time: torch.Tensor, l_by: torch.Tensor, r_time: torch.Tensor, r_by: torch.Tensor, n_by: int,
-               carry_in: torch.Tensor | None = None, r_base: int = 0, want_carry: bool = False):
+               carry_in: torch.Tensor | None = None, r_base: int = 0, want_carry: bool = False, *, strategy: str = "backward",
+               tolerance: int | None = None, carry_time: torch.Tensor | None = None, carry_fwd: torch.Tensor | None = None,
+               carry_fwd_time: torch.Tensor | None = None):
     """Sorted-merge as-of join (qk_asof_merge): out[i] = r_base + (row of the newest right row with the same key and
     r_time <= l_time[i]) or carry_in[key] (or -1).  Returns (out, carry_out | None); None, None when n_by is too large
-    for the shared-memory table (the caller then uses asof_backward)."""
-    ws_bytes = L.lib().qk_asof_merge_workspace_bytes(l_time.numel(), r_time.numel(), n_by)
+    for the shared-memory table (the caller then uses asof_backward).
+    Another strategy or a tolerance runs qk_asof_join: carry_in (with carry_time, the times of its rows) is the backward carry
+    (rows below r_base), carry_fwd (with carry_fwd_time) the forward one (rows at or past r_base + len(r_time)); carry_out is
+    the newest row of every key for backward, the oldest for forward, and there is none for nearest."""
+    code = _asof_strategy(strategy)
+    plain = strategy == "backward" and tolerance is None
+    ws_bytes = (L.lib().qk_asof_merge_workspace_bytes(l_time.numel(), r_time.numel(), n_by) if plain else
+                L.lib().qk_asof_join_workspace_bytes(l_time.numel(), r_time.numel(), n_by, code))
     if ws_bytes == 0:
         return None, None
     out = torch.empty(l_time.numel(), dtype=torch.int32, device=l_time.device)
     carry_out = torch.empty(n_by, dtype=torch.int32, device=l_time.device) if want_carry else None
     ws = _ws(ws_bytes, l_time.device)
     a, b, c, d = col(l_time), col(l_by), col(r_time), col(r_by)
-    L.check(L.lib().qk_asof_merge(C.byref(a), C.byref(b), C.byref(c), C.byref(d), n_by,
-                                  carry_in.data_ptr() if carry_in is not None else None, int(r_base),
-                                  carry_out.data_ptr() if carry_out is not None else None, out.data_ptr(), ws.data_ptr(), ws.numel(),
-                                  _stream()), "qk_asof_merge")
+    ptr = lambda t: t.data_ptr() if t is not None else None      # noqa: E731
+    if plain:
+        L.check(L.lib().qk_asof_merge(C.byref(a), C.byref(b), C.byref(c), C.byref(d), n_by, ptr(carry_in), int(r_base),
+                                      ptr(carry_out), out.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "qk_asof_merge")
+        return out, carry_out
+    L.check(L.lib().qk_asof_join(C.byref(a), C.byref(b), C.byref(c), C.byref(d), n_by, code, -1 if tolerance is None else int(tolerance),
+                                 ptr(carry_in), ptr(carry_time), ptr(carry_fwd), ptr(carry_fwd_time), int(r_base), ptr(carry_out),
+                                 out.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "qk_asof_join")
     return out, carry_out
 
 

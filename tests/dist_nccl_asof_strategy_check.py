@@ -1,0 +1,19 @@
+"""The as-of strategy cases (tests/asof_strategy_api_cases.py) on real kernels across ranks, launched by
+tests/test_gpu_asof_strategy.py through ranks.torchrun:
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... tests/dist_nccl_asof_strategy_check.py
+It is tests/dist_nccl_check.py with this feature's case list: rank 0 prints `<case>: ok` after each case and the marker
+ranks.NCCL_MARKER at the end."""
+import os
+import sys
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, HERE)
+sys.path.insert(0, os.path.dirname(HERE))
+
+import asof_strategy_api_cases as A
+import dist_nccl_check
+import ranks
+
+if __name__ == "__main__":
+    ranks.SUITES.setdefault("asof_strategy", A.NAMES)
+    dist_nccl_check.main(["asof_strategy"])
