@@ -465,8 +465,8 @@ static int asof_merge_pass(const qk_column* l_time, const qk_column* l_by, const
     k_asof_bounds<FWD><<<(unsigned)((nwin + 1 + 127) / 128), 128, 0, st>>>((const long long*)r_time->data, nr, (const long long*)l_time->data, nl, nwin, wr, wl);
     QK_LAUNCH_CHECK("k_asof_bounds");
     const size_t table_bytes = align_up((size_t)n_by * 4, 16);
-    QK_CUDA(cudaFuncSetAttribute(k_asof_local<FWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)table_bytes));
-    QK_CUDA(cudaFuncSetAttribute(k_asof_sweep<FWD, PICK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    QK_CUDA(qk::raise_smem_limit((const void*)k_asof_local<FWD>, (size_t)table_bytes));
+    QK_CUDA(qk::raise_smem_limit((const void*)k_asof_sweep<FWD, PICK>, (size_t)smem));
     k_asof_local<FWD><<<P, AS_NT, table_bytes, st>>>((const int32_t*)r_by->data, wr, nwin, wpc, n_by, tables);
     QK_LAUNCH_CHECK("k_asof_local");
     k_asof_carry<FWD><<<(n_by + 255) / 256, 256, 0, st>>>(tables, P, n_by, carry_in, r_base, carry_out);

@@ -5,6 +5,9 @@
 #include <stdio.h>
 #include <stdarg.h>
 #include <atomic>
+#include <map>
+#include <mutex>
+#include <utility>
 #include <string>
 #include "../../include/qk.h"
 
@@ -257,6 +260,23 @@ __device__ __forceinline__ T cta_sum(T v, T* wsum) {
     if (threadIdx.x == 0)
         for (int w = 0; w < NT / 32; ++w) t += wsum[w];
     return t;
+}
+
+// The dynamic shared-memory limit of a kernel is one value per kernel and device, shared by every host thread.  A call that
+// set it to its own size could lower it between another thread's setting and that thread's launch, which then fails with
+// "invalid argument".  Here the limit only ever rises, to the most any call has needed, under one lock.
+inline cudaError_t raise_smem_limit(const void* kernel, size_t bytes) {
+    static std::mutex mu;
+    static std::map<std::pair<const void*, int>, size_t> limit;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& cur = limit[{kernel, dev}];
+    if (bytes <= cur) return cudaSuccess;
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) cur = bytes;
+    return e;
 }
 
 }  // namespace qk

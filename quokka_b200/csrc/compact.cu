@@ -395,7 +395,7 @@ int try_filter_compact_tma(const qk_column* cols, int ncols, int64_t nrows, cons
     }
     A.stage_bytes = off;
     const size_t smem = (size_t)C_STAGES * A.stage_bytes;
-    QK_CUDA(cudaFuncSetAttribute(k_filter_compact_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    QK_CUDA(qk::raise_smem_limit((const void*)k_filter_compact_tma, (size_t)smem));
     const int sms = sm_count();
     // contiguous chunks of whole tiles, one per CTA
     const int64_t ntiles = (nrows + tile - 1) / tile;

@@ -296,7 +296,7 @@ template <class C, int MMA>
 int launch_tiles(const TileArgs& a, int ntiles, int nsplit, cudaStream_t st) {
     auto kern = k_gram_tiles<C, MMA>;
     const size_t smem = C::smem(a.nops);
-    QK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    QK_CUDA(qk::raise_smem_limit((const void*)kern, (size_t)smem));
     kern<<<dim3((unsigned)ntiles, (unsigned)nsplit), C::NT, smem, st>>>(a);
     QK_LAUNCH_CHECK("k_gram_tiles");
     return QK_OK;

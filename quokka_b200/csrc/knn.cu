@@ -353,7 +353,7 @@ template <class C>
 int blocks_per_sm(int k) {
     int nb = 0;
     const size_t sm = C::smem(k, 4);
-    cudaFuncSetAttribute(k_knn_scan<float, true, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    qk::raise_smem_limit((const void*)k_knn_scan<float, true, C>, (size_t)sm);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_knn_scan<float, true, C>, KNN_NT, sm) != cudaSuccess || nb < 1) nb = 1;
     return nb;
 }
@@ -372,7 +372,7 @@ int row_ctas_for(int64_t n, int q, int k) {
 template <class T, bool VEC, class C>
 int launch_cfg(const KnnArgs& A, cudaStream_t st) {
     const size_t sm = C::smem(A.k, sizeof(T));
-    QK_CUDA(cudaFuncSetAttribute(k_knn_scan<T, VEC, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    QK_CUDA(qk::raise_smem_limit((const void*)k_knn_scan<T, VEC, C>, (size_t)sm));
     k_knn_scan<T, VEC, C><<<dim3((A.q + C::PT - 1) / C::PT, A.row_ctas), KNN_NT, sm, st>>>(A);
     QK_LAUNCH_CHECK("k_knn_scan");
     return QK_OK;

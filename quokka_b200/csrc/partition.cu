@@ -247,7 +247,7 @@ static int smem_plan(const qk_column* key, int32_t nparts, int32_t mode, int32_t
     const SmemPlanWs w(n, nparts, workspace);
     const unsigned nb = grid_size(nchunks, 8, 1);                      // grid-stride over the chunks
     const size_t smem = (size_t)nparts * 4;
-    QK_CUDA(cudaFuncSetAttribute(k_part_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    QK_CUDA(qk::raise_smem_limit((const void*)k_part_hist, (size_t)smem));
     k_part_hist<<<nb, P_NT, smem, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, w.hist);
     QK_LAUNCH_CHECK("k_part_hist");
     // pass 2: every partition's per-chunk counts (a row of the partition-major histogram) -> offsets relative to the
@@ -255,7 +255,7 @@ static int smem_plan(const qk_column* key, int32_t nparts, int32_t mode, int32_t
     if (int rc = count_offsets(w.hist, nparts, nchunks, w.offsets, w.totals, st)) return rc;
     if (int rc = count_offsets(w.totals, 1, nparts, part_offsets, part_offsets + nparts, st)) return rc;
     const size_t smem_dest = (size_t)nparts * 12;
-    QK_CUDA(cudaFuncSetAttribute(k_part_dest, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_dest));
+    QK_CUDA(qk::raise_smem_limit((const void*)k_part_dest, (size_t)smem_dest));
     k_part_dest<<<nb, P_NT, smem_dest, st>>>(key->data, key->dtype, n, nparts, mode, nchunks, chunk_rows, w.offsets, part_offsets, dest);
     QK_LAUNCH_CHECK("k_part_dest");
     return QK_OK;

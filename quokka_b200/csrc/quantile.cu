@@ -329,7 +329,7 @@ extern "C" int qk_qsketch_update(const qk_column* cols, const uint8_t* const* va
     a.table = table; a.mask = (unsigned long long)capacity - 1; a.half = (unsigned long long)capacity / 2;
     a.ctrl = (unsigned long long*)ctrl; a.deferred = deferred;
     const size_t smem = sizeof(Smem);
-    QK_CUDA(cudaFuncSetAttribute(k_qsketch_update, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    QK_CUDA(qk::raise_smem_limit((const void*)k_qsketch_update, (size_t)smem));
     const int64_t grid = std::min<int64_t>(ntiles, (int64_t)CTAS_PER_SM * sm_count());
     k_qsketch_update<<<(unsigned)grid, NT, smem, st>>>(a);
     QK_LAUNCH_CHECK("k_qsketch_update");

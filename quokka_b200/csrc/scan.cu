@@ -606,7 +606,7 @@ int launch_tma(const FusedArgs& F, const DenseArgs& A, int64_t nrows, double* pa
     const size_t smem = (size_t)F_STAGES * L::stage_bytes + acc_bytes;
     if (smem > 227 * 1024 - 64) return 1;     // does not fit: caller tries the next configuration
     auto kern = k_dense_agg_fused_tma<Plan, V>;
-    QK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    QK_CUDA(qk::raise_smem_limit((const void*)kern, (size_t)smem));
     const int sms = sm_count();
     const int64_t nfull = nrows / (F_NT * V);
     int nb = (int)(nfull < sms ? (nfull > 0 ? nfull : 1) : sms);       // persistent: one CTA per SM
@@ -1153,11 +1153,11 @@ static int launch_dyn_v(DyArgs& D, const DenseArgs& A, int64_t nrows, double* pa
     const int nb = (int)(nfull < want ? (nfull > 0 ? nfull : 1) : want);
     if (fast) {
         auto kern = k_dense_agg_dyn_tma<NT, V, STAGES, true>;
-        QK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        QK_CUDA(qk::raise_smem_limit((const void*)kern, (size_t)smem));
         kern<<<nb, NT, smem, st>>>(D, A, nrows, part_acc, part_cnt);
     } else {
         auto kern = k_dense_agg_dyn_tma<NT, V, STAGES, false>;
-        QK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        QK_CUDA(qk::raise_smem_limit((const void*)kern, (size_t)smem));
         kern<<<nb, NT, smem, st>>>(D, A, nrows, part_acc, part_cnt);
     }
     QK_LAUNCH_CHECK("k_dense_agg_dyn_tma");
@@ -1375,7 +1375,7 @@ extern "C" int qk_scan_filter_agg_dense(const qk_column* cols, int32_t ncols, in
     if (!done) {
         const size_t smem = (size_t)ng * (nagg * 8 + 4) * GEN_NT;
         if (smem > 200 * 1024) QK_FAIL(QK_ERR_UNSUPPORTED, "%s: %lld groups x %d aggregates exceed the shared-memory dense path; use the hash aggregate", who, (long long)ng, nagg);
-        QK_CUDA(cudaFuncSetAttribute(k_dense_agg_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        QK_CUDA(qk::raise_smem_limit((const void*)k_dense_agg_generic, (size_t)smem));
         int per_sm = (int)((220 * 1024) / (smem + 1024));
         if (per_sm < 1) per_sm = 1;
         if (per_sm > 4) per_sm = 4;

@@ -272,7 +272,7 @@ extern "C" int qk_sort_perm(const qk_column* key, const uint8_t* valid, int32_t 
     k_sort_plan<<<1, 256, 0, st>>>(w.S, n, d_lo, d_hi, descending ? 0xff : 0);
     QK_LAUNCH_CHECK("k_sort_plan");
     const int64_t chunk_rows = sort_chunk_rows(n), nchunks = (n + chunk_rows - 1) / chunk_rows;
-    QK_CUDA(cudaFuncSetAttribute(k_sort_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S_SCATTER_SMEM));
+    QK_CUDA(qk::raise_smem_limit((const void*)k_sort_scatter, (size_t)S_SCATTER_SMEM));
     for (int d = d_lo; d < d_hi; ++d) {
         k_sort_count<<<(unsigned)nchunks, S_NT, 0, st>>>(w.S, d, w.img[0], w.img[1], w.row[0], w.row[1], n, chunk_rows, nchunks, w.counts);
         QK_LAUNCH_CHECK("k_sort_count");

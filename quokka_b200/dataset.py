@@ -16,6 +16,7 @@ import pyarrow.parquet as pq
 import torch
 
 from . import _lib as L
+from . import columns
 from . import parquet as PQ
 from .columns import DeviceColumn, DeviceTable, DictionaryRegistry
 
@@ -277,7 +278,7 @@ class InputDeviceDataset(_ReaderBase):
 
     def get_own_state(self, num_channels):
         n = len(self.table)
-        rank = int(os.environ.get("RANK", "0")) if num_channels > 1 else 0
+        rank = columns.rank() if num_channels > 1 else 0
         return {rank: [(a, min(a + self.batch_rows, n)) for a in range(0, n, self.batch_rows)] or [(0, 0)]}
 
     @property
@@ -319,7 +320,7 @@ class InputPinnedDataset(_ReaderBase):
         return self.n
 
     def get_own_state(self, num_channels):
-        rank = int(os.environ.get("RANK", "0")) if num_channels > 1 else 0
+        rank = columns.rank() if num_channels > 1 else 0
         self._chunks = [(a, min(a + self.chunk_rows, self.n)) for a in range(0, self.n, self.chunk_rows)]
         self._next = {}
         return {rank: list(range(len(self._chunks)))}

@@ -239,7 +239,10 @@ class BuildProbeJoinExecutor(Executor):
     """sql_executors.py:325-377.  stream 1 = build (right), stream 0 = probe (left); every build batch
     must arrive before the first probe batch (assert, :357); how in inner/left/semi/anti; the result
     keeps the left key (renamed to the right key when key_to_keep == "right", :372-373); an anti join
-    against an empty build side passes the probe through, the others emit nothing (:362-366)."""
+    against an empty build side passes the probe through, the others emit nothing (:362-366) -- except a left join on a rank
+    that owns no build rows while another rank does: its probe rows keep their place with NULL build columns, whose types
+    come from one build row of another rank (`left_template_row` / `set_left_template`, sent by the runtime once the build
+    side is complete; the reference drops those rows)."""
 
     silent_streams = (1,)        # build batches never produce output: nothing to push downstream after them
     emits_on_done = False        # done() returns nothing: the runtime skips the (empty) exchange after it
@@ -261,6 +264,7 @@ class BuildProbeJoinExecutor(Executor):
         self.things_seen = []
         self._pending = []          # build batches, hashed once at the first probe
         self._build = None
+        self._template = None       # one build row of any rank: the NULL columns of a left join without build rows here
 
     def build_rows(self) -> int:
         return sum(len(b) for b in self._pending) + (len(self.state) if self.state is not None else 0)
@@ -276,6 +280,22 @@ class BuildProbeJoinExecutor(Executor):
         """String keys are compared by value across unrelated dictionaries: their codes cannot feed a filter."""
         cols = [b[self.right_on] for b in self._pending] + ([self.state[self.right_on]] if self.state is not None else [])
         return all(c.dictionary is None and c.data.dtype != torch.float64 for c in cols)
+
+    def left_template_row(self):
+        """One build row of this rank (None: it has none)."""
+        if self.state is not None and len(self.state):
+            return self.state.slice(0, 1)
+        return next((b.slice(0, 1) for b in self._pending if len(b)), None)
+
+    def set_left_template(self, row):
+        self._template = row
+
+    def _unmatched(self, batch: DeviceTable) -> DeviceTable:
+        """A left join's probe rows with NULL build columns (typed like the template row)."""
+        dev = batch[self.left_on].data.device
+        none = torch.full((len(batch),), -1, dtype=torch.int32, device=dev)
+        right = self._template.drop([self.right_on]).gather(none).with_validity(torch.zeros(len(batch), dtype=torch.uint8, device=dev))
+        return _append_right(batch, right.columns, "_right")
 
     def _freeze_build(self):
         if self._build is not None:
@@ -297,11 +317,14 @@ class BuildProbeJoinExecutor(Executor):
             if self.state is None and not self._pending:
                 if self.how == "anti":
                     return batch
-                return
-            if self.phase == "build":
-                self._freeze_build()
-            self.phase = "probe"
-            result = self._build.probe(batch, self.left_on, self.how, "_right")
+                if self.how != "left" or self._template is None:
+                    return
+                result = self._unmatched(batch)
+            else:
+                if self.phase == "build":
+                    self._freeze_build()
+                self.phase = "probe"
+                result = self._build.probe(batch, self.left_on, self.how, "_right")
             if self.key_to_keep == "right":
                 result = result.rename({self.left_on: self.right_on})
             return result

@@ -429,7 +429,8 @@ class Exchange:
 
     def _native_oversize(self, link, plan: _SendPlan, edge_key, need, have) -> list:
         """Somebody's share does not fit its mailbox (every rank sees that in the same meta matrix): the rows go in R
-        rounds, each a complete exchange of a slice of every sender's rows."""
+        rounds, each a complete exchange of a slice of every sender's rows.  Returns what one exchange returns: the tables
+        per source rank in rank order, each source's in round order (consumers fed through the graph depend on it)."""
         R = -(-int(need) // int(have)) * 2
         out = []
         w = len(plan.lo)
@@ -447,7 +448,7 @@ class Exchange:
                 else:
                     sub = {}
                 out += self._native_call(link, sub, None, edge_key)
-            return out
+            return sorted(out, key=lambda t: t.src_rank)          # stable: rounds stay in order within a source
         for r in range(R):
             sub = {}
             if plan.table is not None:
@@ -457,7 +458,7 @@ class Exchange:
                     if b > a:
                         sub[d] = plan.table.slice(a, b)
             out += self._native_call(link, sub, None, edge_key)
-        return out
+        return sorted(out, key=lambda t: t.src_rank)
 
     # ------------------------------------------------------------------ transport 2: torch.distributed collectives
     @staticmethod
@@ -700,9 +701,26 @@ class TaskGraph:
             for ti in sinks:
                 ti.bloom = ops.Bloom(bits, words, w)
 
+    def _publish_left_template(self, actor: _Actor):
+        """`actor` just delivered the last build batch of every join it feeds on stream 1.  A left join's probe rows on a rank
+        that owns no build rows still need the build columns' types: every rank sends one of its build rows (if it has one) to
+        every rank, and each join keeps the first it receives.  Nothing to do where the build side is replicated (every rank
+        holds all of it), at one rank, or for a single-channel join; the decision depends on the plan alone, so all ranks
+        take it alike."""
+        w = world_size()
+        for tgt_id, stream_id, edge in actor.targets:
+            tgt = self.actors[tgt_id]
+            if (w == 1 or stream_id != 1 or tgt.single or isinstance(edge.partitioner, BroadcastPartitioner)
+                    or getattr(tgt.instance, "how", None) != "left" or not hasattr(tgt.instance, "set_left_template")):
+                continue
+            row = tgt.instance.left_template_row()
+            got = self.exchange({r: row for r in range(w)} if row is not None else {}, w, edge_key=("left-template", tgt_id))
+            tgt.instance.set_left_template(got[0] if got else None)
+
     def _finish(self, actor: _Actor):
         actor.done = True
         self._publish_bloom(actor)
+        self._publish_left_template(actor)
         for tgt_id, _, _ in actor.targets:
             tgt = self.actors[tgt_id]
             if tgt.done or not all(self.actors[s].done for s in tgt.sources.values()):

@@ -189,4 +189,3 @@ def case_invalid_args(qc):
 
 API_CASES = [case_strategies, case_rank_boundaries, case_hash_plan, case_many_symbols, case_string_by, case_timestamp_timedelta,
              case_small_batches, case_golden_reference, case_invalid_args]
-NAMES = ["asof_strategy_api_cases:API_CASES"]       # the case list the gloo run names

@@ -10,10 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.dirname(HERE))
 
-import asof_strategy_api_cases as A
 import dist_nccl_check
-import ranks
 
 if __name__ == "__main__":
-    ranks.SUITES.setdefault("asof_strategy", A.NAMES)
     dist_nccl_check.main(["asof_strategy"])

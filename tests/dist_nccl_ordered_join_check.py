@@ -11,9 +11,6 @@ sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.dirname(HERE))
 
 import dist_nccl_check
-import ordered_join_api_cases as A
-import ranks
 
 if __name__ == "__main__":
-    ranks.SUITES.setdefault("ordered_join", A.NAMES)
     dist_nccl_check.main(["ordered_join"])

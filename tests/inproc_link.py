@@ -11,13 +11,21 @@ every launch so that each flag a wait reads is already released:
     the turn they are overwritten with POISON, so that the check at the end of the round sees only what the kernels wrote;
   * payload: every rank's push completes (its stream synchronised) before any rank's recv is launched.
 
-As a backstop every wait's flags are read before it is launched (`HarnessError` if one is missing), and channels get a
-deadline of a few seconds, so a harness bug becomes a QkError, not a long spin.
+As a backstop every wait's flags are read before it is launched (`HarnessError` if one is missing), channels get a
+deadline of a few seconds, and the rank barrier of a channel times out after a minute, so a harness bug becomes an error,
+not a long spin or a stall.
 
-`ops` is quokka_b200.ops (the kernels) or tests/xchg_shim.py (numpy, CPU).  `run_ranks` drives runtime.Exchange: one
-thread and one stream per virtual rank, runtime.native_link / world_size / rank patched to thread-local values."""
+`ops` is quokka_b200.ops (the kernels) or tests/xchg_shim.py (numpy, CPU).  `run_ranks` runs a function on every virtual
+rank: one thread and one stream per rank, with the world, the rank, the link and the lane streams answered per rank
+(`install`).  A rank sees its link as runtime.NativeLink lays it out: channel 0 for the driver thread, channel 1 + i for
+pipeline lane i, each channel an InprocLink of its own.  `run_program_ranks` runs DataStream programs (tests/ranks.py
+run_cases) that way and checks every channel afterwards."""
 from __future__ import annotations
 
+import collections
+import importlib
+import sys
+import tempfile
 import threading
 import types
 
@@ -69,8 +77,10 @@ class InprocLink:
     """W channels over one allocation: W control blocks, then W mailboxes, then a mailbox-sized guard zone that no kernel
     may write (`guard_clean`)."""
 
-    def __init__(self, world: int, mailbox_bytes: int, device, ops, timeout_ms: int = 5000):
+    def __init__(self, world: int, mailbox_bytes: int, device, ops, timeout_ms: int = 5000, barrier_timeout_s: float = 60.0):
         self.world, self.device, self.ops = int(world), torch.device(device), ops
+        self.barrier = threading.Barrier(self.world, timeout=barrier_timeout_s)      # the rank threads of this channel
+        self.rows = [(0, None)] * self.world
         self.mailbox_bytes = (int(mailbox_bytes) + 4095) // 4096 * 4096
         self.head = (self.world * CTRL + 65535) // 65536 * 65536
         self.buf = torch.zeros(self.head + (self.world + 1) * self.mailbox_bytes, dtype=torch.uint8, device=self.device)
@@ -98,6 +108,16 @@ class InprocLink:
     def guard_clean(self) -> bool:
         o = self.head + self.world * self.mailbox_bytes
         return not bool(self.buf[o:o + self.mailbox_bytes].any())
+
+    def check_clean_end(self, what=""):
+        """After a run: the guard zone is untouched, no wait of any rank timed out, and every rank's channel has seen the
+        same number of epochs."""
+        self._sync()
+        assert self.guard_clean(), f"{what}: a kernel wrote past the last mailbox"
+        errs = [int(self.ctrl(r).err[0]) for r in range(self.world)]
+        assert not any(errs), f"{what}: error words {[hex(e) for e in errs]}"
+        epochs = [ch.epoch for ch in self.channels]
+        assert len(set(epochs)) == 1, f"{what}: the ranks end at different epochs {epochs}"
 
     def _write(self, byte_off: int, words: np.ndarray):
         src = torch.from_numpy(np.ascontiguousarray(words).view(np.uint8).copy())
@@ -164,11 +184,11 @@ class InprocLink:
 
 # ------------------------------------------------------------------ runtime.Exchange on the in-process link
 class _Rank:
-    """The `.channels[0]` runtime.Exchange sees on one virtual rank: the real channel, with the calls ordered across the
-    rank threads (meta in turns, every push before any recv)."""
+    """One channel runtime.Exchange sees on one virtual rank: the real channel, with the calls ordered across the rank
+    threads of that channel (meta in turns, every push before any recv)."""
 
-    def __init__(self, link: InprocLink, r: int, barrier: threading.Barrier, rows: list):
-        self.link, self.ch, self.barrier, self.rows = link, link.channels[r], barrier, rows
+    def __init__(self, link: InprocLink, r: int):
+        self.link, self.ch, self.barrier, self.rows = link, link.channels[r], link.barrier, link.rows
         self.world, self.rank, self.mailbox_bytes = link.world, r, link.mailbox_bytes
 
     def meta(self, words, part_offsets=None):
@@ -204,47 +224,228 @@ class _Rank:
         self.link.recv(self.rank, src_byte_off, outs)
 
 
-_tls = threading.local()
+_tls = threading.local()              # .ctx: the virtual rank of the calling thread
+_running = [0]                        # rank runs in progress
+_real = {}                            # the functions `install` replaces, saved before anything is patched
+
+
+def _ctx():
+    ctx = getattr(_tls, "ctx", None)
+    if ctx is None and _running[0]:
+        raise HarnessError(f"thread {threading.current_thread().name!r} belongs to no virtual rank, and ranks are running")
+    return ctx
+
+
+def _world_size():
+    ctx = _ctx()
+    return ctx.world if ctx is not None else 1
+
+
+def _rank():
+    ctx = _ctx()
+    return ctx.rank if ctx is not None else 0
+
+
+def _native_link(device):
+    ctx = _ctx()
+    return ctx.link if ctx is not None else None
+
+
+def _lane_streams(device):
+    """Every virtual rank owns its lane streams, as a real rank (a process) does."""
+    ctx = _ctx()
+    if ctx is None:
+        return _real["lane_streams"](device)
+    if ctx.lane_streams is None:
+        from quokka_b200 import runtime as RT
+        ctx.lane_streams = [torch.cuda.Stream(device) for _ in range(RT.N_LANES)]
+    return ctx.lane_streams
+
+
+class _RankThread(threading.Thread):
+    """A thread that runtime starts from a rank's thread (a pipeline lane) belongs to that rank."""
+
+    def __init__(self, *a, **kw):
+        super().__init__(*a, **kw)
+        self._rank_ctx = getattr(_tls, "ctx", None)
+
+    def run(self):
+        _tls.ctx = self._rank_ctx
+        try:
+            super().run()
+        finally:
+            _tls.ctx = None
+
+
+class _Threading(types.ModuleType):
+    """runtime's `threading`, with Thread replaced by _RankThread."""
+    Thread = _RankThread
+
+    def __getattr__(self, name):
+        return getattr(threading, name)
 
 
 def install(patch):
-    """runtime.world_size / rank / native_link answer for the calling rank thread (1 / 0 / None elsewhere)."""
+    """columns.world_size / columns.rank / runtime.native_link answer for the virtual rank of the calling thread (1 / 0 / None
+    outside a run), wherever a quokka_b200 module bound them by name; runtime's lane threads join the rank that starts them,
+    and runtime.lane_streams gives each rank streams of its own."""
+    from quokka_b200 import columns as C
     from quokka_b200 import runtime as RT
-    patch.setattr(RT, "world_size", lambda: getattr(_tls, "world", 1))
-    patch.setattr(RT, "rank", lambda: getattr(_tls, "rank", 0))
-    patch.setattr(RT, "native_link", lambda device: getattr(_tls, "link", None))
+    if not _real:
+        _real.update(world_size=C.world_size, rank=C.rank, native_link=RT.native_link, lane_streams=RT.lane_streams)
+    fakes = [(_real["world_size"], _world_size), (_real["rank"], _rank), (_real["native_link"], _native_link),
+             (_real["lane_streams"], _lane_streams)]
+    for name, mod in list(sys.modules.items()):
+        if mod is None or not (name == "quokka_b200" or name.startswith("quokka_b200.")):
+            continue
+        for attr, value in list(vars(mod).items()):
+            for real, fake in fakes:
+                if value is real:
+                    patch.setattr(mod, attr, fake)
+    patch.setattr(RT, "threading", _Threading("threading"))
 
 
-def run_ranks(link: InprocLink, fn, timeout_s: float = 600.0):
-    """fn(rank) on every virtual rank, each in its own thread (and CUDA stream), with runtime's view of the world patched
-    by `install`.  Returns the per-rank results; re-raises the first failure."""
-    W = link.world
-    barrier = threading.Barrier(W, timeout=timeout_s)
-    rows = [(0, None)] * W
+def make_links(world: int, mailbox_bytes: int, device, ops) -> list:
+    """The channels of runtime.NativeLink: 1 + runtime.N_LANES in-process links of `mailbox_bytes` each."""
+    from quokka_b200 import runtime as RT
+    return [InprocLink(world, mailbox_bytes, device, ops) for _ in range(1 + RT.N_LANES)]
+
+
+def run_ranks(links, fn):
+    """fn(rank) on every virtual rank, each in its own thread (and CUDA stream), with runtime's view of the world answered
+    per rank by `install`.  `links`: one InprocLink, or the channels of make_links.  Returns the per-rank results;
+    re-raises the first failure (after aborting every channel's barrier, so no rank waits for a failed one)."""
+    links = [links] if isinstance(links, InprocLink) else list(links)
+    W, device = links[0].world, links[0].device
     results, errors = [None] * W, [None] * W
 
     def body(r):
-        _tls.world, _tls.rank = W, r
-        _tls.link = types.SimpleNamespace(channels=[_Rank(link, r, barrier, rows)], mailbox_bytes=link.mailbox_bytes)
+        _tls.ctx = types.SimpleNamespace(world=W, rank=r, lane_streams=None, link=types.SimpleNamespace(
+            channels=[_Rank(link, r) for link in links], mailbox_bytes=links[0].mailbox_bytes))
         try:
-            if link.device.type == "cuda":
-                with torch.cuda.stream(torch.cuda.Stream(link.device)):
+            if device.type == "cuda":
+                with torch.cuda.stream(torch.cuda.Stream(device)):
                     results[r] = fn(r)
-                    link._sync()
+                    links[0]._sync()
             else:
                 results[r] = fn(r)
         except BaseException as e:      # noqa: B902 -- reported below; the other ranks must not wait for this one
             errors[r] = e
-            barrier.abort()
+            for link in links:
+                link.barrier.abort()
         finally:
-            del _tls.world, _tls.rank, _tls.link
+            _tls.ctx = None
 
     threads = [threading.Thread(target=body, args=(r,), name=f"inproc-rank{r}") for r in range(W)]
-    for t in threads:
-        t.start()
-    for t in threads:
-        t.join()
+    _running[0] += 1
+    try:
+        for t in threads:
+            t.start()
+        for t in threads:
+            t.join()
+    finally:
+        _running[0] -= 1
     real = [e for e in errors if e is not None and not isinstance(e, threading.BrokenBarrierError)]
     if real or any(e is not None for e in errors):
         raise (real or [e for e in errors if e is not None])[0]
     return results
+
+
+# ------------------------------------------------------------------ DataStream programs on in-process ranks
+def _count_calls(patch, ops, counts, lock):
+    """Counts, in `counts`, the calls that only multi-rank execution makes: an ordered join's placement of the owners'
+    matches, an as-of merge over the ranks' time ranges with the carried rows of earlier / later ranks (the streaming path
+    passes a carry of its own on one rank too, so only SortedAsofExecutor._join_carried's calls count), a shift with
+    boundary rows, the merge of top-k lists and of quantile sketch entries, an exchange that goes in rounds, a left join's
+    NULL columns on a rank without build rows; and the most lanes a TaskGraph ran on."""
+    from quokka_b200 import executors as X
+    from quokka_b200 import runtime as RT
+    carried = threading.local()         # .on: inside _join_carried on this thread
+
+    def bump(key, n=1):
+        with lock:
+            counts[key] += n
+
+    def wrap(owner, name, key_of, static=False):
+        real = getattr(owner, name)
+
+        def counted(*a, **kw):
+            for key in key_of(*a, **kw):
+                bump(key)
+            return real(*a, **kw)
+        patch.setattr(owner, name, staticmethod(counted) if static else counted)
+
+    def asof_keys(*a, **kw):
+        if not getattr(carried, "on", False):
+            return []
+        back = a[5] if len(a) > 5 else kw.get("carry_in")
+        return (["asof_carry"] if back is not None else []) + (["asof_carry_fwd"] if kw.get("carry_fwd") is not None else [])
+
+    wrap(ops.JoinTable, "place", lambda *a, **kw: ["join_place"], static=True)
+    wrap(ops, "asof_merge", asof_keys)
+    wrap(ops, "shift_gather", lambda a, b, *r, **kw: ["shift_boundary"] if b is not None else [])
+    wrap(ops, "knn_merge", lambda *a, **kw: ["knn_merge"])
+    wrap(ops.QuantileSketch, "merge", lambda *a, **kw: ["qsketch_merge"])
+    wrap(RT.Exchange, "_native_oversize", lambda *a, **kw: ["exchange_rounds"])
+    wrap(X.BuildProbeJoinExecutor, "_unmatched", lambda *a, **kw: ["left_template"])
+    real_carried = X.SortedAsofExecutor._join_carried
+
+    def join_carried(self, *a, **kw):
+        carried.on = True
+        try:
+            return real_carried(self, *a, **kw)
+        finally:
+            carried.on = False
+    patch.setattr(X.SortedAsofExecutor, "_join_carried", join_carried)
+    real_run = RT.TaskGraph.run
+
+    def run(self):
+        out = real_run(self)
+        with lock:
+            counts["lanes_used"] = max(counts["lanes_used"], self.lanes_used)
+        return out
+    patch.setattr(RT.TaskGraph, "run", run)
+
+
+def run_program_ranks(world: int, names, device, mailbox_bytes: int) -> collections.Counter:
+    """tests/ranks.py run_cases(names) on `world` virtual ranks in threads of this process: on the kernels (quokka_b200.ops)
+    over the in-process link when `device` is CUDA, on tests/cpu_shim.py with the channels of tests/xchg_shim.py on CPU.
+    Every case checks what each rank gathers.  Afterwards every channel must end clean (InprocLink.check_clean_end).
+    Returns the counters of _count_calls, summed over the ranks."""
+    import pytest
+    import ranks
+    device = torch.device(device)
+    counts, lock = collections.Counter(), threading.Lock()
+    for name in ranks.expand(names):          # case modules install their CPU stand-ins on import: before anything is wrapped
+        head, _, rest = name.partition(":")
+        importlib.import_module(head if rest and head not in ranks._API_PREFIXES else "api_cases")
+    with pytest.MonkeyPatch.context() as mp, tempfile.TemporaryDirectory() as files:
+        if device.type == "cuda":
+            from quokka_b200 import ops
+        else:
+            import asof_strategy_shim
+            import cpu_shim as ops
+            import ordered_join_shim
+            ops.install(mp)
+            ordered_join_shim.install()           # the stand-ins of the feature kernels (idempotent; the case modules do it too)
+            asof_strategy_shim.install()
+        _count_calls(mp, ops, counts, lock)
+        install(mp)
+        links = make_links(world, mailbox_bytes, device, ops)
+        run_ranks(links, lambda r: ranks.run_cases(names, r, world, files))
+        for i, link in enumerate(links):
+            link.check_clean_end(f"channel {i}")
+    return counts
+
+
+# the counters of _count_calls that a suite of tests/ranks.py SUITES must reach at world > 1, on any mailbox
+REACHES = {
+    "api": ["asof_carry"],
+    "sort": ["asof_carry"],
+    "shift": ["shift_boundary"],
+    "knn": ["knn_merge"],
+    "ordered_join": ["join_place"],
+    "asof_strategy": ["asof_carry", "asof_carry_fwd"],
+    "quantile": ["qsketch_merge"],
+}
+IN_ROUNDS_AT_1MB = ("ordered_join", "asof_strategy")         # suites whose larger exchanges go in rounds with 1 MB mailboxes

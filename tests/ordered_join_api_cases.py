@@ -222,6 +222,5 @@ def case_join_then_ordered_ops(qc):
             _frames_equal(got, exp, name)
 
 
-NAMES = ["ordered_join_api_cases:API_CASES"]       # the case list the gloo and NCCL runs name
 API_CASES = [case_inner_and_left, case_semi_and_anti, case_keep_right_order, case_many_build_rows, case_string_and_fp64_keys,
              case_empty_sides, case_filter_after_join, case_join_then_ordered_ops]

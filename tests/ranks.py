@@ -18,7 +18,8 @@ import torch.multiprocessing as mp
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = os.path.join(HERE, "golden")
 
-# the case lists that the gloo test of a feature and dist_nccl_check.py's arguments share
+# the case lists that the gloo test of a feature, dist_nccl_check.py's arguments and the in-process runs
+# (tests/inproc_link.py run_program_ranks) share
 SUITES = {
     "api": ["case_q1_sql", "case_q1_dict_api", "case_q3", "case_q5", "case_join_kinds", "case_asof", "case_executor_protocol",
             "case_misc_ops", "case_scalar_aggs", "case_string_key_join", "case_agg_types", "case_windows", "case_asof_reference_result"],
@@ -34,6 +35,11 @@ SUITES = {
                                                "case_shift_out_of_order")],
     "knn": ["knn_cases:" + c for c in ("case_vector_roundtrip", "case_vector_ops", "case_knn_api", "case_knn_fewer_rows")],
     "pattern": ["pattern_cases:API_CASES"],
+    "ordered_join": ["ordered_join_api_cases:API_CASES"],
+    "asof_strategy": ["asof_strategy_api_cases:API_CASES"],
+    "gram": ["test_dist_gloo_gram:case_gram_shares", "test_dist_gloo_gram:case_gram_device_batches", "gram_cases:case_gram_filtered_ints",
+             "gram_cases:case_gram_empty"],
+    "quantile": ["test_dist_gloo_quantile:case_quantile_shares", "quantile_cases:case_quantile_tpch_606", "quantile_cases:case_quantile_empty"],
 }
 NCCL_MARKER = "DIST_NCCL_OK"
 _API_PREFIXES = ("hash", "cb", "cbmix", "random_programs", "random_asof", "asof_rank_shards")

@@ -2,9 +2,8 @@
 tests/asof_strategy_shim.py): the time-range plan with equal quote times straddling the boundary, a gap, ranks without quotes
 or trades and a symbol quoted only on the later rank; the hash-partitioned plan; the search path; every rank collects the
 global join."""
-import asof_strategy_api_cases as A
 import ranks
 
 
 def test_asof_strategy_two_ranks_gloo(tmp_path):
-    ranks.spawn(tmp_path, 2, ranks.gloo_rank, A.NAMES)
+    ranks.spawn(tmp_path, 2, ranks.gloo_rank, ranks.SUITES["asof_strategy"])

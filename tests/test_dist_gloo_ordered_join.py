@@ -2,9 +2,8 @@
 replicated and hash-partitioned: the ordered side stays on its rank, and the gathered result is the ordered join of the
 collected inputs row for row -- string keys whose dictionaries differ by rank, fp64 keys, a rank without left or build rows,
 and the ordered operators downstream without a re-sort."""
-import ordered_join_api_cases as A
 import ranks
 
 
 def test_ordered_join_two_ranks_gloo(tmp_path):
-    ranks.spawn(tmp_path, 2, ranks.gloo_rank, A.NAMES)
+    ranks.spawn(tmp_path, 2, ranks.gloo_rank, ranks.SUITES["ordered_join"])

@@ -15,5 +15,4 @@ def case_quantile_shares(qc):
 
 
 def test_quantile_two_ranks_gloo(tmp_path):
-    ranks.spawn(tmp_path, 2, ranks.gloo_rank, ["test_dist_gloo_quantile:case_quantile_shares",
-                                               "quantile_cases:case_quantile_tpch_606", "quantile_cases:case_quantile_empty"])
+    ranks.spawn(tmp_path, 2, ranks.gloo_rank, ranks.SUITES["quantile"])

@@ -129,5 +129,33 @@ def test_asof_strategy_two_ranks_nccl():
         pytest.skip("needs >= 2 GPUs")
     rc, out = ranks.torchrun("dist_nccl_asof_strategy_check.py", 2)
     assert rc == 0 and ranks.NCCL_MARKER in out, out[-4000:]
-    missing = [n for n in ranks.expand(A.NAMES) if not re.search(f"^{re.escape(n)}: ok", out, re.M)]
+    missing = [n for n in ranks.expand(ranks.SUITES["asof_strategy"]) if not re.search(f"^{re.escape(n)}: ok", out, re.M)]
     assert not missing, f"no ok line for {missing}\n{out[-4000:]}"
+
+
+def test_merge_join_from_two_threads_with_different_key_counts():
+    """Two host threads (two ranks of one process, or two pipeline lanes) run the merge join at once, one with 40 000 keys and
+    one with 3: the dynamic shared-memory limit of a kernel is one value for all threads, so one thread's call must never
+    lower it below what the other thread's launch needs (csrc/common.cuh raise_smem_limit)."""
+    import threading
+    from quokka_b200 import ops
+    cases = [_inputs(5_000, 20_000, n_by, n_by) + (n_by,) for n_by in (40_000, 3)]
+    errors = []
+
+    def body(lt, lb, rt, rb, n_by):
+        try:
+            args = _cuda(lt, lb, rt, rb)
+            exp = S.merge_join(lt, lb, rt, rb, n_by, "backward", None, None, None, None, None, 0)
+            with torch.cuda.stream(torch.cuda.Stream()):
+                for _ in range(25):
+                    got, _ = ops.asof_merge(*args, n_by)
+                    assert np.array_equal(got.cpu().numpy(), exp), n_by
+        except BaseException as e:          # noqa: B902 -- reported on the test's thread
+            errors.append(e)
+
+    threads = [threading.Thread(target=body, args=c) for c in cases]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    assert not errors, errors[0]

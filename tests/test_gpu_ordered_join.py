@@ -126,5 +126,5 @@ def test_ordered_join_two_ranks_nccl():
         pytest.skip("needs >= 2 GPUs")
     rc, out = ranks.torchrun("dist_nccl_ordered_join_check.py", 2)
     assert rc == 0 and ranks.NCCL_MARKER in out, out[-4000:]
-    missing = [n for n in ranks.expand(A.NAMES) if not re.search(f"^{re.escape(n)}: ok", out, re.M)]
+    missing = [n for n in ranks.expand(ranks.SUITES["ordered_join"]) if not re.search(f"^{re.escape(n)}: ok", out, re.M)]
     assert not missing, f"no ok line for {missing}\n{out[-4000:]}"

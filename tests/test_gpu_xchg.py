@@ -434,3 +434,27 @@ def test_hash_edge_placement_rule(n):
     codes = rng.integers(0, len(words), 8_000).astype(np.int32)
     part = _edge_placement(DeviceColumn(_dev(codes), words, None), n)
     assert np.array_equal(part, np.array([zlib.crc32(words[c].encode()) % n for c in codes]))
+
+
+def test_partition_plan_from_two_threads_with_different_part_counts():
+    """Two host threads plan partitions at once, into 16 384 parts and into 3: k_part_hist's shared memory grows with the
+    part count, and one thread's call must never lower the kernel's limit below what the other's launch needs."""
+    import threading
+    rng = np.random.default_rng(11)
+    keys = rng.integers(I64.min, I64.max, 300_000, dtype=np.int64, endpoint=True)
+    errors = []
+
+    def body(nparts):
+        try:
+            with torch.cuda.stream(torch.cuda.Stream()):
+                for _ in range(25):
+                    assert np.array_equal(_placement(_dev(keys), nparts), np.mod(keys, nparts)), nparts
+        except BaseException as e:          # noqa: B902 -- reported on the test's thread
+            errors.append(e)
+
+    threads = [threading.Thread(target=body, args=(n,)) for n in (16_384, 3)]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    assert not errors, errors[0]

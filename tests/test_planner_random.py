@@ -374,9 +374,9 @@ def run_asof_rank_shards(qc, seed, trials=14):
     """The multi-rank as-of join over TIME RANGES (SortedAsofExecutor._join_time_ranges): every rank passes its own contiguous
     slice of the two sorted streams, cut independently -- so trades sit on the "wrong" side of a quote boundary, ranks have no
     quotes, no trades, or nothing at all, and equal timestamps straddle the cuts -- and every rank must collect the global join."""
-    import torch.distributed as dist
+    from quokka_b200 import runtime
     from quokka_b200.columns import DeviceTable
-    w, me = dist.get_world_size(), dist.get_rank()
+    w, me = runtime.world_size(), runtime.rank()
     rng = np.random.default_rng(seed)                      # the same draws on every rank
     for trial in range(trials):
         nt, nq, nsym = int(rng.integers(0, 300)), int(rng.integers(1, 600)), int(rng.integers(1, 5))

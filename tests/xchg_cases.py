@@ -2,7 +2,8 @@
 peer-memory link or NCCL), on gloo ranks (tests/test_dist_gloo_exchange.py) and on the in-process link (tests/inproc_link.py:
 tests/test_gpu_xchg.py on one GPU, tests/test_xchg_cpu.py over the numpy shim).  Every rank draws the SAME global table
 from a seed, keeps its shard, runs the exchange and checks what it received against numpy: rows with key % world == rank,
-per source rank in source order (the partition is stable), bit-exact; and the bytes it sent to other ranks (validity masks
+per source rank in source order (the partition is stable), bit-exact, in a list whose source ranks never decrease (also when
+the payload went in rounds); and the bytes it sent to other ranks (validity masks
 included) and every rank's received-row total on the edge, exactly.  Covers hash-partitioned edges at several sizes,
 ranks with nothing to send, validity masks, edges of 20 columns and of 12 masked columns (24 buffers), broadcast with a
 validity mask and per-rank dictionaries, vector columns, a hash edge whose dictionaries differ per rank and grow, single
@@ -31,6 +32,13 @@ def _shard(n, r):
 def _width(v: np.ndarray) -> int:
     """Bytes of one row of a column."""
     return v.dtype.itemsize * (v.shape[1] if v.ndim == 2 else 1)
+
+
+def _check_source_order(got, what):
+    """The received tables come per source rank in rank order, a source's rounds one after the other: consumers fed through
+    the task graph see them in list order."""
+    srcs = [g.src_rank for g in got]
+    assert srcs == sorted(srcs), (what, runtime.rank(), srcs)
 
 
 def _check_accounting(ex, edge_key, sent_before, sent, recv_rows):
@@ -66,6 +74,7 @@ def check_hash(ex, dev, n, seed, empty_ranks=(), tag="", masked=False, skew=Fals
     parts = apply_partitioner(HashPartitioner("k"), t, me, w) if hi > lo else {}
     sent0 = ex.bytes_sent
     got = ex(parts, w, edge_key=("hash", tag))
+    _check_source_order(got, tag)
     nonempty = [np.arange(*_shard(n, s)) for s in range(w) if s not in empty_ranks]
     dest_all = np.concatenate(nonempty) if nonempty else np.zeros(0, np.int64)
     recv_rows = np.bincount(cols["k"][dest_all] % w, minlength=w)
@@ -105,6 +114,7 @@ def check_broadcast_and_single_owner(ex, dev):
     t = _table_of(dev, cols, lo, hi, {"s": mydict}, valid)
     sent0, row_bytes = ex.bytes_sent, 8 + 4 + 1
     got = ex({r: t for r in range(w)}, w, edge_key=("bcast",))
+    _check_source_order(got, "bcast")
     _check_accounting(ex, ("bcast",), sent0, (hi - lo) * (w - 1) * row_bytes, [n] * w)
     assert sorted(set(g.src_rank for g in got)) == list(range(w))
     for s in range(w):
@@ -116,6 +126,7 @@ def check_broadcast_and_single_owner(ex, dev):
         assert [g["s"].dictionary[c] for g in mine_ for c in g["s"].data.cpu().numpy()] == [sdict[c] for c in cols["s"][a:b]], "values survive the re-coding"
     sent0 = ex.bytes_sent
     got = ex({0: t}, 1, single_owner=0, edge_key=("single",))
+    _check_source_order(got, "single")
     _check_accounting(ex, ("single",), sent0, 0 if me == 0 else (hi - lo) * row_bytes, [n] + [0] * (w - 1))
     assert (sorted(set(g.src_rank for g in got)) == list(range(w))) if me == 0 else (got == [])
     if me == 0:
@@ -152,6 +163,7 @@ def check_wide(ex, dev, kind, ncols, masked=False, n=30_011, seed=30):
         got = ex({r: t for r in range(w)}, w, edge_key=key)
         mine_ = [np.arange(*_shard(n, s)) for s in range(w)]
         _check_accounting(ex, key, sent0, (hi - lo) * (w - 1) * row_bytes, [n] * w)
+    _check_source_order(got, key)
     mine_ = [(s, sel) for s, sel in enumerate(mine_) if len(sel)]
     assert sorted(set(g.src_rank for g in got)) == [s for s, _ in mine_], (key, me)
     for s, sel in mine_:
@@ -172,6 +184,7 @@ def check_vectors(ex, dev, n=4_099, seed=40):
     t = _table_of(dev, cols, lo, hi)
     sent0 = ex.bytes_sent
     got = ex({r: t for r in range(w)}, w, edge_key=("vectors",))
+    _check_source_order(got, "vectors")
     _check_accounting(ex, ("vectors",), sent0, (hi - lo) * (w - 1) * (8 + 28 + 10), [n] * w)
     srcs = [s for s in range(w) if _shard(n, s)[1] > _shard(n, s)[0]]
     assert sorted(set(g.src_rank for g in got)) == srcs
@@ -210,6 +223,7 @@ def check_dictionaries(ex, dev, n=20_003, seed=50):
         t = _table_of(dev, {"k": k, "s": codes}, lo, hi, {"s": dict_of(me, grown)})
         parts = apply_partitioner(HashPartitioner("k"), t, me, w) if hi > lo else {}
         got = ex(parts, w, edge_key=("dicts",))
+        _check_source_order(got, ("dicts", call))
         for s in range(w):
             if s in empty:
                 continue
