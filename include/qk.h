@@ -408,6 +408,20 @@ QK_API size_t qk_window_session_workspace_bytes(int64_t nrows);
 QK_API int qk_window_session_ids(const qk_column* time, const qk_column* by, int64_t timeout, int64_t* ids, void* workspace,
                                  size_t ws_bytes, void* stream);
 
+/* Per-event (OnEventTrigger) tumbling and session windows: the DuckDB window query of HoppingWindowExecutor /
+ * SessionWindowExecutor (ts_executors.py:64-96, 109-136, 239-288), PARTITION BY key, window ORDER BY time
+ * RANGE UNBOUNDED PRECEDING.  The rows of a key are cut into runs: QK_WIN_RUN_TUMBLING, param = size > 0: the rows with one
+ * floor(time / size); QK_WIN_RUN_SESSION, param = timeout >= 0: a new run after every gap > timeout.  out[o][i] = aggregate
+ * ops[o] of vals[srcs[o]] over the rows of row i's run with time <= time[i] (rows with equal times all get the value that
+ * includes them), all fp64 (COUNT too), in the same arguments as qk_window_sliding.  Deterministic: the same bits on every
+ * call.  Workspace: qk_window_running_workspace_bytes(rows). */
+#define QK_WIN_RUN_TUMBLING 1
+#define QK_WIN_RUN_SESSION 2
+QK_API size_t qk_window_running_workspace_bytes(int64_t nrows);
+QK_API int qk_window_running(const qk_column* time, const qk_column* by, const int64_t* seg, int32_t n_by, int32_t kind, int64_t param,
+                             const qk_column* vals, int32_t nvals, const int32_t* ops, const int32_t* srcs, int32_t nout,
+                             qk_column* out, void* workspace, size_t ws_bytes, void* stream);
+
 /* ---- K8: top-k candidates -------------------------------------------------------------------
  * Replaces the `order by ... limit k` of DataStream.top_k / ConcatThenSQLExecutor
  * (pyquokka/datastream.py:1746-1767, sql_executors.py:45-67) for the primary sort column: radix

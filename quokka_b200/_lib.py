@@ -16,6 +16,7 @@ PATTERN_MAX_EVENTS, PATTERN_STATUS_WORDS, PATTERN_MAX_LINK_NODES = 8, 4, 128   #
 CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_EQ, CMP_NE = range(6)
 AGG_SUM, AGG_MIN, AGG_MAX = 1, 2, 3
 WIN_SUM, WIN_MIN, WIN_MAX, WIN_COUNT, WIN_AVG = 1, 2, 3, 4, 5
+WIN_RUN_TUMBLING, WIN_RUN_SESSION = 1, 2
 PART_MOD, PART_CODE = 0, 1
 JOIN_INNER, JOIN_LEFT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3
 ASOF_BACKWARD, ASOF_FORWARD, ASOF_NEAREST = 0, 1, 2
@@ -141,6 +142,9 @@ _SIGNATURES = {
                                        C.c_void_p, C.c_void_p, C.c_void_p]),
     "qk_window_session_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "qk_window_session_ids": (C.c_int, [_P(qk_column), _P(qk_column), C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "qk_window_running_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "qk_window_running": (C.c_int, [_P(qk_column), _P(qk_column), C.c_void_p, C.c_int32, C.c_int32, C.c_int64, _P(qk_column), C.c_int32,
+                                    _P(C.c_int32), _P(C.c_int32), C.c_int32, _P(qk_column), C.c_void_p, C.c_size_t, C.c_void_p]),
     "qk_topk_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "qk_topk_candidates": (C.c_int, [_P(qk_column), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_size_t, C.c_void_p]),

@@ -1115,7 +1115,12 @@ class OrderedStream(DataStream):
 
     def windowed_transform(self, window, trigger):
         """pyquokka/datastream.py:1650-1700: hopping / tumbling / sliding / session windows per `window.partition_by` key over
-        a stream sorted by `window.order_by`.  New schema: [time, key] + the window's aggregate columns."""
+        a stream sorted by `window.order_by`.  New schema: [time, key] + the window's aggregate columns ([key, time] + ... for
+        session windows).  The trigger decides what comes out of tumbling and session windows, as in the reference:
+        OnCompletionTrigger gives one row per window (time = its start); OnEventTrigger gives one row per input row, with its
+        own time, carrying the aggregates of its window over the window's rows with time <= its own (rows with equal times all
+        get the value that includes them), in key, then time order.  A HoppingWindow with OnEventTrigger raises; sliding
+        windows give one row per input row whatever the trigger."""
         from .executors import HoppingWindowExecutor, SessionWindowExecutor, SlidingWindowExecutor
         from .windowtypes import HoppingWindow, SessionWindow, SlidingWindow
         time_col, by_col = window.order_by, window.partition_by

@@ -1731,19 +1731,43 @@ class _HashedWindow(_WindowExecutor):
         return ok, out
 
 
+    def _per_event(self, kind: int, length, key_first: bool):
+        """OnEventTrigger (ts_executors.py:64-96, 109-136, 239-288: DuckDB's PARTITION BY key, window ORDER BY time RANGE
+        UNBOUNDED PRECEDING): one row per input row, in key-segmented order, with its own time and the aggregates of its
+        window's rows with time <= its own (qk_window_running).  `length` is the tumbling size or the session timeout; a
+        timedelta is converted with Window.ticks in the time column's unit (the reference divides the int64 timestamp by
+        total_seconds())."""
+        seg_in = self._segmented()
+        if seg_in is None:
+            return None
+        time, codes, seg, n_by, vals, spec, (bycol, tcol, unit) = seg_in
+        outs = ops.window_sliding(time, codes, seg, n_by, self.window.ticks(length, unit), vals,
+                                  [(_WIN[op], max(src, 0)) for _, op, src in spec], run=kind)
+        key, tc = self._codes.column(codes, bycol), self._time_column(time, tcol)
+        cols = {self.by_col: key, self.time_col: tc} if key_first else {self.time_col: tc, self.by_col: key}
+        for (name, op, _), o in zip(spec, outs):
+            cols[name] = _int_result(op, o)
+        return DeviceTable(cols)
+
+
 class HoppingWindowExecutor(_HashedWindow):
     """ts_executors.py:12-145: aggregates per key over the windows [k * hop, k * hop + size) (Polars groupby_dynamic(every=hop,
     period=size, by=key): closed on the left, labelled by the window start, windows before the key's first truncated
-    timestamp are not produced, empty windows neither).  TumblingWindow = hop == size.  Output: time (window start), key, aggregates."""
+    timestamp are not produced, empty windows neither).  TumblingWindow = hop == size.  Output: time (window start), key, aggregates.
+    A TumblingWindow with OnEventTrigger gives one row per input row instead (_per_event): time, key and the aggregates of the
+    row's window [k * size, (k + 1) * size) up to its time; computed in done(), like every window here, not as the rows stream."""
 
     def __init__(self, time_col, by_col, window, trigger) -> None:
-        from .windowtypes import HoppingWindow, OnEventTrigger
+        from .windowtypes import HoppingWindow, OnEventTrigger, TumblingWindow
         assert issubclass(type(window), HoppingWindow)
         super().__init__(time_col, by_col, window, trigger)
-        if type(trigger) == OnEventTrigger and type(window) == HoppingWindow:
+        if type(trigger) == OnEventTrigger and not isinstance(window, TumblingWindow):
             raise Exception("OnEventTrigger is not supported for hopping windows")
 
     def done(self, executor_id):
+        from .windowtypes import OnEventTrigger
+        if type(self.trigger) == OnEventTrigger:
+            return self._per_event(L.WIN_RUN_TUMBLING, self.window.size, key_first=False)
         seg_in = self._segmented()
         if seg_in is None:
             return None
@@ -1763,7 +1787,10 @@ class HoppingWindowExecutor(_HashedWindow):
 
 class SessionWindowExecutor(_HashedWindow):
     """ts_executors.py:197-288: per key, a session = a run of rows whose gaps are all <= timeout; aggregates per session.
-    Output: key, time (the session's first timestamp; the reference emits its internal window id instead), aggregates."""
+    Output: key, time (the session's first timestamp; the reference emits its internal window id instead), aggregates.
+    With OnEventTrigger one row per input row instead (_per_event): key, time and the aggregates of the row's session up to
+    its time.  The time column is `order_by` (the reference's per-event path reads a column named "ts", ts_executors.py:228),
+    and the result is computed in done(), not as the rows stream."""
 
     def __init__(self, time_col, by_col, window, trigger) -> None:
         from .windowtypes import SessionWindow
@@ -1771,6 +1798,9 @@ class SessionWindowExecutor(_HashedWindow):
         super().__init__(time_col, by_col, window, trigger)
 
     def done(self, executor_id):
+        from .windowtypes import OnEventTrigger
+        if type(self.trigger) == OnEventTrigger:
+            return self._per_event(L.WIN_RUN_SESSION, self.window.timeout, key_first=True)
         seg_in = self._segmented()
         if seg_in is None:
             return None

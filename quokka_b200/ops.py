@@ -520,15 +520,24 @@ def asof_merge(l_time: torch.Tensor, l_by: torch.Tensor, r_time: torch.Tensor, r
 
 # ------------------------------------------------------------------ time-series windows
 def window_sliding(time: torch.Tensor, by: torch.Tensor, seg: torch.Tensor, n_by: int, size: int, vals: Sequence[torch.Tensor],
-                   aggs: Sequence[tuple]):
-    """aggs = [(QK_WIN_*, index into vals)]; inputs in key-segmented order.  Returns one fp64 column per aggregate."""
+                   aggs: Sequence[tuple], *, run: int | None = None):
+    """aggs = [(QK_WIN_*, index into vals)]; inputs in key-segmented order.  Returns one fp64 column per aggregate.
+    run=None: every row aggregates its key's rows with time in (t - size, t] (qk_window_sliding).  run=WIN_RUN_TUMBLING /
+    WIN_RUN_SESSION: per-event windows (qk_window_running), `size` being the tumbling size / the session timeout; every row
+    aggregates the rows of its run (its tumbling window or session) with time <= its own."""
     n = time.numel()
     outs = [torch.empty(n, dtype=torch.float64, device=time.device) for _ in aggs]
     t, b = col(time), col(by)
     opv = (C.c_int32 * max(1, len(aggs)))(*[int(a[0]) for a in aggs])
     srcv = (C.c_int32 * max(1, len(aggs)))(*[int(a[1]) for a in aggs])
-    L.check(L.lib().qk_window_sliding(C.byref(t), C.byref(b), seg.data_ptr(), int(n_by), int(size), cols(vals) if vals else None, len(vals),
-                                      opv, srcv, len(aggs), cols(outs, "output"), _stream()), "qk_window_sliding")
+    vc = cols(vals) if vals else None
+    if run is None:
+        L.check(L.lib().qk_window_sliding(C.byref(t), C.byref(b), seg.data_ptr(), int(n_by), int(size), vc, len(vals), opv, srcv, len(aggs),
+                                          cols(outs, "output"), _stream()), "qk_window_sliding")
+    else:
+        ws = _ws(L.lib().qk_window_running_workspace_bytes(n), time.device)
+        L.check(L.lib().qk_window_running(C.byref(t), C.byref(b), seg.data_ptr(), int(n_by), int(run), int(size), vc, len(vals), opv, srcv,
+                                          len(aggs), cols(outs, "output"), ws.data_ptr(), ws.numel(), _stream()), "qk_window_running")
     return outs
 
 
