@@ -205,11 +205,6 @@ class DenseAggState:
                                                  self.cnt.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
                                                  int(variant), _stream()), "qk_scan_filter_agg_dense")
 
-    def merge_(self, other_acc: torch.Tensor, other_cnt: torch.Tensor):
-        """Fold another partial state (e.g. from a peer rank) into this one (SUM only)."""
-        self.acc += other_acc
-        self.cnt += other_cnt
-
 
 def last_variant() -> str:
     return L.lib().qk_last_variant().decode()

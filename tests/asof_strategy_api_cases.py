@@ -11,8 +11,6 @@ import pyarrow as pa
 
 import asof_strategy_shim as S
 
-S.install()         # the CPU runs (1 rank, gloo ranks) read the strategies from the numpy stand-in
-
 CASES_TOL = (None, 0, 3)
 
 

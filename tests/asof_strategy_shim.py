@@ -1,13 +1,12 @@
 """TEST-ONLY numpy statements of the as-of strategies (csrc/asof.cu qk_asof_join, qk_asof_search_join).  `asof_join` is the
 plain restatement of pandas.merge_asof(direction=strategy, tolerance=tolerance) that the other tests compare against;
-`merge_join` states what the merge kernel returns with its carry tables.  install() puts stand-ins of ops.asof_merge and
-ops.asof_backward that take `strategy=` / `tolerance=` into tests/cpu_shim.py, so OrderedStream.join_asof(strategy=...) runs
+`merge_join` states what the merge kernel returns with its carry tables.  The asof_merge and asof_backward of
+tests/cpu_shim.py answer with them when given a `strategy=` / `tolerance=`, so OrderedStream.join_asof(strategy=...) runs
 through the planner, the executors and the gloo exchange without a GPU.  The GPU tests compare both kernels with these, bit
 for bit."""
 from __future__ import annotations
 
 import numpy as np
-import torch
 
 STRATEGIES = ("backward", "forward", "nearest")
 
@@ -113,42 +112,3 @@ def table_pass(r_by, n_by, forward, carry=None, r_base=0):
         out = np.where(out >= 0, out, np.asarray(carry, np.int64))
     return out
 
-
-def _np(t):
-    return None if t is None else t.numpy()
-
-
-def install():
-    """Give tests/cpu_shim.py asof_merge / asof_backward that take strategy= and tolerance=.  Idempotent; calls without them go
-    to the stand-ins it had, so programs that do not use them run as before.  On the GPU nothing reads them."""
-    import cpu_shim
-    if getattr(cpu_shim.asof_merge, "_strategies", False):
-        return
-    plain_merge, plain_backward = cpu_shim.asof_merge, cpu_shim.asof_backward
-
-    def asof_merge(l_time, l_by, r_time, r_by, n_by, carry_in=None, r_base=0, want_carry=False, *, strategy="backward", tolerance=None,
-                   carry_time=None, carry_fwd=None, carry_fwd_time=None):
-        if strategy == "backward" and tolerance is None:
-            return plain_merge(l_time, l_by, r_time, r_by, n_by, carry_in, r_base, want_carry)
-        if strategy not in STRATEGIES:
-            raise ValueError(strategy)
-        if n_by > cpu_shim.MERGE_MAX_KEYS:
-            return None, None
-        if strategy == "nearest" and want_carry:
-            raise cpu_shim.L.QkError("qk_asof_join: a nearest join has no carry_out")
-        out = merge_join(l_time.numpy(), l_by.numpy(), r_time.numpy(), r_by.numpy(), n_by, strategy, tolerance, _np(carry_in),
-                         _np(carry_time), _np(carry_fwd), _np(carry_fwd_time), r_base)
-        carry = None
-        if want_carry:
-            fwd = strategy == "forward"
-            carry = torch.from_numpy(table_pass(r_by.numpy(), n_by, fwd, _np(carry_fwd if fwd else carry_in), r_base).astype(np.int32))
-        return torch.from_numpy(out.astype(np.int32)), carry
-
-    def asof_backward(l_time, l_by, r_time, r_by, n_by, *, strategy="backward", tolerance=None):
-        if strategy == "backward" and tolerance is None:
-            return plain_backward(l_time, l_by, r_time, r_by, n_by)
-        out = asof_join(l_time.numpy(), l_by.numpy(), r_time.numpy(), r_by.numpy(), strategy, tolerance)
-        return torch.from_numpy(out.astype(np.int32))
-
-    asof_merge._strategies = True
-    cpu_shim.asof_merge, cpu_shim.asof_backward = asof_merge, asof_backward

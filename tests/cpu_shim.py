@@ -4,15 +4,18 @@ GPU.  Every function mirrors the signature of its quokka_b200.ops counterpart an
 numpy oracle; nothing here ships -- the product has no CPU path, and the same tests run against the real
 kernels on the GPU (tests/test_gpu_api.py).  The stand-ins of the feature kernels live in modules of their
 own (tests/<feature>_shim.py), which the GPU tests also compare the kernels against; this module's namespace
-holds them all, so one install serves every program.  tests/test_shim_surface.py checks that it covers ops."""
+holds them all, so one install serves every program.  tests/test_shim_surface.py checks that it covers ops,
+parameter for parameter."""
 from __future__ import annotations
 
 import numpy as np
 import torch
 
+from asof_strategy_shim import STRATEGIES, asof_join, merge_join, table_pass
 from gram_shim import GramState, gram_last_plan
 from knn_shim import knn_merge, knn_topk
 from oracle import relops as R
+from ordered_join_shim import join_place, ordered_pairs
 from pattern_shim import PatternBudgetError, pattern_search
 from quantile_shim import QuantileSketch
 from quokka_b200 import _lib as L
@@ -21,6 +24,7 @@ from quokka_b200 import ops as real_ops
 from quokka_b200.executors import order_image
 from shift_shim import shift_gather, shift_plan
 from sort_shim import sort_last_plan, sort_perm
+from window_events_shim import window_running
 from xchg_shim import XchgChannel
 
 # host-only helpers of ops: they run as they are on CPU tensors
@@ -281,32 +285,53 @@ class JoinTable:
         li, ri = R.join_indices(key.numpy().astype(np.int64), bk, name)
         return _t(li.astype(np.int32)), (None if ri is None else _t(ri.astype(np.int32)))
 
+    def probe_ordered(self, key, how=L.JOIN_INNER, expect=None):
+        bk = np.concatenate(self.keys) if self.keys else np.zeros(0, np.int64)
+        li, ri = ordered_pairs(key.numpy(), bk, how)
+        return _t(li), (None if ri is None else _t(ri))
 
-def asof_backward(l_time, l_by, r_time, r_by, n_by):
-    return _t(R.asof_backward(l_time.numpy(), l_by.numpy(), r_time.numpy(), r_by.numpy()).astype(np.int32))
+    place = staticmethod(join_place)
 
 
-def asof_merge(l_time, l_by, r_time, r_by, n_by, carry_in=None, r_base=0, want_carry=False):
+def _np(t):
+    return None if t is None else t.numpy()
+
+
+def asof_backward(l_time, l_by, r_time, r_by, n_by, *, strategy="backward", tolerance=None):
+    lt, lb, rt, rb = l_time.numpy(), l_by.numpy(), r_time.numpy(), r_by.numpy()
+    if strategy == "backward" and tolerance is None:
+        return _t(R.asof_backward(lt, lb, rt, rb).astype(np.int32))
+    return _t(asof_join(lt, lb, rt, rb, strategy, tolerance).astype(np.int32))
+
+
+def asof_merge(l_time, l_by, r_time, r_by, n_by, carry_in=None, r_base=0, want_carry=False, *, strategy="backward", tolerance=None,
+               carry_time=None, carry_fwd=None, carry_fwd_time=None):
+    if strategy not in STRATEGIES:
+        raise ValueError(strategy)
     if n_by > MERGE_MAX_KEYS:
         return None, None
+    if strategy == "nearest" and want_carry:
+        raise L.QkError("qk_asof_join: a nearest join has no carry_out")
+    lt, rt = l_time.numpy(), r_time.numpy()
     lb, rb = l_by.numpy().astype(np.int64), r_by.numpy().astype(np.int64)
-    idx = R.asof_backward(l_time.numpy(), lb, r_time.numpy(), rb).astype(np.int64)
-    cin = carry_in.numpy().astype(np.int64) if carry_in is not None else np.full(n_by, -1, np.int64)
-    ok = (lb >= 0) & (lb < n_by)
-    fallback = np.where(ok, cin[np.clip(lb, 0, n_by - 1)], -1)
-    out = np.where(idx >= 0, idx + r_base, fallback)
+    if strategy == "backward" and tolerance is None:
+        idx = R.asof_backward(lt, lb, rt, rb).astype(np.int64)
+        cin = carry_in.numpy().astype(np.int64) if carry_in is not None else np.full(n_by, -1, np.int64)
+        fallback = np.where((lb >= 0) & (lb < n_by), cin[np.clip(lb, 0, n_by - 1)], -1)
+        out = np.where(idx >= 0, idx + r_base, fallback)
+    else:
+        out = merge_join(lt, lb, rt, rb, n_by, strategy, tolerance, _np(carry_in), _np(carry_time), _np(carry_fwd), _np(carry_fwd_time),
+                         r_base)
     carry = None
     if want_carry:
-        carry = cin.copy()
-        good = (rb >= 0) & (rb < n_by)
-        last = np.full(n_by, -1, np.int64)
-        np.maximum.at(last, rb[good], np.nonzero(good)[0])
-        carry = np.where(last >= 0, last + r_base, carry)
-        carry = _t(carry.astype(np.int32))
+        fwd = strategy == "forward"
+        carry = _t(table_pass(rb, n_by, fwd, _np(carry_fwd if fwd else carry_in), r_base).astype(np.int32))
     return _t(out.astype(np.int32)), carry
 
 
-def window_sliding(time, by, seg, n_by, size, vals, aggs):
+def window_sliding(time, by, seg, n_by, size, vals, aggs, *, run=None):
+    if run is not None:
+        return window_running(time, by, seg, n_by, run, size, vals, aggs)
     t, b = time.numpy(), by.numpy()
     names = {L.WIN_SUM: "sum", L.WIN_MIN: "min", L.WIN_MAX: "max", L.WIN_COUNT: "count", L.WIN_AVG: "avg"}
     res = R.sliding_window(t, b, size, {str(i): (names[op], None if op == L.WIN_COUNT else vals[src].numpy()) for i, (op, src) in enumerate(aggs)})

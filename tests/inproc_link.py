@@ -23,7 +23,6 @@ run_cases) that way and checks every channel afterwards."""
 from __future__ import annotations
 
 import collections
-import importlib
 import sys
 import tempfile
 import threading
@@ -416,19 +415,12 @@ def run_program_ranks(world: int, names, device, mailbox_bytes: int) -> collecti
     import ranks
     device = torch.device(device)
     counts, lock = collections.Counter(), threading.Lock()
-    for name in ranks.expand(names):          # case modules install their CPU stand-ins on import: before anything is wrapped
-        head, _, rest = name.partition(":")
-        importlib.import_module(head if rest and head not in ranks._API_PREFIXES else "api_cases")
     with pytest.MonkeyPatch.context() as mp, tempfile.TemporaryDirectory() as files:
         if device.type == "cuda":
             from quokka_b200 import ops
         else:
-            import asof_strategy_shim
             import cpu_shim as ops
-            import ordered_join_shim
             ops.install(mp)
-            ordered_join_shim.install()           # the stand-ins of the feature kernels (idempotent; the case modules do it too)
-            asof_strategy_shim.install()
         _count_calls(mp, ops, counts, lock)
         install(mp)
         links = make_links(world, mailbox_bytes, device, ops)

@@ -5,11 +5,8 @@ build side replicated (or one rank) and the build side hash-partitioned across r
 import numpy as np
 import pyarrow as pa
 
-import ordered_join_shim
 from oracle import relops as R
 from quokka_b200.datastream import OrderedStream
-
-ordered_join_shim.install()         # the CPU runs (1 rank, gloo ranks) read the ordered probe from the numpy stand-in
 
 PLANS = ({"broadcast_rows": 1 << 40, "broadcast_cost_based": False}, {"broadcast_rows": 0, "broadcast_cost_based": False})
 

@@ -1,6 +1,6 @@
-"""TEST-ONLY numpy stand-ins for quokka_b200.ops.JoinTable.probe_ordered and JoinTable.place (csrc/join.cu).  install() adds
-them to the JoinTable of tests/cpu_shim.py, so DataStream.join(maintain_sort_order=...) runs through the planner, the executors
-and the gloo exchange without a GPU.  The GPU tests compare both kernels with these, bit for bit."""
+"""TEST-ONLY numpy statements of quokka_b200.ops.JoinTable.probe_ordered and JoinTable.place (csrc/join.cu).  The JoinTable of
+tests/cpu_shim.py answers with them, so DataStream.join(maintain_sort_order=...) runs through the planner, the executors and the
+gloo exchange without a GPU.  The GPU tests compare both kernels with these, bit for bit."""
 from __future__ import annotations
 
 import numpy as np
@@ -18,13 +18,6 @@ def ordered_pairs(probe_key: np.ndarray, build_key: np.ndarray, how: int):
     return li.astype(np.int32), (None if ri is None else ri.astype(np.int32))
 
 
-def probe_ordered(table, key, how=L.JOIN_INNER, expect=None):
-    """JoinTable.probe_ordered of the shim's JoinTable (its build keys in build-row order)."""
-    bk = np.concatenate(table.keys) if table.keys else np.zeros(0, np.int64)
-    li, ri = ordered_pairs(key.numpy(), bk, how)
-    return torch.from_numpy(li), (None if ri is None else torch.from_numpy(ri))
-
-
 def join_place(pos, nleft):
     """Received rows in left order: a stable sort by position (one position's rows are contiguous, so it keeps their order)."""
     p = pos.numpy()
@@ -33,10 +26,3 @@ def join_place(pos, nleft):
     src = np.argsort(p, kind="stable").astype(np.int32)
     return torch.from_numpy(src), torch.from_numpy(p[src].astype(np.int32))
 
-
-def install():
-    """Give the CPU stand-in's JoinTable the ordered probe and the placement.  Idempotent; it only adds methods, so programs
-    that do not use them run as before, and on the GPU (where quokka_b200.ops is the real module) nothing reads them."""
-    import cpu_shim
-    cpu_shim.JoinTable.probe_ordered = probe_ordered
-    cpu_shim.JoinTable.place = staticmethod(join_place)

@@ -8,7 +8,6 @@ import sys
 import pytest
 import torch
 
-import asof_strategy_shim
 import cpu_shim
 import test_bench_flow as TBF
 
@@ -17,7 +16,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_bench_asof_strategy_on_the_shim(monkeypatch):
     TBF.install(monkeypatch)
-    asof_strategy_shim.install()
     bj = TBF.load_tool("bench_asof_strategy")
     monkeypatch.setattr(bj, "ops", cpu_shim)
     monkeypatch.setattr(bj, "event_ms", TBF.cpu_ms)

@@ -9,7 +9,6 @@ import pytest
 import torch
 
 import cpu_shim
-import ordered_join_shim
 import test_bench_flow as TBF
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -23,7 +22,6 @@ def test_byte_model():
 
 def test_bench_ordered_join_on_the_shim(monkeypatch):
     TBF.install(monkeypatch)
-    ordered_join_shim.install()
     bj = TBF.load_tool("bench_ordered_join")
     monkeypatch.setattr(bj, "ops", cpu_shim)
     monkeypatch.setattr(bj, "event_ms", TBF.cpu_ms)

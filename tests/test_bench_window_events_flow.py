@@ -13,8 +13,6 @@ import cpu_shim
 import test_bench_flow as TBF
 import window_events_shim as S
 
-S.install()         # cpu_shim.window_sliding with run=, which the K and T legs call
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 

@@ -53,7 +53,7 @@ def test_session_gap_does_not_overflow():
 
 
 def test_shim_matches_the_row_loop():
-    """cpu_shim.window_sliding(run=...), as window_events_shim.install() leaves it, against the row loop."""
+    """cpu_shim.window_sliding(run=...) against the row loop."""
     import torch
     from quokka_b200 import _lib as L
     for seed in range(30):

@@ -9,8 +9,6 @@ import pyarrow as pa
 
 import window_events_shim as S
 
-S.install()         # the CPU runs (1 rank, gloo ranks) read the per-event windows from the numpy stand-in
-
 RTOL = 1e-9
 U = 2.0 ** -53
 AGGD = {"avg_bid": "AVG(bid)", "max_spread": "MAX(ask - bid)", "n": "count(*)", "sum_ask": "SUM(ask)", "min_bid": "MIN(bid)"}

@@ -1,5 +1,5 @@
 """Per-event (OnEventTrigger) tumbling and session windows in numpy: the references the kernel (csrc/window.cu qk_window_running)
-is tested against, and the CPU stand-in of ops.window_sliding(..., run=...) that install() gives tests/cpu_shim.py.
+is tested against, and the stand-in that window_sliding(..., run=...) of tests/cpu_shim.py calls.
 
 The rows of a key, in time order, are cut into runs -- tumbling: one run per floor(t / size); session: a new run at the key's
 first row and after every gap t - t_prev > timeout -- and every row aggregates the rows of its run with time <= its own
@@ -94,18 +94,3 @@ def window_running(time, by, seg, n_by, kind, param, vals, aggs):
         outs.append(torch.from_numpy(r))
     return outs
 
-
-def install():
-    """Give tests/cpu_shim.py a window_sliding that takes run=.  Idempotent; calls without it go to the stand-in it had, so
-    programs that do not use per-event windows run as before.  On the GPU nothing reads it."""
-    import cpu_shim
-    if getattr(cpu_shim.window_sliding, "_runs", False):
-        return
-    plain = cpu_shim.window_sliding
-
-    def window_sliding(time, by, seg, n_by, size, vals, aggs, *, run=None):
-        if run is None:
-            return plain(time, by, seg, n_by, size, vals, aggs)
-        return window_running(time, by, seg, n_by, run, size, vals, aggs)
-    window_sliding._runs = True
-    cpu_shim.window_sliding = window_sliding
