@@ -204,6 +204,12 @@ def _float_key(t: torch.Tensor) -> torch.Tensor:
     return (t + 0.0).view(torch.int64) if t.dtype == torch.float64 else t
 
 
+def _null_rows(template: DeviceTable, n: int, device) -> DeviceTable:
+    """n NULL rows typed like the one-row table `template`: what a left join puts where a probe row has no build row."""
+    none = torch.full((n,), -1, dtype=torch.int32, device=device)
+    return template.gather(none).with_validity(torch.zeros(n, dtype=torch.uint8, device=device))
+
+
 class _HashedBuild:
     """The build side of a hash join, hashed once on its key column `on`, and the probe against it: what the shuffled and
     the broadcast join share."""
@@ -292,9 +298,7 @@ class BuildProbeJoinExecutor(Executor):
 
     def _unmatched(self, batch: DeviceTable) -> DeviceTable:
         """A left join's probe rows with NULL build columns (typed like the template row)."""
-        dev = batch[self.left_on].data.device
-        none = torch.full((len(batch),), -1, dtype=torch.int32, device=dev)
-        right = self._template.drop([self.right_on]).gather(none).with_validity(torch.zeros(len(batch), dtype=torch.uint8, device=dev))
+        right = _null_rows(self._template.drop([self.right_on]), len(batch), batch[self.left_on].data.device)
         return _append_right(batch, right.columns, "_right")
 
     def _freeze_build(self):
@@ -347,7 +351,8 @@ class OrderedJoinExecutor(Executor):
         its order (qk_join_place) and gathers its own columns.  Only keys, positions and matched build rows cross ranks.  The
         rank holds its whole probe side in device memory until then.
     As in BuildProbeJoinExecutor, an anti join against an empty build side passes the probe side through and the other
-    joins emit nothing."""
+    joins emit nothing, and a left join's owner without build rows answers with NULL build columns typed like a build row of
+    another rank (`left_template_row` / `set_left_template`, sent by the runtime once the build side is complete)."""
 
     ordered_output = True            # rows stay on their rank, in the probe side's order
     POS = "__qk_pos"
@@ -360,6 +365,15 @@ class OrderedJoinExecutor(Executor):
         self._right = _SourceRanks()
         self._left = []
         self._build, self._frozen = None, False
+        self._template = None        # one build row of any rank, without its key: the NULL columns of a left join
+
+    def left_template_row(self):
+        """One build row of this rank without its key column (None: it has none)."""
+        b = next((b for r in sorted(self._right.parts) for b in self._right.parts[r] if len(b)), None)
+        return b.slice(0, 1).drop([self.build_on]) if b is not None else None
+
+    def set_left_template(self, row):
+        self._template = row
 
     def explain(self) -> str:
         return (f"ordered {self.how} join {self.probe_on} = {self.build_on}, keeps the {'left' if self.probe_is_left else 'right'} "
@@ -421,14 +435,7 @@ class OrderedJoinExecutor(Executor):
         if n:
             keys = DeviceTable({self.probe_on: P[self.probe_on], self.POS: DeviceColumn(torch.arange(n, dtype=torch.int32, device=dev))})
             parts = apply_partitioner(HashPartitioner(self.probe_on), keys, me, w)
-        got = sorted(ex(parts, w, edge_key=("ordered-join-keys", id(self))), key=lambda g: g.src_rank)
-        # a left join's unmatched rows need the build columns' types where a rank owns no build rows: one row from any rank
-        # that has some (none anywhere: the build side is empty, and a left join emits nothing, as the unordered join does)
-        template = None
-        if self.how == "left":
-            one = self._build.rows(torch.zeros(1, dtype=torch.int32, device=dev), "inner") if self._build is not None else None
-            samples = ex({r: one for r in range(w)} if one is not None else {}, w, edge_key=("ordered-join-template", id(self)))
-            template = samples[0] if samples else None
+        got = ex(parts, w, edge_key=("ordered-join-keys", id(self)))
         # 2. the owner probes the received keys in source-rank order and answers each source with (position, build columns)
         replies = {}
         if got:
@@ -441,15 +448,15 @@ class OrderedJoinExecutor(Executor):
                     reply = _append_right(reply, self._payload(bi).columns, "")
             elif self.how == "anti":
                 pi, reply = torch.arange(len(K), dtype=torch.int32, device=dev), K.select([self.POS])
-            elif self.how == "left" and template is not None:
+            elif self.how == "left" and self._template is not None:
+                # no build rows here, some on another rank (none anywhere: a left join emits nothing, as the unordered one)
                 pi = torch.arange(len(K), dtype=torch.int32, device=dev)
-                none = torch.full((len(K),), -1, dtype=torch.int32, device=dev)
-                reply = _append_right(K.select([self.POS]), template.gather(none).with_validity(torch.zeros(len(K), dtype=torch.uint8, device=dev)).columns, "")
+                reply = _append_right(K.select([self.POS]), _null_rows(self._template, len(K), dev).columns, "")
             if reply is not None and len(reply):
                 starts = torch.tensor([0] + [len(g) for g in got], device=dev).cumsum(0)
                 cut = torch.searchsorted(pi.to(torch.int64), starts).tolist()     # the reply is in source order
                 replies = {g.src_rank: reply.slice(cut[i], cut[i + 1]) for i, g in enumerate(got) if cut[i + 1] > cut[i]}
-        back = sorted(ex(replies, w, edge_key=("ordered-join-rows", id(self))), key=lambda g: g.src_rank)
+        back = ex(replies, w, edge_key=("ordered-join-rows", id(self)))
         # 3. the source puts what came back into its order and gathers its own columns
         if not n or not back:
             return None
@@ -790,7 +797,7 @@ class SortExecutor(Executor):
         if w == 1:
             self.state = self._sorted(t)[0] if t is not None else None
             return self.state
-        me, dev, first = RT.rank(), default_device(), self.columns[0]
+        dev, first = default_device(), self.columns[0]
         ex = RT.Exchange(dev)
         if t is not None and t[first].dictionary is not None:
             # string first column: the ranks compare images, so they need one dictionary -- every rank's entries to everybody
@@ -798,9 +805,8 @@ class SortExecutor(Executor):
             entries = DeviceTable({first: DeviceColumn(torch.arange(len(d), device=dev).to(t[first].data.dtype), d)})
         else:
             entries = None
-        has_dict = max(r[0] for r in ex.allgather_words([int(entries is not None)]))
-        if has_dict:
-            got = ex({r: entries for r in range(w)} if entries is not None else {}, w, edge_key=("sort-dictionary", id(self)))
+        if ex.max_over_ranks([int(entries is not None)])[0]:
+            got = ex.to_ranks(entries, ("sort-dictionary", id(self)))
             if entries is not None:
                 union = DeviceColumn(torch.empty(0, dtype=t[first].data.dtype, device=dev), got[0][first].dictionary)
                 t = t.with_column(first, unify_dictionaries([t[first], union])[1][0])
@@ -813,29 +819,24 @@ class SortExecutor(Executor):
             fv = run[first].valid
             null = (fv[at] == 0).to(torch.uint8) if fv is not None else torch.zeros(len(at), dtype=torch.uint8, device=dev)
             samples = DeviceTable({"image": DeviceColumn(image[at] ^ _SIGN_I64), "null": DeviceColumn(null)})
-        got = ex({r: samples for r in range(w)} if samples is not None else {}, w, edge_key=("sort-samples", id(self)))
+        got = ex.to_ranks(samples, ("sort-samples", id(self)))
         if not got:
             return None
-        allsamp = concat_tables(sorted(got, key=lambda g: g.src_rank))
+        allsamp = concat_tables(got)
         order = ops.sort_perm(allsamp["image"].data.contiguous(), (1 - allsamp["null"].data).contiguous(), False)
         cut = order[(torch.arange(1, w, device=dev) * len(order)) // w].long()
         split_img, split_null = allsamp["image"].data[cut], allsamp["null"].data[cut].tolist()
         # ---- my run's slice for every rank: rows whose image is below splitter r stay left of it; NULLs are past every value
-        parts, own = {}, None
+        bounds = None
         if run is not None:
             fv = run[first].valid
             nvalid = len(run) if fv is None else int(fv.sum().item())      # NULLS LAST: the run's valid rows come first
             pos = torch.searchsorted(image[:nvalid] ^ _SIGN_I64, split_img).tolist()
             bounds = [0] + [nvalid if isnull else p for p, isnull in zip(pos, split_null)] + [len(run)]
-            parts = {r: run.slice(bounds[r], bounds[r + 1]) for r in range(w) if r != me and bounds[r + 1] > bounds[r]}
-            own = run.slice(bounds[me], bounds[me + 1])
-        mine = list(ex(parts, w, edge_key=("sort-rows", id(self))))
-        if own is not None and len(own) > 0:
-            own.src_rank = me
-            mine.append(own)
+        mine = ex.hand_off(run, bounds, ("sort-rows", id(self)))
         if not mine:
             return None
-        self.state = self._sorted(concat_tables(sorted(mine, key=lambda g: g.src_rank)))[0]
+        self.state = self._sorted(concat_tables(mine))[0]
         return self.state
 
 
@@ -1470,11 +1471,9 @@ class SortedAsofExecutor(Executor):
                 oldest = quotes.gather(self._end_rows(quotes[qt].data, codes, n_by, forward=True))
         earlier, later = [], []
         if self.strategy != "forward":
-            got = ex({r: newest for r in range(w)} if newest is not None and len(newest) > 0 else {}, w, edge_key=("asof-newest", id(self)))
-            earlier = [g for g in sorted(got, key=lambda g: g.src_rank) if g.src_rank < me]
+            earlier = [g for g in ex.to_ranks(newest, ("asof-newest", id(self))) if g.src_rank < me]
         if self.strategy != "backward":
-            got = ex({r: oldest for r in range(w)} if oldest is not None and len(oldest) > 0 else {}, w, edge_key=("asof-oldest", id(self)))
-            later = [g for g in sorted(got, key=lambda g: g.src_rank) if g.src_rank > me]
+            later = [g for g in ex.to_ranks(oldest, ("asof-oldest", id(self))) if g.src_rank > me]
         # ---- trades to the rank whose quote range holds them: the k-th rank that has quotes takes the trades from its first quote
         #      time up to the next such rank's (the first one also takes everything earlier: those trades match nothing, but
         #      only a rank with quotes knows the columns to fill with NULLs); ranks without quotes take none.  Forward: the k-th
@@ -1485,7 +1484,7 @@ class SortedAsofExecutor(Executor):
             if any(rows[r][0] for r in range(w)):
                 raise L.QkError("as-of join: no quotes were received")
             return None
-        parts, own = {}, None
+        bounds = None
         if trades is not None and len(trades) > 0:
             fwd = self.strategy == "forward"
             cuts = [rows[o][6] for o in owners[:-1]] if fwd else [rows[o][5] for o in owners[1:]]
@@ -1494,13 +1493,7 @@ class SortedAsofExecutor(Executor):
             bounds = [0]
             for r in range(w):
                 bounds.append(ends[r] if r in ends else bounds[-1])
-            parts = {r: trades.slice(bounds[r], bounds[r + 1]) for r in range(w) if r != me and bounds[r + 1] > bounds[r]}
-            own = trades.slice(bounds[me], bounds[me + 1])           # the bulk: stays where it is
-        mine = ex(parts, w, edge_key=("asof-trades", id(self)))
-        if own is not None and len(own) > 0:
-            own.src_rank = me
-            mine = list(mine) + [own]
-        mine = sorted(mine, key=lambda g: g.src_rank)
+        mine = ex.hand_off(trades, bounds, ("asof-trades", id(self)))      # the own slice, the bulk, stays where it is
         self.trade_state = self.quote_state = None
         self._carry, self._swept, self._whole_state = None, 0, False
         all_q = earlier + ([quotes] if quotes is not None and len(quotes) > 0 else []) + later
@@ -1996,16 +1989,17 @@ class ShiftExecutor(Executor):
     """OrderedStream.shift (pyquokka/orderedstream.py:13-35; the reference never defines its ShiftOperator, so the semantics are
     Polars' pl.all().shift(n, fill_value).over(by)): every row receives the values of `columns` from the row n places earlier
     (n > 0) or |n| later (n < 0) among the rows of its `by` key in stream order -- rank order, then arrival order -- or the fill.
-    Rows stay where they are; answered in done().
-      * one rank: KeyCodes codes, the stable code partition, qk_shift_plan (source rows and the order check in one pass) and
-        qk_shift_gather (every shifted column in one launch).  Unshifted columns are passed on as they are.
-      * several ranks: each rank holds a contiguous piece of the stream (sort(), sorted readers, from_device(sorted_by=...), or a
-        hash edge on `by`), so nothing is shuffled.  A rank flags the last n rows of each of its keys (first |n| for a lead)
-        and sends them to every later (earlier) rank -- at most |n| x keys rows; it then plans over the key codes of
-        [earlier ranks' tails in rank order | own rows] (lead: [own rows | later ranks' heads]) and gathers the payload from
-        its shard and from that small boundary table.  A key with fewer than |n| rows on the neighbouring rank still finds its
-        rows, because the tails of ALL earlier ranks arrive.  String payload columns of the boundary table are re-coded onto
-        the shard's dictionary (new entries appended); the shard is not re-coded.
+    Rows stay where they are; answered in done(), by one path at every world size:
+      * each rank holds a contiguous piece of the stream (sort(), sorted readers, from_device(sorted_by=...), or a hash edge on
+        `by`), so nothing is shuffled.  A rank that has later (earlier) ranks flags the last n rows of each of its keys (first
+        |n| for a lead; qk_shift_plan with want_edge) and sends them to every later (earlier) rank -- at most |n| x keys rows;
+      * every rank then plans over the KeyCodes codes of [earlier ranks' tails in rank order | own rows] (lead: [own rows |
+        later ranks' heads]) -- the stable code partition and qk_shift_plan (source rows and the order check in one pass) --
+        and gathers the payload from its shard and from that small boundary table (qk_shift_gather, every shifted column in
+        one launch); unshifted columns are passed on as they are.  At one rank there is no boundary table.
+    A key with fewer than |n| rows on the neighbouring rank still finds its rows, because the tails of ALL earlier ranks
+    arrive.  String payload columns of the boundary table are re-coded onto the shard's dictionary (new entries appended);
+    the shard is not re-coded.
     When `time_col` (the stream's sorted_by) is an integer, date or timestamp column, rows of a key whose time falls below the
     previous row's raise QkError, across rank boundaries too (NULL times count as the largest, where sort() puts them)."""
 
@@ -2048,10 +2042,6 @@ class ShiftExecutor(Executor):
             raise L.QkError(f"shift: `by` column {self.by!r} must be a string column or integer codes")
         return self._codes.codes(col)
 
-    def _require_order(self, bad):
-        if bad:
-            raise L.QkError(f"shift: the stream is not sorted by {self.time_col}")
-
     def _gather(self, t: DeviceTable, boundary: DeviceTable | None, src: torch.Tensor) -> DeviceTable:
         a, b, av, bv, fills, dicts = [], [], [], [], [], []
         for c in self.columns:
@@ -2087,83 +2077,57 @@ class ShiftExecutor(Executor):
             cols[c if self.suffix is None else c + self.suffix] = DeviceColumn(o, dic, t[c].arrow_type, v)
         return DeviceTable(cols)
 
-    def done(self, executor_id):
-        t, self._batches = (concat_tables(self._batches) if self._batches else None), []
-        if world_size() > 1:
-            self.state = self._across_ranks(t)
-            return self.state
-        if t is None:
-            return None
-        if self.n == 0:
-            self.state = self._unchanged(t)
-            return self.state
-        nrows = len(t)
-        time = self._time(t)
-        if self.by is None:
-            src, _, bad = ops.shift_plan(self.n, nrows, time=time, device=t.device)
-        else:
-            codes = self._key_codes(t)
-            n_by = max(1, self._codes.n_by)
-            dest, seg = ops.partition_plan(codes, n_by, L.PART_CODE)
-            src, _, bad = ops.shift_plan(self.n, nrows, codes, n_by, dest, seg, time=time)
-        self._require_order(bad)
-        self.state = self._gather(t, None, src)
-        return self.state
-
     def _unchanged(self, t: DeviceTable) -> DeviceTable:
         if self.suffix is None:
             return t
         return DeviceTable(dict(t.columns) | {c + self.suffix: t[c] for c in self.columns})
 
-    def _across_ranks(self, t: DeviceTable | None):
+    def _plan(self, n: int, nrows: int, codes: torch.Tensor | None, **kw):
+        """ops.shift_plan over the key codes `codes` (None: the whole stream is one key) and their stable code partition."""
+        if codes is None:
+            return ops.shift_plan(n, nrows, **kw)
+        n_by = max(1, self._codes.n_by)
+        return ops.shift_plan(n, nrows, codes, n_by, *ops.partition_plan(codes, n_by, L.PART_CODE), **kw)
+
+    def done(self, executor_id):
         from . import runtime as RT
-        w, me, dev = RT.world_size(), RT.rank(), default_device()
+        t, self._batches = (concat_tables(self._batches) if self._batches else None), []
         if self.n == 0:
-            return self._unchanged(t) if t is not None else None
+            self.state = self._unchanged(t) if t is not None else None
+            return self.state
+        w, me, dev = RT.world_size(), RT.rank(), default_device()
         ex = RT.Exchange(dev)
         lag = self.n > 0
+        receivers = range(me + 1, w) if lag else range(me)              # the ranks that need this rank's boundary rows
         # a shift past 2^31 rows has no sources; the boundary then only serves the order check: one row per key
         edge_n = self.n if abs(self.n) < self.HUGE else (1 if lag else -1)
         na = len(t) if t is not None else 0
-        parts, codes, time = {}, None, None
+        boundary = codes = time = None
         if na:
             time = self._time(t)
-            if self.by is not None:
-                codes = self._key_codes(t)
-                n_by = max(1, self._codes.n_by)
-                dest, seg = ops.partition_plan(codes, n_by, L.PART_CODE)
-                _, edge, _ = ops.shift_plan(edge_n, na, codes, n_by, dest, seg, lo=0, hi=0, want_edge=True)
-            else:
-                _, edge, _ = ops.shift_plan(edge_n, na, lo=0, hi=0, want_edge=True, device=t.device)
-            need = list(dict.fromkeys(self.columns + ([self.by] if self.by is not None else [])
-                                      + ([self.time_col] if time is not None else [])))
+            codes = self._key_codes(t) if self.by is not None else None
+        if na and len(receivers):
+            _, edge, _ = self._plan(edge_n, na, codes, lo=0, hi=0, want_edge=True, device=t.device)
             rows = torch.nonzero(edge).flatten().to(torch.int32)
             if rows.numel():
+                need = list(dict.fromkeys(self.columns + ([self.by] if self.by is not None else [])
+                                          + ([self.time_col] if time is not None else [])))
                 boundary = t.select(need).gather(rows)
-                parts = {r: boundary for r in range(w) if (r > me if lag else r < me)}
-        got = sorted(ex(parts, w, edge_key=("shift-boundary", id(self))), key=lambda g: g.src_rank)
+        got = ex.to_ranks(boundary, ("shift-boundary", id(self)), ranks=receivers)
         B = concat_tables(got) if got else None
         nb = len(B) if B is not None else 0
         bad = 0
         if na:
             lo = nb if lag else 0
-            allcodes = alltime = None
+            allcodes, alltime = codes, None
             if nb and self.by is not None:
                 bcodes = self._key_codes(B)
                 allcodes = torch.cat([bcodes, codes] if lag else [codes, bcodes])
-            elif self.by is not None:
-                allcodes = codes
             if time is not None:
                 btime = self._time(B) if nb else None
                 alltime = time if btime is None else torch.cat([btime, time] if lag else [time, btime])
-            if self.by is not None:
-                n_by = max(1, self._codes.n_by)
-                dest, seg = ops.partition_plan(allcodes, n_by, L.PART_CODE)
-                src, _, bad = ops.shift_plan(self.n, na + nb, allcodes, n_by, dest, seg, lo=lo, hi=lo + na, time=alltime)
-            else:
-                src, _, bad = ops.shift_plan(self.n, na + nb, lo=lo, hi=lo + na, time=alltime, device=t.device)
-        if any(r[0] for r in ex.allgather_words([int(bad or 0)])):          # every rank raises, or none does
-            self._require_order(1)
-        if not na:
-            return None
-        return self._gather(t, B if nb else None, src)
+            src, _, bad = self._plan(self.n, na + nb, allcodes, lo=lo, hi=lo + na, time=alltime, device=t.device)
+        if ex.max_over_ranks([int(bad or 0)])[0]:          # every rank raises, or none does
+            raise L.QkError(f"shift: the stream is not sorted by {self.time_col}")
+        self.state = self._gather(t, B if nb else None, src) if na else None
+        return self.state

@@ -323,10 +323,16 @@ class Exchange:
         dist.all_gather_into_tensor(out, t)
         return out.cpu().view(w, len(words)).tolist()
 
+    def max_over_ranks(self, words: list) -> list:
+        """The element-wise maximum of `words` over all ranks (one allgather_words)."""
+        return [max(col) for col in zip(*self.allgather_words(words))]
+
     def __call__(self, parts, n_target: int, single_owner: int | None = None, edge_key=None) -> list:
         """parts: {target_channel: DeviceTable} or edge.Parts.  Target channel c lives on rank c (or on
         `single_owner` when the consumer has a single channel).  Returns the tables received by this rank,
-        one per source rank that sent rows."""
+        one per source rank that sent rows, in source-rank order (`src_rank` on each, at more than one rank) on both
+        transports -- a payload that goes in rounds too, a source's rounds one after the other.  Callers rely on that order
+        and do not sort."""
         if world_size() == 1:
             if isinstance(parts, Parts):
                 return parts.tables()
@@ -335,6 +341,33 @@ class Exchange:
         if link is not None:
             return self._native_call(link, parts, single_owner, edge_key)
         return self._collective_call(parts, single_owner, edge_key)
+
+    def to_ranks(self, table, edge_key, ranks=None) -> list:
+        """`table` (None or empty: nothing) to every rank in `ranks` (default: all of them, this one included).  Returns the
+        tables this rank received in source-rank order, each with its `src_rank`, at one rank too."""
+        w = world_size()
+        send = table is not None and len(table) > 0
+        got = self({r: table for r in (range(w) if ranks is None else ranks)} if send else {}, w, edge_key=edge_key)
+        if w == 1:                           # the table itself came back: the caller gets a view that names its source
+            got = [DeviceTable(g.columns) for g in got]
+            for g in got:
+                g.src_rank = 0
+        return got
+
+    def hand_off(self, table, bounds, edge_key) -> list:
+        """Rows [bounds[r], bounds[r + 1]) of `table` (None or empty: nothing) to rank r.  This rank's own slice stays where
+        it is, without a trip through the mailbox.  Returns the own and received slices in source-rank order, each with its
+        `src_rank`."""
+        w, me = world_size(), rank()
+        parts, own = {}, None
+        if table is not None and len(table) > 0:
+            parts = {r: table.slice(bounds[r], bounds[r + 1]) for r in range(w) if r != me and bounds[r + 1] > bounds[r]}
+            own = table.slice(bounds[me], bounds[me + 1])
+        got = self(parts, w, edge_key=edge_key)
+        if own is None or len(own) == 0:
+            return got
+        own.src_rank = me
+        return [g for g in got if g.src_rank < me] + [own] + [g for g in got if g.src_rank > me]
 
     # ------------------------------------------------------------------ what both transports do with the meta rows
     def _count_received(self, edge_key, counts):
@@ -681,8 +714,7 @@ class TaskGraph:
                     # (string keys: codes of unrelated dictionaries; fp64 keys are matched on their bit pattern, not filtered)
                     no_filter = 1 if (sch is not None and any(name == right and (dic is not None or "float" in dt) for name, dt, dic, _, _ in sch)) else 0
                 else:
-                    rows = self.exchange.allgather_words([n_local, no_filter])
-                    n_local, no_filter = max(r[0] for r in rows), max(r[1] for r in rows)
+                    n_local, no_filter = self.exchange.max_over_ranks([n_local, no_filter])
             if no_filter:
                 continue
             words = ops.Bloom.words_for(-(-n_local // w) if replicated else n_local)
@@ -691,8 +723,7 @@ class TaskGraph:
             if w > 1 and not replicated:            # a replicated build side yields the complete filter on every rank
                 mine = bits[me * words:(me + 1) * words].contiguous()
                 if native_link(self.device) is not None:     # my slice to every rank over the peer-memory link
-                    t = DeviceTable({"bits": DeviceColumn(mine)})
-                    got = self.exchange({r: t for r in range(w)}, w, edge_key=("bloom", tgt_id))
+                    got = self.exchange.to_ranks(DeviceTable({"bits": DeviceColumn(mine)}), ("bloom", tgt_id))
                     bits = torch.cat([g["bits"].data for g in got]) if len(got) > 1 else got[0]["bits"].data
                 else:
                     allbits = torch.empty(w * words, dtype=bits.dtype, device=self.device)
@@ -713,8 +744,7 @@ class TaskGraph:
             if (w == 1 or stream_id != 1 or tgt.single or isinstance(edge.partitioner, BroadcastPartitioner)
                     or getattr(tgt.instance, "how", None) != "left" or not hasattr(tgt.instance, "set_left_template")):
                 continue
-            row = tgt.instance.left_template_row()
-            got = self.exchange({r: row for r in range(w)} if row is not None else {}, w, edge_key=("left-template", tgt_id))
+            got = self.exchange.to_ranks(tgt.instance.left_template_row(), ("left-template", tgt_id))
             tgt.instance.set_left_template(got[0] if got else None)
 
     def _finish(self, actor: _Actor):
@@ -753,7 +783,7 @@ class TaskGraph:
                 if fixed is not None:
                     rounds = fixed                              # the same on every rank by construction: no agreement round
                 elif w > 1:
-                    rounds = max(r[0] for r in self.exchange.allgather_words([rounds]))
+                    rounds = self.exchange.max_over_ranks([rounds])[0]
                 if not self._run_laned(a, mine, rounds):
                     for i in range(rounds):
                         batch = a.obj.execute(me, mine[i])[1] if i < len(mine) else None
@@ -840,11 +870,4 @@ def _is_silent(instance, stream_id) -> bool:
 def gather_to_all(tables: list, device) -> list:
     """collect(): every rank receives every rank's sink batches (quokka_dataset.py:107-117: the result is
     the unordered concatenation of all sink batches)."""
-    w = world_size()
-    local = concat_tables(tables) if tables else None
-    if w == 1:
-        return [local] if local is not None and len(local) > 0 else []
-    ex = Exchange(device)
-    # broadcast partitioner semantics: send my batch to every rank
-    parts = {r: local for r in range(w)} if local is not None and len(local) > 0 else {}
-    return ex(parts, w)
+    return Exchange(device).to_ranks(concat_tables(tables) if tables else None, None)
